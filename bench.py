@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- SSB Q4.1 (scan -> 4-way hash join -> group-by) rows/sec on N B200s, beside the CPU oracle.
+"""bench.py -- SSB Q4.1 (scan -> 4-way hash join -> group-by) rows/sec on N H100s, beside the CPU oracle.
 
 Contract (see DESIGN.md "Measurement"):
   python bench.py --gpus N --steps K --warmup W          (N > 1: launched by torchrun, one rank per GPU)
@@ -11,8 +11,11 @@ rows per GPU, weak scaling) goes through the fused fragment (scan -> probe x4 ->
 group-by states are pulled, and for N > 1 gathered over NCCL and merged by a final GPU aggregate on rank 0.
   value : rows/s with the fact columns already resident in HBM when the timed region starts
   e2e   : the same through the C-ABI with HOST (pinned) column buffers, H2D inside the timed region
-The inputs (14.4 GB of fact columns per GPU) are far larger than the 126 MB L2, so no L2 flush is needed
+The inputs (14.4 GB of fact columns per GPU) are far larger than the 50 MB L2, so no L2 flush is needed
 between timed iterations (config.l2: "inputs >> L2").
+
+--dump-outputs DIR writes what the last timed step returned (q41: the result groups; groupby: a fixed, seeded sample of
+the groups; q3 / q95: the query's summary numbers) as DIR/<name>.npy.  The inputs are generated from fixed seeds, so two builds can be compared output for output.
 """
 import argparse
 import json
@@ -37,20 +40,20 @@ def parse_args():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="gpu", choices=["gpu", "reference"])
     ap.add_argument("--workload", default="q41", choices=["q41", "groupby", "q3", "q95"],
-                    help="q41: SSB SF100 Q4.1 (BASELINE.json's metric; the default).  groupby: BASELINE.json config 5, 1e9 rows / 1e8 "
-                         "distinct int64 keys, SUM + COUNT, on one B200 (N > 1: one independent key range per GPU, no exchange).  "
-                         "q3: BASELINE.json config 3, TPC-H Q3 with the NCCL hash shuffle (tools/q3_distributed.py; --sf = TPC-H scale).  "
+                    help="q41: SSB SF100 Q4.1 (BASELINE.json's metric; the default).  groupby: BASELINE.json config 5 at half size, 5e8 rows / 5e7 "
+                         "distinct int64 keys, SUM + COUNT, on one H100 (N > 1: one independent key range per GPU, no exchange).  "
+                         "q3: BASELINE.json config 3, TPC-H Q3 with the NCCL hash shuffle (tools/q3_distributed.py; --sf = TPC-H scale, default 300 / 8 per GPU).  "
                          "q95: BASELINE.json config 4, the TPC-DS Q95 shape (tools/q95_distributed.py; --sf = TPC-DS scale, default 1000 / 8 per GPU)")
     ap.add_argument("--scaling", default="weak", choices=["weak", "strong"],
                     help="q41 with N > 1: weak = --sf per GPU (default), strong = --sf split over the N GPUs")
-    ap.add_argument("--groupby-rows", type=int, default=1_000_000_000)
-    ap.add_argument("--groupby-keys", type=int, default=100_000_000)
+    # config 5 is 1e9 rows / 1e8 keys; its partitioned push needs ~82 GB there, so an 80 GB H100 runs it at half size
+    ap.add_argument("--groupby-rows", type=int, default=500_000_000)
+    ap.add_argument("--groupby-keys", type=int, default=50_000_000)
     ap.add_argument("--sf", type=float, default=100.0, help="SSB scale factor per GPU (weak scaling)")
     ap.add_argument("--rows", type=int, default=0, help="override fact rows per GPU")
     ap.add_argument("--e2e-steps", type=int, default=3)
     ap.add_argument("--e2e-morsel-rows", type=int, default=1 << 22,
-                    help="e2e: the host columns are pushed in morsels of this many rows (measured: 4 M-row morsels 170.6 ms per 600 M rows, "
-                         "one 600 M-row batch 197 ms; tools/e2e_batches.py)")
+                    help="e2e: the host columns are pushed in morsels of this many rows (tools/e2e_batches.py compares morsel sizes)")
     ap.add_argument("--no-operator-e2e", action="store_true", help="skip e2e.operator_api (the C++ operator path, starrocks_b200/host/bench)")
     ap.add_argument("--cpu-sample-rows", type=int, default=0, help="rows of the CPU baseline sample (0 = auto)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
@@ -58,11 +61,25 @@ def parse_args():
     ap.add_argument("--merge", choices=["allreduce", "gather"], default="allreduce",
                     help="N>1 merge of the partial aggregates: in-place all-reduce of the dense slot arrays (SURVEY 8e) or "
                          "gather of partial rows to rank 0 + final aggregate (the reference plan's UNPARTITIONED exchange)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step returned as DIR/<name>.npy (float64): q41 the result groups, "
+                         "groupby a seeded sample of the groups, q3 / q95 the query's summary numbers")
     return ap.parse_args()
 
 
+def dump_outputs(out_dir, arrays):
+    """DIR/<name>.npy per array, as float64: the integer results of these workloads stay below 2^53, so the values are
+    exact; a NULL is written as NaN."""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, (data, nulls) in arrays.items():
+        a = np.asarray(data).astype(np.float64)
+        if nulls is not None:
+            a[np.asarray(nulls) != 0] = np.nan
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+
+
 # ---------------------------------------------------------------------------------------------------
-# clocks sampling (B200_PROFILING.md recipe)
+# clocks sampling
 # ---------------------------------------------------------------------------------------------------
 class ClockSampler:
     """SM clock + throttle reasons sampled through NVML from a background thread (about 1 kHz: the timed region of the
@@ -173,8 +190,7 @@ def gen_lineorder_host(n, sz, seed):
 
 def host_cores():
     """threads the CPU arm can really run at once: the scheduler affinity, capped by the cgroup CPU quota (a 1-GPU lease may
-    see all 128 cores in its affinity mask and still be throttled to a fraction of them: the same CPU arm ran 0.65 and
-    3.5 G rows/s on two `128-core` boxes in round 1).  -> (threads to use, {"affinity": .., "cgroup_quota_cpus": ..})"""
+    see all of a host's cores in its affinity mask and still be throttled to a fraction of them).  -> (threads to use, {"affinity": .., "cgroup_quota_cpus": ..})"""
     try:
         aff = len(os.sched_getaffinity(0))
     except Exception:
@@ -201,7 +217,7 @@ def measured_peak():
         m = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         return float(m["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return 3350.0, "fallback (H100 SXM data sheet: 3.35 TB/s HBM3)"
 
 
 def known_traffic():
@@ -575,7 +591,7 @@ def run_gpu(args):
             "config": {"workload": f"SSB SF{sf:g} Q4.1 4-way hash join + group-by (scan->probe x4->aggregate), fused fragment",
                        "fact_rows_per_gpu": n, "global_fact_rows": n * world, "dims": {k: int(v) for k, v in sz.items() if k != "lineorder"},
                        "parallelism": f"dp{world}: fact sharded, dimensions replicated (broadcast join), partial aggregates gathered over NCCL",
-                       "l2": "inputs (14.4 GB/GPU) >> 126 MB L2, no flush needed", "late_materialization": True,
+                       "l2": "inputs (14.4 GB/GPU) >> 50 MB L2, no flush needed", "late_materialization": True,
                        "fragment_plan": plan,
                        "rows_reaching_aggregate_per_gpu": int(rows_passed), "build_ms": build_ms},
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
@@ -590,6 +606,15 @@ def run_gpu(args):
             "cpu_baseline": cpu, "e2e": e2e, "gpu_launches": int(launches), "clocks": clocks, "parity": parity,
         }
         print(json.dumps(line))
+        if args.dump_outputs:
+            # the groups of the last timed step in (d_year, c_nation) order, and how many fact rows reached the aggregate
+            names = {ssb.D_YEAR: "d_year", ssb.C_NATION: "c_nation", ssb.OUT_SUM_REVENUE: "sum_lo_revenue",
+                     ssb.OUT_SUM_SUPPLYCOST: "sum_lo_supplycost"}
+            by_slot = {slot: (data, nulls) for slot, _, data, nulls in result}
+            order = np.lexsort([by_slot[ssb.C_NATION][0], by_slot[ssb.D_YEAR][0]])
+            arrays = {names[slot]: (data[order], None if nulls is None else nulls[order]) for slot, (data, nulls) in by_slot.items()}
+            arrays["rows_reaching_aggregate"] = (np.array([rows_passed]), None)
+            dump_outputs(args.dump_outputs, arrays)
     frag.close()
     if world > 1:
         dist.destroy_process_group()
@@ -615,7 +640,7 @@ def step_tail(frag, final, ctx, gpu, abi, ssb, torch, dist, dev, world, rank, MA
 
 
 # ---------------------------------------------------------------------------------------------------
-# workload "groupby": BASELINE.json config 5 -- 1e9 rows, 1e8 distinct int64 keys, SUM + COUNT on one B200
+# workload "groupby": BASELINE.json config 5 at half size -- 5e8 rows, 5e7 distinct int64 keys, SUM + COUNT on one H100
 # ---------------------------------------------------------------------------------------------------
 GROUPBY_BYTES_PER_ROW = 16   # SURVEY.md 8d: key + value in; + 24 B per group out
 
@@ -773,6 +798,16 @@ def run_gpu_groupby(args):
     del present, gk, gs, gc
     if not all(checks.values()):
         raise SystemExit(f"bench.py: group-by invariants violated: {checks}")
+    if args.dump_outputs and rank == 0:
+        # 1 M groups of the last timed step (~24 MB): seeded positions in key order, so equal results give equal samples
+        srt = torch.argsort(device_view(out.cols[0].data, groups, 8, dev))
+        pick = np.sort(np.random.default_rng(7).choice(groups, size=min(groups, 1 << 20), replace=False))
+        idx = srt[torch.from_numpy(pick).to(dev)]
+        dump_outputs(args.dump_outputs, {
+            nm: (device_view(out.cols[c].data, groups, 8, dev)[idx].cpu().numpy(), None)
+            for c, nm in enumerate(("key", "sum_value", "count"))})
+        dump_outputs(args.dump_outputs, {"groups": (np.array([groups]), None)})
+        del srt, idx
 
     # ---- e2e: host (pinned) key / value columns through sr_agg_push, result pulled to host memory ----
     e2e = None
@@ -846,7 +881,7 @@ def run_gpu_groupby(args):
             "scaling": "weak", "vs_baseline": None, "dtype": "int64", "data": "synthetic",
             "config": {"workload": f"group-by {n} rows, {nk} distinct int64 keys, SUM + COUNT", "rows_per_gpu": n, "distinct_keys_per_gpu": nk,
                        "groups_per_gpu": groups, "parallelism": f"dp{world}: one key range per GPU (rows already hash-exchanged), no collective",
-                       "l2": "inputs (16 GB/GPU) >> 126 MB L2, no flush needed"},
+                       "l2": f"inputs ({n * 16 / 1e9:g} GB/GPU) >> 50 MB L2, no flush needed"},
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": traffic,
                          "kernel": "sr_agg_push (k_aggp_scatter x 2 + k_aggp_apply) + result materialisation (k_agg_count / k_agg_emit)",
                          "kernel_ms": ms_per_step, "push_ms": push_ms, "algorithmic_bytes_per_launch": abytes, "peak_source": peak_src,
@@ -862,6 +897,9 @@ def run_gpu_groupby(args):
 
 if __name__ == "__main__":
     a = parse_args()
+    if a.dump_outputs and a.impl == "reference":
+        raise SystemExit("bench.py: --dump-outputs writes what the GPU arm computed; the reference arm has no timed GPU path")
+    dump = ["--dump-outputs", a.dump_outputs] if a.dump_outputs else []
     if a.workload == "q3":
         if a.impl == "reference":
             if int(os.environ.get("RANK", "0")) == 0:
@@ -869,7 +907,8 @@ if __name__ == "__main__":
         else:
             sys.path.insert(0, os.path.join(ROOT, "tools"))
             import q3_distributed
-            q3_distributed.main(q3_distributed.parse(["--sf", str(a.sf if a.sf != 100.0 else 300.0), "--steps", str(a.steps), "--warmup", str(a.warmup)]))
+            world = int(os.environ.get("WORLD_SIZE", "1"))
+            q3_distributed.main(q3_distributed.parse(["--sf", str(a.sf if a.sf != 100.0 else 37.5 * world), "--steps", str(a.steps), "--warmup", str(a.warmup)] + dump))
     elif a.workload == "q95":
         if a.impl == "reference":
             if int(os.environ.get("RANK", "0")) == 0:
@@ -878,7 +917,7 @@ if __name__ == "__main__":
             sys.path.insert(0, os.path.join(ROOT, "tools"))
             import q95_distributed
             world = int(os.environ.get("WORLD_SIZE", "1"))
-            q95_distributed.main(q95_distributed.parse(["--sf", str(a.sf if a.sf != 100.0 else 125.0 * world), "--steps", str(a.steps), "--warmup", str(a.warmup)]))
+            q95_distributed.main(q95_distributed.parse(["--sf", str(a.sf if a.sf != 100.0 else 125.0 * world), "--steps", str(a.steps), "--warmup", str(a.warmup)] + dump))
     elif a.workload == "groupby":
         run_reference_groupby(a) if a.impl == "reference" else run_gpu_groupby(a)
     elif a.impl == "reference":

@@ -1,5 +1,5 @@
 /*
- * sr_gpu_ops.h -- C-ABI of the B200-native StarRocks BE hot path
+ * sr_gpu_ops.h -- C-ABI of the H100-native StarRocks BE hot path
  * (columnar Chunk scan -> predicate/filter -> hash-join build+probe -> hash aggregate,
  *  plus the hash-partition step of ExchangeSink).
  *

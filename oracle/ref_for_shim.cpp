@@ -2,7 +2,7 @@
 // behind FrameOfReferencePageBuilder / FrameOfReferencePageDecoder, be/src/storage/rowset/frame_of_reference_page.h),
 // compiled from the reference tree where it lies together with be/src/base/string/faststring.cc.  oracle/ref_shims/ holds
 // stand-ins for the third-party headers that code pulls in but does not need here (glog, butil, fmt, arrow, boost via
-// bit_stream_utils); no reference source is copied.  Built by `make -C oracle ref` only where /root/reference exists.
+// bit_stream_utils); no reference source is copied.  Built by `make -C oracle ref` only where a reference tree is given.
 // tests/test_oracle_golden.py checks orc_for_encode / orc_for_decode (the restatement) byte for byte against it.
 #include "util/frame_of_reference_coding.h"
 

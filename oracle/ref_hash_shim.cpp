@@ -3,7 +3,7 @@
 //     hashes of column_hash.cpp / exchange_sink_operator.cpp:586-637),
 //   crc_hash_32  (be/src/base/hash/hash.h:96-130: JoinKeyHash<Slice> and the 1/2-byte JoinKeyHash, join_hash_map_helper.h:27,60).
 // be/src/base/hash/hash_util.cpp and be/src/gutil/cpu.cc are compiled along for the out-of-line parts; oracle/ref_shims/ stands
-// in for glog / butil.  Built by `make -C oracle ref` only where /root/reference exists; tests/test_oracle_golden.py checks the
+// in for glog / butil.  Built by `make -C oracle ref` only where a reference tree is given; tests/test_oracle_golden.py checks the
 // restatements (orc_fnv_hash, orc_zlib_crc32, orc_crc_hash_32) against it on random byte strings.
 #include "base/hash/hash.h"
 #include "base/hash/hash_util.hpp"

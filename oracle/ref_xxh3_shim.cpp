@@ -1,6 +1,6 @@
 // oracle/_ref: the REAL reference code for the one piece of the path that compiles from the reference tree on its own --
 // the vendored single-header xxHash (be/src/base/hash/xxhash.h) behind HashUtil::xx_hash3_64
-// (be/src/base/hash/hash_util.cpp:100-102).  Built by `make -C oracle ref` ONLY where /root/reference exists; the header is
+// (be/src/base/hash/hash_util.cpp:100-102).  Built by `make -C oracle ref` ONLY where a reference tree is given; the header is
 // included from where it lies (no reference source is copied into this repository); the output goes to oracle/_ref/.
 // tests/test_oracle_golden.py cross-checks orc_xxh3_64 (the restatement) against it on random inputs.
 #ifndef SR_REFERENCE_XXHASH

@@ -1,5 +1,5 @@
-"""Turn an `ncu --set full` report into the text summary + traffic.json kept under profiles/.
-  python scripts/ncu_summary.py gpurun_out/r1_final.ncu-rep profiles/r1_frag_full_summary.txt profiles/traffic.json
+"""Turn an `ncu --set full` report into a text summary + traffic.json (bench.py reads profiles/traffic.json when it exists).
+  mkdir -p profiles && python scripts/ncu_summary.py report.ncu-rep profiles/frag_full_summary.txt profiles/traffic.json
 """
 import csv
 import json
@@ -36,7 +36,7 @@ def main():
     head, units = rows[0], rows[1]
     idx = {k: i for i, k in enumerate(head)}
     lines = ["# ncu --set full --clock-control none --import-source on, k_frag_* kernels of `python bench.py --steps 2 --warmup 1`",
-             "# (SSB SF100 Q4.1, 600 M rows, 1 x B200); per-launch values; one launch of each kernel = one fragment push over the shard", ""]
+             "# (SSB SF100 Q4.1, 600 M rows, one GPU); per-launch values; one launch of each kernel = one fragment push over the shard", ""]
     traffic = {}
     for r in rows[2:]:
         name = r[idx["Kernel Name"]].split("(")[0].replace("void ", "").replace("srd::", "")

@@ -1,9 +1,9 @@
 // Scratch measurement (not part of the product): cost of sparse 4-byte reads of pinned host memory from a kernel.
 //  (1) as a function of the distance between the words read -> the PCIe read granularity a late-materialising pass
-//      pays per surviving row (measured on B200 / PCIe Gen5: 64-byte blocks, <= ~700 M requests/s, 51.5 GB/s dense);
+//      pays per surviving row (kernel reads of mapped host memory move 64-byte blocks);
 //  (2) the same number of sparse reads spread over 1 or 4 separate columns, independent or chained, grid-stride or
 //      block-contiguous -> how a gather pass should be organised.
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o pcie_stride pcie_stride.cu
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o pcie_stride pcie_stride.cu
 #include <cstdint>
 #include <cstdio>
 #include <cuda_runtime.h>
@@ -81,29 +81,31 @@ int main() {
     }
     for (int c = 0; c < 4; c++)
         for (int64_t i = 0; i < colwords; i++) h[c * colwords + i] = (int)i;
+    int sms = 0;
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
     unsigned long long* out;
     cudaMalloc(&out, 8);
     cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, 32);
     const int strides[] = {1, 8, 16, 32, 64, 256};
     for (int s : strides) {
-        const float ms = best_of([&] { k_stride<<<148 * 8, 256>>>(h, colwords, s, 4, out); });
+        const float ms = best_of([&] { k_stride<<<sms * 8, 256>>>(h, colwords, s, 4, out); });
         const double reqs = (double)colwords / s;
         printf("1 column, stride %4d B: %8.2f ms  %7.1f M words/s\n", s * 4, ms, reqs / ms / 1e3);
     }
     for (int s : {16, 64}) { // rows 64 B / 256 B apart
         const double reqs1 = (double)(colwords / s);
         float ms;
-        ms = best_of([&] { k_cols<1, false, false><<<148 * 4, 256>>>(h, colwords, s, out); });
+        ms = best_of([&] { k_cols<1, false, false><<<sms * 4, 256>>>(h, colwords, s, out); });
         printf("stride %4d B  1 col               grid-stride: %8.2f ms %7.1f M reads/s\n", s * 4, ms, reqs1 / ms / 1e3);
-        ms = best_of([&] { k_cols<4, false, false><<<148 * 4, 256>>>(h, colwords, s, out); });
+        ms = best_of([&] { k_cols<4, false, false><<<sms * 4, 256>>>(h, colwords, s, out); });
         printf("stride %4d B  4 cols independent  grid-stride: %8.2f ms %7.1f M reads/s\n", s * 4, ms, 4 * reqs1 / ms / 1e3);
-        ms = best_of([&] { k_cols<4, true, false><<<148 * 4, 256>>>(h, colwords, s, out); });
+        ms = best_of([&] { k_cols<4, true, false><<<sms * 4, 256>>>(h, colwords, s, out); });
         printf("stride %4d B  4 cols chained      grid-stride: %8.2f ms %7.1f M reads/s\n", s * 4, ms, 4 * reqs1 / ms / 1e3);
-        ms = best_of([&] { k_cols<1, false, true><<<148 * 4, 256>>>(h, colwords, s, out); });
+        ms = best_of([&] { k_cols<1, false, true><<<sms * 4, 256>>>(h, colwords, s, out); });
         printf("stride %4d B  1 col               block-contig: %8.2f ms %7.1f M reads/s\n", s * 4, ms, reqs1 / ms / 1e3);
-        ms = best_of([&] { k_cols<4, false, true><<<148 * 4, 256>>>(h, colwords, s, out); });
+        ms = best_of([&] { k_cols<4, false, true><<<sms * 4, 256>>>(h, colwords, s, out); });
         printf("stride %4d B  4 cols independent  block-contig: %8.2f ms %7.1f M reads/s\n", s * 4, ms, 4 * reqs1 / ms / 1e3);
-        ms = best_of([&] { k_cols<4, true, true><<<148 * 4, 256>>>(h, colwords, s, out); });
+        ms = best_of([&] { k_cols<4, true, true><<<sms * 4, 256>>>(h, colwords, s, out); });
         printf("stride %4d B  4 cols chained      block-contig: %8.2f ms %7.1f M reads/s\n", s * 4, ms, 4 * reqs1 / ms / 1e3);
     }
     printf("%s\n", cudaGetErrorString(cudaGetLastError()));

@@ -1,5 +1,5 @@
-"""SASS excerpts of the hot kernels for profiles/ (cuobjdump -sass of the in-tree library; runs without a GPU).
-    python scripts/sass_excerpts.py > profiles/r2_sass_excerpts.txt"""
+"""SASS excerpts of the hot kernels (cuobjdump -sass of the in-tree library; runs without a GPU), printed to stdout.
+    python scripts/sass_excerpts.py > sass_excerpts.txt"""
 import collections
 import os
 import re
@@ -44,7 +44,7 @@ def section(title, sub, pats, maxhits=24):
     print()
 
 
-print("SASS excerpts of the hot kernels (cuobjdump -sass starrocks_b200/libsr_gpu.so, sm_100a, CUDA 12.9), round 2.\n"
+print("SASS excerpts of the hot kernels (cuobjdump -sass starrocks_b200/libsr_gpu.so, sm_90a).\n"
       "For every kernel: the opcode census of the whole function, then the lines that show the memory path it uses.\n")
 section("k_frag_stream_tests<false> (streaming pass, LDG form): 128-bit streaming loads of the two key columns (LDG.E.NA.128), bitmap word fetches from "
         "shared memory (LDS) and global memory (predicated LDG.E.CONSTANT), clamp onto the guard bit (VIMNMX / VIADDMNMX), selection-vector stores",

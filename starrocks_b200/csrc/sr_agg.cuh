@@ -469,7 +469,7 @@ __device__ __forceinline__ void acc_smem_flush(const AggDev& a, const AccPtrs& p
 constexpr int AGG_BLOCK = 256;
 // the row-at-a-time push kernels wait on one DRAM access after the other (ncu: 55-60 % of the stall samples are
 // long-scoreboard waits at the key / input loads), so their throughput is proportional to the warps in flight: cap the
-// registers at 32 for full occupancy (measured: 40 registers = 6 CTAs/SM made the dense push 2.93 -> 4.07 ms per 200 M rows)
+// registers at 32 for full occupancy (the push is latency bound: fewer resident CTAs make it slower)
 constexpr int AGG_MIN_BLOCKS = 8;
 
 // standalone aggregate sink: one pass over a chunk.

@@ -3,8 +3,8 @@
 // Replaces, for large batches, the row-at-a-time lazy_emplace + update of
 //   AggHashMap*::compute_agg_states            be/src/exec/aggregate/agg_hash_map.h:303-361
 //   Aggregator::compute_batch_agg_states       be/src/exec/aggregator.cpp:1616-1640
-// whose GPU transcription (k_agg_push) pays one L2 atomic transaction per row and state word (measured: 60-90 G
-// atomics/s whatever the table size).  Here the batch is first moved next to the table slices it updates:
+// whose GPU transcription (k_agg_push) pays one L2 atomic transaction per row and state word, a rate
+// that does not improve with the table size.  Here the batch is first moved next to the table slices it updates:
 //
 //   k_aggp_scatter   packed RECORDS (key, evaluated function inputs, null mask; W 8-byte words) are partitioned by the
 //                    top bits of their home slot.  Inside a tile every row takes its rank in its bucket with one shared-memory
@@ -17,7 +17,7 @@
 //                    loaded / initialised in shared memory, the bucket's records are applied with shared-memory atomics,
 //                    the slices are written back with coalesced stores.
 //   k_aggp_apply_l2  global-atomics apply for the overflow list, for slices that filled up, and for tables of more
-//                    than 2^18 buckets (buckets of several CTA-loads: table range prefetched into L2, as in round 1).
+//                    than 2^18 buckets (buckets of several CTA-loads: table range prefetched into L2).
 #pragma once
 
 namespace srd {
@@ -208,10 +208,9 @@ __global__ void __launch_bounds__(AGGP_BLOCK, 1024 / AGGP_BLOCK) k_aggp_scatter(
         locate(tile, row0, tile_n, cbase);
         if (sa.l2_prefetch && MODE == SCATTER_CHUNK_SIMPLE && tile + gridDim.x < ntiles) {
             // the input columns of the CTA's NEXT tile are requested into L2 while this tile is ranked, scanned and copied
-            // out.  Measured per 1e9 rows (SR_AGG_NO_L2_PREFETCH=1 switches it off): level 1 11.90 -> 11.47 ms.  The same
-            // prefetch on the record tiles of level 2 and on the next bucket of the apply pass cost 0.5 ms each (8.09 ->
-            // 8.65, 9.94 -> 10.40 ms: their input was written by the previous kernel and is largely L2-resident already,
-            // the prefetch instructions only compete for issue slots) and is not done.
+            // out (SR_AGG_NO_L2_PREFETCH=1 switches it off).  The same prefetch on the record tiles of level 2 and on the
+            // next bucket of the apply pass is not done: their input was written by the previous kernel and is largely
+            // L2-resident already, so the prefetch instructions would only compete for issue slots.
             int64_t nrow0;
             int ntile_n;
             uint32_t ncbase;
@@ -288,8 +287,8 @@ __global__ void __launch_bounds__(AGGP_BLOCK, 1024 / AGGP_BLOCK) k_aggp_scatter(
                     }
             }
         }
-        // rank inside (tile, bucket): one shared-memory atomic per row.  (Measured against a ballot-per-bit match with
-        // warp-private counters, which needs no atomic: 14.4 / 11.1 ms vs 13.3 / 8.7 ms per 1e9 rows for the two levels.)
+        // rank inside (tile, bucket): one shared-memory atomic per row (a ballot-per-bit match with warp-private counters
+        // needs no atomic but costs more instructions than it saves).
 #pragma unroll
         for (int k = 0; k < R; k++)
             if (lr[k] != 0xFFFFFFFFu) lr[k] = lr[k] << 16 | atomicAdd(&s_hist[lr[k]], 1u);
@@ -501,9 +500,8 @@ __global__ void __launch_bounds__(AGGP_APPLY_BLOCK, 4) k_aggp_apply(const AggDev
         }
         __syncthreads();
         uint32_t my_new = 0;
-        // (Measured and rejected: a special loop for the 8-byte-key COUNT + SUM shape with four record loads in flight per
-        // thread and the probe on 32-bit shared addresses (ld.volatile.shared / atom.shared.cas): 9.9 -> 14.4 ms per 1e9 rows.
-        // The four CTAs of an SM already overlap each other's load latency; the wider loop body only cost issue slots.)
+        // (No special loop for the 8-byte-key COUNT + SUM shape with several record loads in flight per thread: the four
+        // CTAs of an SM already overlap each other's load latency, and a wider loop body only costs issue slots.)
         for (int64_t q = tid; q < nrec; q += AGGP_APPLY_BLOCK) {
             const unsigned long long* rp = brec + (size_t)q * W;
             HKey key;

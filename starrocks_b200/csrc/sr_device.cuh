@@ -1,6 +1,6 @@
 // sr_device.cuh -- device-side building blocks shared by all kernels of libsr_gpu.so:
 // typed column loads, the reference's hash functions, the compiled expression interpreter,
-// block scan / ordered compaction helpers.  sm_100a only.
+// block scan / ordered compaction helpers.  sm_90a only.
 #pragma once
 
 #include <cuda_runtime.h>
@@ -65,15 +65,17 @@ __device__ __forceinline__ int4 ldg_stream_v4(const void* p) {
                  : "l"(p));
     return r;
 }
-// one 256-bit load (sm_100: LDG.E.256): a whole 32-byte sector per lane in one instruction / one L1 wavefront per line
-// instead of two 128-bit halves.  p must be 32-byte aligned.
+// a whole 32-byte sector per lane: sm_90 has no 256-bit load, so two 128-bit loads issued back to back (both halves are
+// in flight before either is used).  p must be 32-byte aligned.
 __device__ __forceinline__ void ldg_nc_u32x8(const void* p, uint32_t (&w)[8]) {
-    asm volatile("ld.global.nc.v8.u32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
+    asm volatile("ld.global.nc.v4.u32 {%0,%1,%2,%3}, [%8];\n\t"
+                 "ld.global.nc.v4.u32 {%4,%5,%6,%7}, [%8+16];"
                  : "=r"(w[0]), "=r"(w[1]), "=r"(w[2]), "=r"(w[3]), "=r"(w[4]), "=r"(w[5]), "=r"(w[6]), "=r"(w[7])
                  : "l"(p));
 }
 __device__ __forceinline__ void ldg_stream_u32x8(const void* p, uint32_t (&w)[8]) {
-    asm volatile("ld.global.nc" SR_LD_HINT ".v8.u32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
+    asm volatile("ld.global.nc" SR_LD_HINT ".v4.u32 {%0,%1,%2,%3}, [%8];\n\t"
+                 "ld.global.nc" SR_LD_HINT ".v4.u32 {%4,%5,%6,%7}, [%8+16];"
                  : "=r"(w[0]), "=r"(w[1]), "=r"(w[2]), "=r"(w[3]), "=r"(w[4]), "=r"(w[5]), "=r"(w[6]), "=r"(w[7])
                  : "l"(p));
 }

@@ -7,7 +7,7 @@
 //     -> JoinHashMap::probe (lookup_init + _probe_from_ht + _probe_output/_build_output)
 //   AggregateBlockingSinkOperator::push_chunk               aggregate/aggregate_blocking_sink_operator.cpp:101-138
 //
-// B200 design (HBM-bound integer/gather work, no tensor cores):
+// H100 design (HBM-bound integer/gather work, no tensor cores):
 //  * persistent CTAs (grid = SMs x resident CTAs).  The main loop streams the scan-predicate
 //    columns and the FIRST join's key column: each thread owns groups of 4 consecutive rows, so a
 //    tile column is one 128-bit ld.global.nc.L1::no_allocate per thread and group;
@@ -343,8 +343,8 @@ static int32_t frag_plan(sr_fragment* f, const VTab& vt, int64_t n) {
                     if (ah.fns[q].input.nodes[k].op == srd::C_LOAD_I || ah.fns[q].input.nodes[k].op == srd::C_LOAD_D) want(ah.fns[q].input.nodes[k].arg);
             for (int k = 0; k < SR_FINAL_PREFETCH; k++) f->pass.final_vals[k] = -1;
             for (int k = 0; k < SR_MAX_VALUES; k++) f->pass.final_slot[k] = -1;
-            // measured on B200 (profiles/r1_notes.md): the burst costs more issue slots and registers than the
-            // latency it hides -- the final pass is L1TEX-gather bound, not latency bound -- so it stays off
+            // the burst costs more issue slots and registers than the latency it hides -- the final pass is
+            // L1TEX-gather bound, not latency bound -- so it stays off
             const bool kFinalPrefetch = false;
             for (size_t k = 0; k < need.size() && k < SR_FINAL_PREFETCH; k++) {
                 f->pass.final_vals[k] = (int8_t)need[k]; // also the L2 prefetch list of host-resident input
@@ -472,7 +472,7 @@ static int32_t frag_push(sr_fragment* f, const sr_chunk_view* fact) {
         // this push's pass parameters: the carried key (planned in f->pass) is only used for host-resident input
         srd::PassDev pass = f->pass;
         pass.host_input = fact->mem == SR_MEM_HOST_PINNED ? 1 : 0;
-        const bool carry = pass.host_input && pass.carry_join >= 0; // (HBM input, measured: stream +0.27 ms, final -0.09 ms)
+        const bool carry = pass.host_input && pass.carry_join >= 0; // (HBM input: the register cost in the stream pass outweighs the saved re-read)
         if (!carry) pass.carry_join = pass.carry_value_id = -1;
         unsigned long long* cnt = f->pass_counters.as<unsigned long long>();
         SR_CUDA(ctx, cudaMemsetAsync(cnt, 0, 16 * sizeof(uint64_t), ctx->stream));

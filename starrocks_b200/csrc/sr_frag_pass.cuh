@@ -360,10 +360,9 @@ __device__ __forceinline__ uint32_t stream_test(const StreamTest& st, const Frag
     return join_test_batch<N>(s_joins[st.join], smem, k, alive);
 }
 
-// The two vector-column tests of k_frag_stream_tests with their parameters held in REGISTERS for the whole kernel.  ncu
-// (profiles/r2_notes.md) showed that kernel issue bound at 47.8 instructions per row, 6.4 of them re-reading the
-// warp-uniform test descriptors from shared memory on every call (the compiler cannot hoist them over the selection-vector
-// stores) and 13.5 in the shared-memory bitmap test.  kind: 0 = range conjunct, 1 = bitmap in shared memory (int32 index
+// The two vector-column tests of k_frag_stream_tests with their parameters held in REGISTERS for the whole kernel.  The
+// kernel is issue bound, and otherwise re-reads the warp-uniform test descriptors from shared memory on every call (the
+// compiler cannot hoist them over the selection-vector stores) next to the shared-memory bitmap test.  kind: 0 = range conjunct, 1 = bitmap in shared memory (int32 index
 // arithmetic, zero GUARD bit at index span + 1: an out-of-range key is clamped onto it, so the test needs neither a
 // predicate nor a select), 2 = bitmap in global memory (predicated word fetches, issued back to back), 3 = anything else
 // (falls back to stream_test).
@@ -542,7 +541,7 @@ __global__ void __launch_bounds__(STREAM_BLOCK, 2) k_frag_stream_tests(const Fra
 // their eight keys per column with 128-bit shared loads and release the stage through a second mbarrier, on which thread 0
 // waits before it issues the copy of tile + 2.  The register prefetch of k_frag_stream_tests and its LDG.128 / L1TEX tag
 // traffic are gone; the price is 64 KB more shared memory per CTA and two shared loads per column.
-// Opt-in (SR_FRAG_STREAM_TMA=1): measured against the LDG form in profiles/r2_notes.md.
+// Opt-in (SR_FRAG_STREAM_TMA=1): the pass is issue bound, so the LDG form stays the default.
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"((uint32_t)__cvta_generic_to_shared(bar)), "r"(count) : "memory");
 }
@@ -703,8 +702,7 @@ __device__ __forceinline__ void warp_sel_range(unsigned long long n, unsigned lo
 }
 
 // the final pass is a chain of dependent gathers per row: latency bound, so resident warps matter more than spills.
-// Measured on SSB Q4.1 SF100 (9.6 M rows reach it): 66 registers / 3 CTAs per SM 0.89 ms, 62 / 4: 0.73, 48 / 5: 0.667,
-// 40 / 6: 0.669, 32 / 8: 0.70 ms.
+// Five CTAs per SM (48 registers) balance resident warps against spills.
 #ifndef SR_GATHER_AGG_MIN_BLOCKS
 #define SR_GATHER_AGG_MIN_BLOCKS 5
 #endif
@@ -771,11 +769,10 @@ __global__ void __launch_bounds__(GATHER_BLOCK, SR_GATHER_AGG_MIN_BLOCKS) k_frag
         acc_ptrs_global(ad, acc);
     }
     __syncthreads(); // s_joins and the shared accumulators are filled cooperatively: no warp may run ahead of that
-    // Measured and rejected (profiles/r1_notes.md): requesting the NEXT row's fact sectors with prefetch.global.L2
-    // while the current row walks its dependent chain.  HBM-resident input: 0.73 -> 1.27 ms (the prefetch fetches
-    // whole 128-byte lines where the loads need one 32-byte sector: 4x the DRAM traffic of a pass that is bound by
-    // random-sector throughput, not latency).  Host-resident input: mapped host memory is not kept in L2, the
-    // prefetch only doubled the PCIe requests (117 -> 224 ms on SSB Q4.1 SF100).
+    // Not done: requesting the NEXT row's fact sectors with prefetch.global.L2 while the current row walks its dependent
+    // chain.  For HBM-resident input the prefetch fetches whole 128-byte lines where the loads need one 32-byte sector
+    // (4x the DRAM traffic of a pass that is bound by random-sector throughput, not latency); mapped host memory is not
+    // kept in L2, so for host-resident input the prefetch only doubles the PCIe requests.
     const unsigned long long n_in = *n_in_ptr;
     unsigned long long passed = 0;
     constexpr bool single = SINGLE;
@@ -787,8 +784,8 @@ __global__ void __launch_bounds__(GATHER_BLOCK, SR_GATHER_AGG_MIN_BLOCKS) k_frag
         const SelEntry entry = sel_in[i];
         const uint32_t row = sel_row(entry);
         if (row == SEL_INVALID) continue;
-        // (a variant that fetched every fact value of the row in one burst before the dependent lookups was
-        // measured slower on B200 -- more issue slots and registers than latency hidden, see profiles/)
+        // (a variant that fetches every fact value of the row in one burst before the dependent lookups costs more
+        // issue slots and registers than the latency it hides)
         FragLoader ld{vt, (int64_t)row, {0, 0, 0, 0, 0, 0}, pd.carry_join >= 0 ? (int32_t)pd.carry_value_id : -1, sel_carry(entry)};
         bool ok = true;
 #pragma unroll 1

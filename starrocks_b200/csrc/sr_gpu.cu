@@ -1,5 +1,5 @@
 // sr_gpu.cu -- C-ABI of libsr_gpu.so (include/sr_gpu_ops.h).  One translation unit: the device
-// code lives in the headers included below.  sm_100a only; there is no CPU fallback: without a
+// code lives in the headers included below.  sm_90a only; there is no CPU fallback: without a
 // CUDA device every entry point fails with SR_ERR_NO_DEVICE / SR_ERR_CUDA.
 #include "sr_frag.cuh"
 #include "sr_serde.cuh"
@@ -1661,7 +1661,7 @@ int32_t sr_pages_decode(sr_page_decoder* d, int32_t encoding, int32_t type, cons
 int32_t sr_flush_l2(sr_ctx* ctx) {
     SR_BIND(ctx);
     if (!ctx->l2_flush) {
-        ctx->l2_flush_bytes = 512ull << 20; // 4x the 126 MB L2
+        ctx->l2_flush_bytes = 512ull << 20; // 10x the 50 MB L2
         SR_CUDA(ctx, cudaMalloc(&ctx->l2_flush, ctx->l2_flush_bytes));
     }
     SR_CUDA(ctx, cudaMemsetAsync(ctx->l2_flush, 0, ctx->l2_flush_bytes, ctx->stream));

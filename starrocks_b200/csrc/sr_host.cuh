@@ -22,7 +22,7 @@ struct sr_ctx {
     int32_t err_code = 0;
     int64_t launches = 0;
     int64_t dev_bytes = 0;
-    int num_sms = 148;
+    int num_sms = 132;
     // pinned scratch for tiny D2H results (counters) -- one slot per use inside a call
     uint64_t* pinned = nullptr; // 64 x u64
     uint64_t* dscratch = nullptr; // 64 x u64 on device

@@ -7,7 +7,7 @@
 //   _probe_output / _build_output           :163-269
 //   JoinHashTable::append_chunk             be/src/exec/join/join_hash_table.cpp:712-752
 //
-// Device layout (B200-first, not the CPU layout):
+// Device layout (GPU-first, not the CPU layout):
 //  * build columns are concatenated in HBM with row 0 reserved as the sentinel (same 1-based
 //    build index convention as the reference, so index pairs are comparable);
 //  * DIRECT / RANGE_DIRECT_MAPPING: first[key - min] (uint32 head row) + next[] chain, built
@@ -334,7 +334,7 @@ constexpr int PROBE_TILE = PROBE_BLOCK * PROBE_ROWS;
 
 // pass 1: heads[row] + per-block output counts.
 // The lookups are dependent chains (key -> table word), so one row per thread leaves the kernel waiting on a single
-// L2 / DRAM access per warp (measured 1.44 ms per 200 M int32 keys = 0.55 TB/s).  Each thread therefore takes
+// L2 / DRAM access per warp.  Each thread therefore takes
 // PROBE_ROWS consecutive rows: one 128-bit key load when the key is a plain int32 column, then all bitmap words, then
 // all first[] words of the rows whose bit is set -- range methods read the 1-bit-per-key bitmap (32x denser than
 // first[], L1/L2 resident) first, so only matching rows gather from first[].
@@ -398,10 +398,9 @@ __global__ void __launch_bounds__(PROBE_BLOCK) k_probe_count(JoinDev j, KeyCols 
     }
 }
 
-// (Measured and rejected, round 2: ONE kernel for unique build keys -- lookup, block ranking, a decoupled look-back over
-// per-tile status words for the global offset, ordered pair write; no heads[] round trip, no separate scan.  200 M probe
-// rows, 20 % match: 4.37 ms against 1.87 ms for the two passes below -- with four rows per thread a tile is too little
-// work to hide the serial look-back chain of 195 K tiles.)
+// (Not done: ONE kernel for unique build keys -- lookup, block ranking, a decoupled look-back over per-tile status words
+// for the global offset, ordered pair write.  With four rows per thread a tile is too little work to hide the serial
+// look-back chain over ~200 K tiles of a 200 M-row probe.)
 // pass 2: write (probe_index, build_index) pairs in probe order
 __global__ void __launch_bounds__(PROBE_BLOCK) k_probe_write(JoinDev j, int32_t join_type, int64_t n, const uint32_t* __restrict__ heads,
                                                               const uint64_t* __restrict__ block_offsets, uint32_t* __restrict__ probe_index,
@@ -811,7 +810,7 @@ static int32_t join_finish(sr_join* j) {
     const int kw = srd::type_width(j->desc.key_types[0]);
     // --- method selection (JoinHashMapSelector::_determine_hash_map_method, join_hash_table.cpp:225-350,
     // with the CPU L2/L3 thresholds replaced by an HBM/L2 budget: a direct table is used while it
-    // stays within 64x the row count or 64 MiB (half of B200's L2)) ---
+    // stays within 64x the row count or 25 MiB, half of H100's 50 MB L2) ---
     j->method = SR_JOIN_METHOD_LINEAR_CHAINED;
     if (one_key && kw <= 2) {
         j->method = SR_JOIN_METHOD_DIRECT_MAPPING;
@@ -824,7 +823,7 @@ static int32_t join_finish(sr_join* j) {
         }
     } else if (one_key && j->desc.enable_range_direct_mapping && valid > 0) {
         const unsigned __int128 interval = (unsigned __int128)((__int128)mm[1] - (__int128)mm[0]) + 1;
-        const uint64_t budget = std::max<uint64_t>((uint64_t)valid * 64, (64ull << 20) / 4);
+        const uint64_t budget = std::max<uint64_t>((uint64_t)valid * 64, (25ull << 20) / 4);
         if (interval < 0xFFFFFFFFull && (uint64_t)interval <= budget) {
             j->method = SR_JOIN_METHOD_RANGE_DIRECT_MAPPING;
             j->min_value = mm[0];

@@ -7,7 +7,7 @@
 // (uint32 LE).  Storage format 0: value = min + delta; 1 (ascending input): value = previous + delta, the first previous
 // being min; 2: the values themselves in 8 * sizeof(T) bits.
 //
-// B200 mapping (HBM- / PCIe-bound byte work): pages are read where they lie -- device memory or page-locked mapped host
+// H100 mapping (HBM- / PCIe-bound byte work): pages are read where they lie -- device memory or page-locked mapped host
 // memory (the decode then IS the host->device transfer, at 4-22 bits per value instead of 32 / 64) -- or staged once when they
 // are pageable.  k_page_footers reads the value counts, the host turns them into row / frame offsets (one small
 // read-back per batch of pages), k_for_frames expands every page's frame table into per-frame descriptors (byte position by

@@ -239,7 +239,7 @@ __device__ __forceinline__ void compact_rows_vec32(const void* __restrict__ src,
 
 // survivors of a tile staged in shared memory (in order), then written by consecutive lanes: the direct form above lets
 // every lane store to its own run of the output, i.e. up to 32 partially written sectors per store instruction, which is
-// what bounded the 50 %-pass case (1.37 ms per 200 M rows x 4 columns)
+// what bounds the dense-pass case
 template <typename T>
 __device__ __forceinline__ void compact_rows_staged(const void* __restrict__ src, void* __restrict__ dst, int64_t base, uint32_t m, bool vec, T* __restrict__ stage,
                                                     uint32_t my_off, uint32_t tile_total, uint64_t tile_out) {
@@ -263,7 +263,7 @@ __device__ __forceinline__ void compact_rows_staged(const void* __restrict__ src
 }
 
 // STAGED: instantiated with the staging buffer; the host picks it when at least 1/8 of the rows survive (the buffer's
-// 16 KB per CTA and the extra registers cost the sparse case its latency hiding: 0.74 -> 1.04 ms at 1.9 % pass)
+// 16 KB per CTA and the extra registers cost the sparse case its latency hiding)
 template <bool STAGED>
 __global__ void __launch_bounds__(SCANW_BLOCK) k_scan_compact(const uint8_t* __restrict__ mask_bits, const uint32_t* __restrict__ local_excl,
                                                                const uint64_t* __restrict__ block_offsets, CompactArgs args, int64_t n) {
@@ -385,7 +385,7 @@ __global__ void __launch_bounds__(256) k_gather(const uint32_t* __restrict__ ind
 // ---------------------------------------------------------------------------------------
 // Exclusive scan of n uint32 counts into uint64 offsets, total -> ctx->dscratch[0].  Small inputs: one block walks
 // the array (k_scan_counts); large inputs: 1024-entry blocks in parallel, a scan of the block sums, a fix-up pass
-// (the single block needs ~2 us per 1024 entries: 1.5 ms for the 781 K tiles of a 200 M-row probe).
+// (a single block walks 1024 entries at a time, far too slow for the ~780 K tiles of a 200 M-row probe).
 struct ScanScratch {
     DevBuf local, sums, bases;
 };

@@ -15,7 +15,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("SR_GPU_LIB") or os.path.join(_HERE, "libsr_gpu.so")   # SR_GPU_LIB: an experimental build
 _LIB = None
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-shared",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-shared",
               "-Xcompiler", "-fPIC", "-cudart", "static"]
 
 
@@ -38,7 +38,7 @@ def _source_hash():
 
 
 def build(verbose=False):
-    """compile libsr_gpu.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).  Safe against concurrent callers
+    """compile libsr_gpu.so in-tree with nvcc for sm_90a (cross-compiles without a GPU).  Safe against concurrent callers
     (the ranks of a torchrun job): one process compiles under a file lock into a temporary name and renames it into place."""
     import fcntl
     src = os.path.join(_HERE, "csrc", "sr_gpu.cu")

@@ -1,4 +1,4 @@
-"""CPU-side checks of the drop-in boundary: the C-ABI shared library builds for sm_100a, loads, exports
+"""CPU-side checks of the drop-in boundary: the C-ABI shared library builds for sm_90a, loads, exports
 every symbol include/sr_gpu_ops.h declares, agrees with the ctypes struct layouts, and fails LOUDLY
 (no CPU fallback) when no CUDA device is present.  No compute calls here."""
 import ctypes as C

@@ -1,7 +1,7 @@
-"""High-cardinality group-by on one B200 (BASELINE.json config 5; SURVEY.md section 8d):
-1e9 rows, key int64 = splitmix64(i) mod 1e8, value int64 U[0, 1000]; SELECT key, SUM(v), COUNT(*) GROUP BY key.
+"""High-cardinality group-by on one H100 (BASELINE.json config 5 at half size, which fits 80 GB; SURVEY.md section 8d):
+5e8 rows, key int64 = splitmix64(i) mod 5e7, value int64 U[0, 1000]; SELECT key, SUM(v), COUNT(*) GROUP BY key.
 
-    python tools/groupby_highcard.py [--rows 1000000000] [--keys 100000000] [--morsel 100000000]
+    python tools/groupby_highcard.py [--rows 500000000] [--keys 50000000] [--morsel 100000000]
 
 The table is the sr_agg hash table (open addressing, 64-bit CAS claim, SoA accumulators); rows are pushed in morsels
 through the C-ABI (sr_agg_push) from HBM-resident columns.  Size-independent checks (the CPU oracle would need minutes
@@ -34,9 +34,9 @@ def splitmix64(x):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--rows", type=int, default=1_000_000_000)
-    ap.add_argument("--keys", type=int, default=100_000_000)
-    ap.add_argument("--morsel", type=int, default=1_000_000_000)
+    ap.add_argument("--rows", type=int, default=500_000_000)
+    ap.add_argument("--keys", type=int, default=50_000_000)
+    ap.add_argument("--morsel", type=int, default=500_000_000)
     ap.add_argument("--reps", type=int, default=3)
     args = ap.parse_args()
     dev = torch.device("cuda:0")

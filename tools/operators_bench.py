@@ -1,5 +1,5 @@
 """Throughput of the separate operator entry points (the non-fused path a BE pipeline takes when a plan shape is not
-covered by the fused fragment) on HBM-resident chunks, one B200:
+covered by the fused fragment) on HBM-resident chunks, one H100:
 
     python tools/operators_bench.py [--rows 200000000]
 

@@ -1,4 +1,4 @@
-"""SSB Q1.1 (flat form: scan + 3 predicates + SUM(lo_extendedprice * lo_discount), no join) on one B200 -- BASELINE.json
+"""SSB Q1.1 (flat form: scan + 3 predicates + SUM(lo_extendedprice * lo_discount), no join) on one H100 -- BASELINE.json
 config 0 at SF100 size, through (a) the fused fragment and (b) the separate operators (sr_scan_filter -> sr_agg_push).
 
     python tools/q11_scan.py [--rows 600000000]

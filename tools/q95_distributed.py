@@ -1,4 +1,4 @@
-"""TPC-DS Q95 shape across the N GPUs of one box (BASELINE.json config 4: SF1000 on 8 x B200, ExchangeSink all-to-all).
+"""TPC-DS Q95 shape across the N GPUs of one box (BASELINE.json config 4: SF1000 on 8 GPUs, ExchangeSink all-to-all).
 
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
         tools/q95_distributed.py --sf 1000 [--check oracle|invariants|none]
@@ -43,6 +43,7 @@ def parse(argv=None):
     ap.add_argument("--steps", type=int, default=2)
     ap.add_argument("--warmup", type=int, default=1)
     ap.add_argument("--morsel-rows", type=int, default=4_000_000)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write the last timed step's result as DIR/<name>.npy (float64)")
     return ap.parse_args(argv)
 
 
@@ -134,6 +135,12 @@ def main(args=None):
                 "plan_rows": {"self_join_output": tot[9], "ws_wh_orders": tot[10], "rows_aggregated": tot[11]},
                 "exchange_bytes": tot[8], "checks": checks, "check_mode": args.check}
         print(json.dumps(line))
+        if args.dump_outputs:
+            # the query's three numbers from the last timed step
+            import numpy as np
+            os.makedirs(args.dump_outputs, exist_ok=True)
+            for nm, v in zip(("count_distinct_orders", "sum_ext_ship_cost", "sum_net_profit"), tot[0:3]):
+                np.save(os.path.join(args.dump_outputs, nm + ".npy"), np.array([v], dtype=np.float64))
     ok = all(checks.values()) if checks else True
     flag = torch.tensor([0 if ok else 1], device=dev)
     dist.broadcast(flag, 0)
