@@ -642,9 +642,13 @@ typedef struct sr_fragment_plan {
     int32_t mode;             /* 1 = fused cascade kernel, 2 = selection-vector passes */
     int32_t num_stream_joins; /* mode 2: joins tested by the streaming pass */
     int32_t num_gather_passes;
-    int32_t reserved;
+    int32_t final_pass; /* mode 2: the final pass of the last push, SR_FINAL_PASS_* */
     double pred_rate; /* fraction of sampled rows passing the scan conjuncts */
 } sr_fragment_plan;
+#define SR_FINAL_PASS_NONE 0    /* no push yet, or the fused cascade kernel */
+#define SR_FINAL_PASS_GENERIC 1 /* k_frag_gather_agg: any join, aggregate and expression */
+#define SR_FINAL_PASS_EXPAND 2  /* k_frag_gather_agg_expand: one-to-many joins */
+#define SR_FINAL_PASS_DENSE 3   /* k_frag_final_dense: slot-digit directories, batched rows, dense shared-memory aggregate */
 int32_t sr_fragment_get_plan(sr_fragment* frag, sr_fragment_plan* plan);
 /* device time of the passes of the LAST push in selection-vector mode (CUDA events on the context's
  * stream; synchronises): ms[0] = streaming pass, ms[1] = gather-join passes, ms[2] = final pass.

@@ -167,7 +167,10 @@ class sr_fragment_plan(C.Structure):
                 ("bitmap_in_smem", C.c_int32 * SR_MAX_FRAG_JOINS), ("pass_rate", C.c_double * SR_MAX_FRAG_JOINS),
                 ("smem_bytes", C.c_int32), ("grid", C.c_int32), ("block", C.c_int32), ("agg_in_smem", C.c_int32),
                 ("mode", C.c_int32), ("num_stream_joins", C.c_int32), ("num_gather_passes", C.c_int32),
-                ("reserved", C.c_int32), ("pred_rate", C.c_double)]
+                ("final_pass", C.c_int32), ("pred_rate", C.c_double)]
+
+
+FINAL_PASS_NAMES = {0: None, 1: "generic", 2: "expand", 3: "dense-batched"}   # sr_fragment_plan.final_pass (SR_FINAL_PASS_*)
 
 
 class sr_part_desc(C.Structure):

@@ -68,6 +68,14 @@ struct sr_fragment {
     size_t stream_smem = 0;
     int stream_grid = 0;
     int final_grid = 0;
+    // the batched final pass (k_frag_final_dense): planned when the shape allows it, used by a push whose fact columns
+    // are all plain int32 and whose aggregate still accumulates in shared memory
+    bool final_dense_ok = false;
+    srd::FinalDense final_dense;             // pointers into the fact chunk and the aggregate are filled per push
+    int8_t final_fn_src[srd::FINAL_MAX_FNS]; // aggregate function behind each FinalDense::fn
+    DevBuf digits[SR_MAX_FRAG_JOINS];        // slot-digit directories, per probe position
+    int final_dense_grid = 0;
+    int32_t final_pass = SR_FINAL_PASS_NONE; // the final pass of the last push
     cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
     bool timed_push = false;
     ~sr_fragment() {
@@ -210,6 +218,124 @@ static int32_t frag_compile(sr_fragment* f) {
     return SR_OK;
 }
 
+// Plan the batched final pass (k_frag_final_dense) of selective mode, once the join order is fixed.  It applies when
+//  * the aggregate is dense, accumulates in shared memory and has fewer slots than the reserved digit values;
+//  * every join the final pass looks up is range-mapped with unique keys and an int32 range, and its payload columns
+//    are only group keys: it gets a slot-digit directory, built here;
+//  * every join the final pass only tests is a bitmap test;
+//  * every aggregate input is one fact column in an integer mode acc_apply_shared handles (COUNT(*), SUM, COUNT, MIN,
+//    MAX on int64 states).
+// Otherwise the generic final pass runs.  That the fact columns are plain int32 is checked per push.
+static int32_t frag_plan_final_dense(sr_fragment* f) {
+    sr_ctx* ctx = f->ctx;
+    const srd::FragDev& h = f->host;
+    const srd::AggDev& ah = f->agg->host;
+    srd::FinalDense& fp = f->final_dense;
+    memset(&fp, 0, sizeof(fp));
+    f->final_dense_ok = false;
+    if (f->expand || !f->smem_agg || !ah.dense || ah.num_keys == 0 || ah.cap >= SR_DIGIT_BAD) return SR_OK;
+    const int nv = f->pass.num_final_vals;
+    if (nv > srd::FINAL_MAX_VALS) return SR_OK;
+    auto val_of = [&](int id) {
+        for (int k = 0; k < nv; k++)
+            if (f->pass.final_vals[k] == id) return k;
+        return -1;
+    };
+    fp.num_vals = nv;
+    fp.carry_val = -1;
+    fp.cap = (int32_t)ah.cap;
+    // group keys that are fact columns; the others must be payloads of a directory join
+    bool key_of_join[SR_MAX_FRAG_JOINS] = {};
+    for (int k = 0; k < ah.num_keys; k++) {
+        const int id = ah.key_value_id[k];
+        const int src = f->value_src[id];
+        if (src >= 0) {
+            key_of_join[src] = true;
+            continue;
+        }
+        if (fp.num_fkeys == srd::FINAL_MAX_FKEYS || val_of(id) < 0) return SR_OK;
+        srd::FinalDense::FKey& fk = fp.fkey[fp.num_fkeys++];
+        fk.val = val_of(id);
+        fk.lo = ah.dense_min[k];
+        fk.base = ah.key_nullable[k] ? 1u : 0u;
+        fk.span = ah.dense_extent[k] - fk.base;
+        fk.stride = (uint32_t)ah.dense_stride[k];
+    }
+    // every value read from a build row must be a group key (then the directory stands for it)
+    for (size_t id = 0; id < f->value_src.size(); id++) {
+        if (f->value_src[id] < 0) continue;
+        bool is_key = false;
+        for (int k = 0; k < ah.num_keys; k++) is_key |= ah.key_value_id[k] == (int)id;
+        if (!is_key) return SR_OK;
+    }
+    // aggregate functions
+    int32_t off = (int32_t)ah.cap; // shared-memory layout of acc_ptrs_smem: [cnt | acc0 per function]
+    for (int q = 0; q < ah.num_fns; q++) {
+        const srd::AggFnDev& fn = ah.fns[q];
+        if (fn.mode == srd::M_COUNT_STAR) continue;
+        if (fn.mode != srd::M_COUNT && fn.mode != srd::M_SUM_I64 && fn.mode != srd::M_MIN_I64 && fn.mode != srd::M_MAX_I64) return SR_OK;
+        if (fn.track_n || fn.n_value_id >= 0 || fn.input.num_nodes != 1 || fn.input.nodes[0].op != srd::C_LOAD_I) return SR_OK;
+        const int id = fn.input.nodes[0].arg;
+        if (f->value_src[id] >= 0 || val_of(id) < 0 || fp.num_fns == srd::FINAL_MAX_FNS) return SR_OK;
+        f->final_fn_src[fp.num_fns] = (int8_t)q;
+        srd::FinalDense::Fn& d = fp.fn[fp.num_fns++];
+        d.mode = fn.mode;
+        d.val = fn.mode == srd::M_COUNT ? -1 : val_of(id);
+        d.smem_off = off;
+        off += (int32_t)ah.cap;
+    }
+    // joins the final pass handles
+    int look_join[srd::FINAL_MAX_LOOK] = {};
+    for (int q = 0; q < f->num_joins; q++) {
+        const srd::FragJoinDev& fj = h.joins[q];
+        const bool test = q >= f->pass.final_first_join;
+        if (!fj.need_head && !test) continue;
+        const int kv = val_of(fj.key_value_id);
+        if (!fj.use_bitmap || !fj.idx32 || fj.expand || kv < 0) return SR_OK;
+        const uint32_t lo = (uint32_t)(int32_t)fj.j.min_value, span = (uint32_t)(fj.j.max_value - fj.j.min_value);
+        if (!fj.need_head) {
+            if (fp.num_test == srd::FINAL_MAX_TEST) return SR_OK;
+            fp.test[fp.num_test++] = srd::FinalDense::Test{fj.j.bitmap, lo, span, kv, 0};
+            continue;
+        }
+        if (!key_of_join[q] || fp.num_look == srd::FINAL_MAX_LOOK) return SR_OK;
+        look_join[fp.num_look] = q;
+        fp.look[fp.num_look++] = srd::FinalDense::Look{nullptr, lo, span, kv, 0};
+    }
+    // the directories
+    for (int L = 0; L < fp.num_look; L++) {
+        const int q = look_join[L];
+        srd::DigitPlan dp;
+        memset(&dp, 0, sizeof(dp));
+        for (int k = 0; k < ah.num_keys; k++) {
+            const int id = ah.key_value_id[k];
+            if (f->value_src[id] != q) continue;
+            const BuildCol* bc = f->value_col[id];
+            srd::DigitKey& dk = dp.k[dp.num_keys++];
+            dk.data = bc->data.p;
+            dk.nulls = bc->nullable ? (const uint8_t*)bc->nulls.p : nullptr;
+            dk.type = bc->type;
+            dk.nullable = ah.key_nullable[k];
+            dk.min = ah.dense_min[k];
+            dk.extent = ah.dense_extent[k];
+            dk.stride = ah.dense_stride[k];
+        }
+        const int64_t range = (int64_t)fp.look[L].span + 1;
+        SR_TRY(f->digits[q].reserve(ctx, sizeof(uint16_t) * (size_t)range));
+        srd::k_frag_build_digits<<<std::min(grid_for(range, 256), ctx->num_sms * 8), 256, 0, ctx->stream>>>(h.joins[q].j.first, range, dp,
+                                                                                                             f->digits[q].as<uint16_t>());
+        SR_LAUNCH_CHECK(ctx);
+        fp.look[L].digit = f->digits[q].as<uint16_t>();
+    }
+    const size_t smem = f->agg->smem_bytes;
+    SR_CUDA(ctx, cudaFuncSetAttribute(srd::k_frag_final_dense<SR_FINAL_ROWS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(smem, 16)));
+    int per_sm = 0;
+    SR_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, srd::k_frag_final_dense<SR_FINAL_ROWS>, srd::GATHER_BLOCK, smem));
+    f->final_dense_grid = std::max(per_sm, 1) * ctx->num_sms;
+    f->final_dense_ok = true;
+    return SR_OK;
+}
+
 // sample pass rates, order the joins, assign shared-memory bitmaps, upload, pick the grid
 static int32_t frag_plan(sr_fragment* f, const VTab& vt, int64_t n) {
     sr_ctx* ctx = f->ctx;
@@ -341,15 +467,8 @@ static int32_t frag_plan(sr_fragment* f, const VTab& vt, int64_t n) {
             for (int q = 0; q < ah.num_fns; q++)
                 for (int k = 0; k < ah.fns[q].input.num_nodes; k++)
                     if (ah.fns[q].input.nodes[k].op == srd::C_LOAD_I || ah.fns[q].input.nodes[k].op == srd::C_LOAD_D) want(ah.fns[q].input.nodes[k].arg);
-            for (int k = 0; k < SR_FINAL_PREFETCH; k++) f->pass.final_vals[k] = -1;
-            for (int k = 0; k < SR_MAX_VALUES; k++) f->pass.final_slot[k] = -1;
-            // the burst costs more issue slots and registers than the latency it hides -- the final pass is
-            // L1TEX-gather bound, not latency bound -- so it stays off
-            const bool kFinalPrefetch = false;
-            for (size_t k = 0; k < need.size() && k < SR_FINAL_PREFETCH; k++) {
-                f->pass.final_vals[k] = (int8_t)need[k]; // also the L2 prefetch list of host-resident input
-                if (kFinalPrefetch) f->pass.final_slot[need[k]] = (int8_t)k;
-            }
+            for (int k = 0; k < SR_FINAL_PREFETCH; k++) f->pass.final_vals[k] = k < (int)need.size() ? (int8_t)need[k] : (int8_t)-1;
+            f->pass.num_final_vals = (int8_t)std::min<size_t>(need.size(), 127);
         }
         f->gather_joins.clear();
         for (int q = ns; q < ff; q++) f->gather_joins.push_back(q);
@@ -391,6 +510,7 @@ static int32_t frag_plan(sr_fragment* f, const VTab& vt, int64_t n) {
             SR_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ga, srd::k_frag_gather_agg<false>, srd::GATHER_BLOCK, 0));
         f->grid = std::max(gj, 1) * ctx->num_sms;
         f->final_grid = std::max(ga, 1) * ctx->num_sms;
+        SR_TRY(frag_plan_final_dense(f));
         SR_TRY(f->pass_counters.reserve(ctx, 16 * sizeof(uint64_t)));
         f->compiled = true;
         return SR_OK;
@@ -522,7 +642,22 @@ static int32_t frag_push(sr_fragment* f, const sr_chunk_view* fact) {
         if (hash) SR_TRY(f->sel[cur ^ 1].reserve(ctx, sizeof(srd::SelEntry) * ((size_t)n + slack)));
         srd::SelEntry* fail_list = hash ? f->sel[cur ^ 1].as<srd::SelEntry>() : nullptr;
         unsigned long long* fail_count = cnt + 8;
-        if (f->expand)
+        // the batched final pass needs plain int32 fact columns and the shared-memory accumulators it was planned for
+        // (a push whose aggregate input turned nullable switches the aggregate to global accumulation)
+        const bool dense_final = f->final_dense_ok && vt.plain32 && f->smem_agg && a->smem_bytes > 0;
+        f->final_pass = dense_final ? SR_FINAL_PASS_DENSE : f->expand ? SR_FINAL_PASS_EXPAND : SR_FINAL_PASS_GENERIC;
+        if (dense_final) {
+            srd::FinalDense fp = f->final_dense;
+            for (int c = 0; c < fp.num_vals; c++) {
+                fp.cols[c] = (const int32_t*)vt.v[pass.final_vals[c]].data;
+                if (pass.carry_join >= 0 && pass.final_vals[c] == pass.carry_value_id) fp.carry_val = c;
+            }
+            for (int q = 0; q < fp.num_fns; q++) fp.fn[q].gacc = ah.fns[f->final_fn_src[q]].acc0;
+            fp.gcnt = ah.cnt_star;
+            fp.flags = ah.flags;
+            fp.rows_passed = f->host.rows_passed;
+            srd::k_frag_final_dense<SR_FINAL_ROWS><<<f->final_dense_grid, srd::GATHER_BLOCK, a->smem_bytes, ctx->stream>>>(fp, f->sel[cur].as<srd::SelEntry>(), cnt + k);
+        } else if (f->expand)
             srd::k_frag_gather_agg_expand<<<f->final_grid, srd::GATHER_BLOCK, 0, ctx->stream>>>(fdev, (const srd::AggDev*)a->dev.p, pass, vt,
                                                                                        f->sel[cur].as<srd::SelEntry>(), cnt + k, fail_list, fail_count);
         else if (ah.num_keys == 0)

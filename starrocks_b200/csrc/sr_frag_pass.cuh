@@ -36,9 +36,10 @@ struct PassDev {
     StreamTest tests[SR_MAX_STREAM_TESTS];
     int32_t num_stream_joins; // joins [0, num_stream_joins) are tested by the streaming pass
     int32_t final_first_join; // joins [final_first_join, S) are tested inline by the final pass
-    // fact columns the final pass reads: fetched for a row in one burst before anything depends on them
-    int8_t final_vals[8];              // value ids, -1 = unused
-    int8_t final_slot[SR_MAX_VALUES];  // value id -> index into final_vals, -1 = not prefetched
+    // fact columns the final pass reads (k_frag_final_dense loads all of them for a batch of rows before anything
+    // depends on them)
+    int8_t final_vals[8];  // value ids, -1 = unused
+    int8_t num_final_vals; // how many the final pass needs (may exceed 8: then only the generic final pass applies)
     int8_t host_input; // the fact columns of this push live in pinned host memory (SR_MEM_HOST_PINNED)
     // the int32 key of one streamed join whose build row the final pass needs travels in the upper half of the
     // selection-vector entries, so the final pass does not gather it from the fact table again
@@ -835,6 +836,251 @@ __global__ void __launch_bounds__(GATHER_BLOCK, SR_GATHER_AGG_MIN_BLOCKS) k_frag
     }
     passed = warp_sum(passed);
     if (lane_id() == 0 && passed) atomicAdd(fd.rows_passed, passed);
+}
+
+// ---- the final pass in batched form for dense star-join aggregates (k_frag_final_dense) ----
+// A SLOT-DIGIT DIRECTORY replaces the two dependent lookups first[key - min] -> payload[b] of a join whose payload
+// columns are only dense group keys: digit[key - min] is that join's share of the group slot, sum of idx_k * stride_k
+// over the group keys that are its payloads (idx_k as agg_find_slot computes it).  Two values are reserved: MISS (no
+// build row: the row fails the join) and BAD (a payload outside the declared range, or NULL where the key is not
+// nullable: the row passes, flags[1] is set, nothing is aggregated -- what agg_find_slot does).  2 bytes per key of
+// the range, half of first[].
+#define SR_DIGIT_MISS 0xFFFFu
+#define SR_DIGIT_BAD 0xFFFEu
+
+// one group key a directory folds in: a payload column of the join, read at the build row
+struct DigitKey {
+    const void* data;
+    const uint8_t* nulls;
+    int32_t type;
+    int32_t nullable;
+    long long min, extent, stride;
+};
+struct DigitPlan {
+    int32_t num_keys;
+    int32_t pad;
+    DigitKey k[SR_MAX_GROUP_KEYS];
+};
+
+__global__ void __launch_bounds__(256) k_frag_build_digits(const uint32_t* __restrict__ first, int64_t n, const __grid_constant__ DigitPlan dp,
+                                                           uint16_t* __restrict__ digit) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+        const uint32_t b = first[i];
+        if (b == 0) {
+            digit[i] = (uint16_t)SR_DIGIT_MISS;
+            continue;
+        }
+        long long slot = 0;
+        bool bad = false;
+#pragma unroll
+        for (int k = 0; k < SR_MAX_GROUP_KEYS; k++) {
+            if (k < dp.num_keys) {
+                const DigitKey& d = dp.k[k];
+                long long idx = 0;
+                if (d.nulls != nullptr && d.nulls[b] != 0) {
+                    bad |= !d.nullable;
+                } else {
+                    const int64_t v = load_int(d.data, d.type, b);
+                    idx = v - d.min + d.nullable;
+                    bad |= (v < d.min) || (idx >= d.extent);
+                }
+                slot += idx * d.stride;
+            }
+        }
+        digit[i] = (uint16_t)(bad ? SR_DIGIT_BAD : (uint32_t)slot);
+    }
+}
+
+constexpr int FINAL_MAX_VALS = 6;  // fact columns loaded per row
+constexpr int FINAL_MAX_LOOK = 2;  // joins looked up through a directory
+constexpr int FINAL_MAX_TEST = 2;  // joins only tested (bitmap)
+constexpr int FINAL_MAX_FKEYS = 2; // group keys that are fact columns
+constexpr int FINAL_MAX_FNS = 4;   // aggregate functions other than COUNT(*)
+// R = 4 rows per lane and batch, three CTAs of 256 threads per SM: 66 registers, no spills (sm_90a).  Four CTAs cap the
+// registers at 64 and spill.
+#ifndef SR_FINAL_ROWS
+#define SR_FINAL_ROWS 4
+#endif
+#ifndef SR_FINAL_MIN_BLOCKS
+#define SR_FINAL_MIN_BLOCKS 3
+#endif
+
+// Everything k_frag_final_dense reads, in one kernel parameter (the constant bank): no shared descriptor copies, no
+// per-row descriptor loads.  `val` fields index the fact values of `cols`.
+struct FinalDense {
+    int32_t num_vals, carry_val; // carry_val: index of the value the selection-vector entries carry, -1 = none
+    const int32_t* cols[FINAL_MAX_VALS];
+    int32_t num_look, num_test, num_fkeys, num_fns;
+    struct Look {
+        const uint16_t* digit;
+        uint32_t lo, span; // directory index = key - lo, valid when <= span
+        int32_t val, pad;
+    } look[FINAL_MAX_LOOK];
+    struct Test {
+        const uint32_t* bitmap;
+        uint32_t lo, span;
+        int32_t val, pad;
+    } test[FINAL_MAX_TEST];
+    struct FKey {
+        long long lo;     // dense_min
+        long long span;   // non-NULL values of the declared range
+        uint32_t base;    // 1 when the key is nullable (index 0 is NULL)
+        uint32_t stride;
+        int32_t val, pad;
+    } fkey[FINAL_MAX_FKEYS];
+    struct Fn {
+        long long* gacc; // global acc0
+        int32_t mode;
+        int32_t val;      // -1 for COUNT (a plain fact column is never NULL)
+        int32_t smem_off; // long-long offset of its accumulators in shared memory
+        int32_t pad;
+    } fn[FINAL_MAX_FNS];
+    int32_t cap, pad;
+    long long* gcnt;
+    int32_t* flags;
+    unsigned long long* rows_passed;
+};
+
+// v[idx] for a warp-uniform idx without indexing the register array (a select chain, no local memory)
+__device__ __forceinline__ int32_t final_pick(const int32_t (&v)[FINAL_MAX_VALS], int32_t idx) {
+    int32_t x = 0;
+#pragma unroll
+    for (int k = 0; k < FINAL_MAX_VALS; k++)
+        if (k == idx) x = v[k];
+    return x;
+}
+
+__device__ __forceinline__ uint32_t ldg_u16_pred(const uint16_t* p, bool pred, uint32_t other) {
+    uint16_t r;
+    asm volatile(
+            "{ .reg .pred q; setp.ne.u32 q, %2, 0; mov.u16 %0, %3;\n"
+            "  @q ld.global.nc.u16 %0, [%1]; }"
+            : "=h"(r)
+            : "l"(p), "r"((uint32_t)pred), "h"((uint16_t)other));
+    return r;
+}
+
+// Final pass for the shape of a star join into a dense shared-memory aggregate: every join the pass looks up has a
+// slot-digit directory, every other join it handles is a bitmap test, every aggregate input is one plain int32 fact
+// column in an integer mode.  A warp takes 32 x R consecutive selection-vector entries per iteration (lane l: entries
+// base + l + 32 r, so each read of the vector is coalesced) and runs them in three phases: (1) every fact load of the
+// R rows, (2) every directory load and bitmap test, (3) the shared-memory updates.  Against k_frag_gather_agg a row
+// waits on two round trips instead of ~8 in a row, and R rows overlap theirs.
+template <int R>
+__global__ void __launch_bounds__(GATHER_BLOCK, SR_FINAL_MIN_BLOCKS) k_frag_final_dense(const __grid_constant__ FinalDense fp, const SelEntry* __restrict__ sel_in,
+                                                                                        const unsigned long long* __restrict__ n_in_ptr) {
+    extern __shared__ __align__(16) uint32_t smem[];
+    long long* const acc = (long long*)smem;
+    const int cap = fp.cap;
+    for (int i = threadIdx.x; i < cap; i += blockDim.x) {
+        acc[i] = 0;
+#pragma unroll
+        for (int f = 0; f < FINAL_MAX_FNS; f++)
+            if (f < fp.num_fns) acc[fp.fn[f].smem_off + i] = acc_init_value(fp.fn[f].mode);
+    }
+    __syncthreads();
+    const unsigned long long n_in = *n_in_ptr;
+    unsigned long long w_begin, w_end;
+    warp_sel_range(n_in, w_begin, w_end);
+    uint32_t passed = 0;
+    bool any_bad = false;
+    for (unsigned long long i0 = w_begin + lane_id(); i0 < w_end; i0 += 32 * R) {
+        uint32_t row[R];
+        int32_t carry[R];
+        uint32_t live = 0;
+#pragma unroll
+        for (int r = 0; r < R; r++) {
+            const unsigned long long i = i0 + 32 * r;
+            const SelEntry e = i < w_end ? sel_in[i] : (SelEntry)SEL_INVALID;
+            row[r] = sel_row(e);
+            carry[r] = sel_carry(e);
+            live |= (row[r] != SEL_INVALID ? 1u : 0u) << r;
+        }
+        // phase 1: every fact value of every row
+        int32_t v[R][FINAL_MAX_VALS];
+#pragma unroll
+        for (int k = 0; k < FINAL_MAX_VALS; k++) {
+#pragma unroll
+            for (int r = 0; r < R; r++) {
+                v[r][k] = 0;
+                if (k < fp.num_vals) v[r][k] = k == fp.carry_val ? carry[r] : ldg_stream_s32_pred(fp.cols[k] + row[r], (live >> r) & 1u);
+            }
+        }
+        // phase 2: directory words and bitmap words
+        uint32_t dg[R][FINAL_MAX_LOOK];
+        uint32_t tw[R][FINAL_MAX_TEST];
+#pragma unroll
+        for (int L = 0; L < FINAL_MAX_LOOK; L++) {
+#pragma unroll
+            for (int r = 0; r < R; r++) {
+                dg[r][L] = 0;
+                if (L < fp.num_look) {
+                    const uint32_t idx = (uint32_t)final_pick(v[r], fp.look[L].val) - fp.look[L].lo;
+                    dg[r][L] = ldg_u16_pred(fp.look[L].digit + idx, ((live >> r) & 1u) && idx <= fp.look[L].span, SR_DIGIT_MISS);
+                }
+            }
+        }
+#pragma unroll
+        for (int t = 0; t < FINAL_MAX_TEST; t++) {
+#pragma unroll
+            for (int r = 0; r < R; r++) {
+                tw[r][t] = 0;
+                if (t < fp.num_test) {
+                    const uint32_t idx = (uint32_t)final_pick(v[r], fp.test[t].val) - fp.test[t].lo;
+                    tw[r][t] = ldg_u32_pred(fp.test[t].bitmap + (idx >> 5), ((live >> r) & 1u) && idx <= fp.test[t].span);
+                    tw[r][t] = (tw[r][t] >> (idx & 31)) & 1u;
+                }
+            }
+        }
+        // phase 3: join verdicts, group slot, shared-memory update
+#pragma unroll
+        for (int r = 0; r < R; r++) {
+            bool ok = (live >> r) & 1u;
+            bool bad = false;
+            uint32_t slot = 0;
+#pragma unroll
+            for (int L = 0; L < FINAL_MAX_LOOK; L++) {
+                if (L < fp.num_look) {
+                    ok &= dg[r][L] != SR_DIGIT_MISS;
+                    bad |= dg[r][L] == SR_DIGIT_BAD;
+                    slot += dg[r][L];
+                }
+            }
+#pragma unroll
+            for (int t = 0; t < FINAL_MAX_TEST; t++)
+                if (t < fp.num_test) ok &= tw[r][t] != 0;
+#pragma unroll
+            for (int k = 0; k < FINAL_MAX_FKEYS; k++) {
+                if (k < fp.num_fkeys) {
+                    const long long idx = (long long)final_pick(v[r], fp.fkey[k].val) - fp.fkey[k].lo;
+                    bad |= (unsigned long long)idx >= (unsigned long long)fp.fkey[k].span;
+                    slot += ((uint32_t)idx + fp.fkey[k].base) * fp.fkey[k].stride;
+                }
+            }
+            if (!ok) continue;
+            passed++;
+            if (bad) {
+                any_bad = true;
+                continue;
+            }
+            smem_add_u64(acc + slot, 1ull);
+#pragma unroll
+            for (int f = 0; f < FINAL_MAX_FNS; f++)
+                if (f < fp.num_fns) acc_apply_shared(fp.fn[f].mode, acc + fp.fn[f].smem_off, nullptr, slot, (long long)final_pick(v[r], fp.fn[f].val));
+        }
+    }
+    if (any_bad) fp.flags[1] = 1;
+    __syncthreads();
+    for (int i = threadIdx.x; i < cap; i += blockDim.x) {
+        const long long c = acc[i];
+        if (c == 0) continue;
+        atomicAdd((unsigned long long*)fp.gcnt + i, (unsigned long long)c);
+#pragma unroll
+        for (int f = 0; f < FINAL_MAX_FNS; f++)
+            if (f < fp.num_fns) acc_merge(fp.fn[f].mode, fp.fn[f].gacc, nullptr, i, acc[fp.fn[f].smem_off + i], 0);
+    }
+    const unsigned long long total = warp_sum((unsigned long long)passed);
+    if (lane_id() == 0 && total) atomicAdd(fp.rows_passed, total);
 }
 
 // Final pass of a fragment with one-to-many joins (reference: JoinHashMap::_probe_from_ht one-to-many walk,

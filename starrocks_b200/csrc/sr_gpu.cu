@@ -1360,6 +1360,7 @@ int32_t sr_fragment_get_plan(sr_fragment* frag, sr_fragment_plan* plan) {
     plan->num_stream_joins = frag->selective ? frag->pass.num_stream_joins : 0;
     plan->num_gather_passes = frag->selective ? (int32_t)frag->gather_joins.size() : 0;
     plan->pred_rate = frag->pred_rate;
+    plan->final_pass = frag->final_pass;
     if (frag->selective) {
         plan->smem_bytes = (int32_t)frag->stream_smem;
         plan->grid = frag->stream_grid;

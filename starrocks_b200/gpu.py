@@ -574,7 +574,7 @@ class Fragment:
                 "block": p.block, "agg_in_smem": bool(p.agg_in_smem),
                 "mode": {1: "fused-cascade", 2: "selection-vector-passes"}.get(p.mode, p.mode),
                 "num_stream_joins": p.num_stream_joins, "num_gather_passes": p.num_gather_passes,
-                "pred_rate": round(p.pred_rate, 4)}
+                "final_pass": abi.FINAL_PASS_NAMES.get(p.final_pass, p.final_pass), "pred_rate": round(p.pred_rate, 4)}
 
     @property
     def rows_passed(self):
