@@ -1442,11 +1442,9 @@ static int32_t agg_push_vtab(sr_agg* a, const VTab& vt, int64_t n) {
     }
     // hash mode
     {
-        // tuning knobs (also let the tests reach the partitioned path with small inputs)
+        // test hook: SR_AGG_PARTITION_MIN_ROWS lets the tests reach the partitioned push with small inputs
         const char* e_rows = getenv("SR_AGG_PARTITION_MIN_ROWS");
-        const char* e_table = getenv("SR_AGG_PARTITION_MIN_TABLE_BYTES");
         const int64_t min_rows = e_rows ? atoll(e_rows) : kPartitionedMinRows;
-        (void)e_table;
         bool merge_fns = false; // the staged records of the partitioned push carry one value per function, not (sum, count)
         for (int f = 0; f < h.num_fns; f++) merge_fns |= h.fns[f].n_value_id >= 0;
         if (!merge_fns && n >= min_rows) return agg_push_partitioned(a, vt, n, fresh);

@@ -91,10 +91,6 @@ static int32_t aggp_apply_l2_drain(sr_agg* a, const srd::PartPlan& pl, const uns
 static int32_t agg_push_partitioned(sr_agg* a, const VTab& vt, int64_t n, bool fresh) {
     sr_ctx* ctx = a->ctx;
     int64_t done = 0;
-    const bool trace = getenv("SR_AGG_TRACE") != nullptr; // phase times (CUDA events) on stderr
-    cudaEvent_t tev[4] = {nullptr, nullptr, nullptr, nullptr};
-    if (trace)
-        for (auto& e : tev) SR_CUDA(ctx, cudaEventCreate(&e));
     while (done < n) {
         const srd::AggDev& h = a->host;
         const int64_t m = std::min<int64_t>(n - done, kPartitionedMaxRows); // bounded by the staging buffers
@@ -151,6 +147,8 @@ static int32_t agg_push_partitioned(sr_agg* a, const VTab& vt, int64_t n, bool f
         while ((1 << log2nw) < nw) log2nw++;
         const size_t apply_smem = ((size_t)nw << srd::AGGP_SLICE_LOG2) * slot_bytes;
         const int bucket_log2 = srd::AGGP_SLICE_LOG2 + log2nw;
+        // test hook: SR_AGG_PARTITION_FORCE_L2 takes the global-atomics plan, which otherwise only tables of more buckets
+        // than two scatter levels address (hundreds of millions of slots) reach
         const bool smem_mode = log2cap > bucket_log2 && log2cap - bucket_log2 <= 2 * srd::AGGP_MAX_FAN_BITS && apply_smem <= 200 * 1024 &&
                                h.slice_log2 == srd::AGGP_SLICE_LOG2 && !getenv("SR_AGG_PARTITION_FORCE_L2");
         pl.apply_slices = nw;
@@ -166,7 +164,6 @@ static int32_t agg_push_partitioned(sr_agg* a, const VTab& vt, int64_t n, bool f
             pl.bucket_shift = log2cap - log2p;
         }
         pl.bits2 = pl.bits > srd::AGGP_MAX_FAN_BITS ? pl.bits / 2 : 0;
-        if (pl.bits2 && getenv("SR_AGG_BITS2")) pl.bits2 = std::min(std::max(atoi(getenv("SR_AGG_BITS2")), pl.bits - srd::AGGP_MAX_FAN_BITS), srd::AGGP_MAX_FAN_BITS); // tuning knob
         const int P = 1 << pl.bits;
         const int F1 = 1 << (pl.bits - pl.bits2);
         pl.cap2 = aggp_region_cap((double)m / P);
@@ -186,7 +183,6 @@ static int32_t agg_push_partitioned(sr_agg* a, const VTab& vt, int64_t n, bool f
         unsigned long long* ovf_count = a->counters.as<unsigned long long>() + 5;
         const srd::AggDev* dev = (const srd::AggDev*)a->dev.p;
         const int grid2 = ctx->num_sms * 2;
-        if (trace) SR_CUDA(ctx, cudaEventRecord(tev[0], ctx->stream));
         SR_CUDA(ctx, cudaMemsetAsync(cursor, 0, sizeof(uint32_t) * ((size_t)P + F1), ctx->stream));
         SR_CUDA(ctx, cudaMemsetAsync(fail_count, 0, 16, ctx->stream));
         srd::ScatterArgs sa;
@@ -196,9 +192,7 @@ static int32_t agg_push_partitioned(sr_agg* a, const VTab& vt, int64_t n, bool f
         sa.ovf = a->part_ovf.as<unsigned long long>();
         sa.ovf_count = ovf_count;
         sa.ovf_cap = (unsigned long long)m;
-        static const bool no_prefetch = getenv("SR_AGG_NO_L2_PREFETCH") != nullptr; // A/B switch of the next-tile L2 prefetch
-        sa.l2_prefetch = no_prefetch ? 0 : 1;
-        sa.pad = 0;
+        sa.l2_prefetch = 1;
         if (pl.bits2 == 0) {
             sa.cursor = cursor;
             sa.dst = rec_final;
@@ -206,7 +200,6 @@ static int32_t agg_push_partitioned(sr_agg* a, const VTab& vt, int64_t n, bool f
             sa.fan_bits = pl.bits;
             sa.local_shift = 0;
             SR_TRY(aggp_scatter(ctx, true, grid2, dev, vt, pl, sa));
-            if (trace) SR_CUDA(ctx, cudaEventRecord(tev[1], ctx->stream));
         } else {
             sa.cursor = cursor1;
             sa.dst = rec_mid;
@@ -214,7 +207,6 @@ static int32_t agg_push_partitioned(sr_agg* a, const VTab& vt, int64_t n, bool f
             sa.fan_bits = pl.bits - pl.bits2;
             sa.local_shift = pl.bits2;
             SR_TRY(aggp_scatter(ctx, true, grid2, dev, vt, pl, sa));
-            if (trace) SR_CUDA(ctx, cudaEventRecord(tev[1], ctx->stream));
             srd::k_aggp_tiles<<<1, 1024, 0, ctx->stream>>>(cursor1, F1, pl.cap1, tile_rows, a->part_tiles.as<uint32_t>());
             SR_LAUNCH_CHECK(ctx);
             sa.src = rec_mid;
@@ -227,7 +219,6 @@ static int32_t agg_push_partitioned(sr_agg* a, const VTab& vt, int64_t n, bool f
             sa.local_shift = 0;
             SR_TRY(aggp_scatter(ctx, false, grid2, dev, vt, pl, sa));
         }
-        if (trace) SR_CUDA(ctx, cudaEventRecord(tev[2], ctx->stream));
         uint64_t failed_buckets = 0, overflowed = 0;
         if (smem_mode) {
             SR_TRY(a->part_fail.reserve(ctx, sizeof(uint32_t) * (size_t)P));
@@ -245,20 +236,11 @@ static int32_t agg_push_partitioned(sr_agg* a, const VTab& vt, int64_t n, bool f
             SR_LAUNCH_CHECK(ctx);
         }
         fresh = false;
-        if (trace) SR_CUDA(ctx, cudaEventRecord(tev[3], ctx->stream));
         SR_CUDA(ctx, cudaMemcpyAsync(ctx->pinned + 8, a->counters.p, 48, cudaMemcpyDeviceToHost, ctx->stream));
         SR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
         a->ngroups_host = (int64_t)ctx->pinned[8];
         failed_buckets = ctx->pinned[8 + 4];
         overflowed = std::min<uint64_t>(ctx->pinned[8 + 5], (uint64_t)m);
-        if (trace) {
-            float t[3];
-            for (int k = 0; k < 3; k++) cudaEventElapsedTime(&t[k], tev[k], tev[k + 1]);
-            fprintf(stderr, "[sr_agg partitioned push] rows %lld, %d-word records, 2^%d buckets (%d + %d bits) of %d slices, regions of %llu / %llu records: scatter %.3f ms, "
-                            "scatter-2 %.3f ms, apply %.3f ms (%s), %llu buckets handed back, %llu records overflowed\n",
-                    (long long)m, pl.words, pl.bits, pl.bits - pl.bits2, pl.bits2, nw, (unsigned long long)pl.cap1, (unsigned long long)pl.cap2, t[0], t[1], t[2],
-                    smem_mode ? "shared-memory slices" : "global atomics follow", (unsigned long long)failed_buckets, (unsigned long long)overflowed);
-        }
         SR_CUDA(ctx, cudaMemsetAsync(fail_count, 0, 8, ctx->stream));
         if (!smem_mode || failed_buckets > 0 || overflowed > 0) SR_TRY(a->part_fail64.reserve(ctx, sizeof(uint64_t) * (size_t)m));
         if (!smem_mode || failed_buckets > 0) {
@@ -305,7 +287,5 @@ static int32_t agg_push_partitioned(sr_agg* a, const VTab& vt, int64_t n, bool f
         a->partitioned_pushes++;
         done += m;
     }
-    if (trace)
-        for (auto& e : tev) cudaEventDestroy(e);
     return SR_OK;
 }

@@ -55,9 +55,7 @@ __host__ __device__ inline bool is_decimal(int32_t t) {
 }
 
 // streaming loads: fact columns are read once -> bypass L1 allocation, keep L1/L2 for tables
-#ifndef SR_LD_HINT
 #define SR_LD_HINT ".L1::no_allocate"
-#endif
 __device__ __forceinline__ int4 ldg_stream_v4(const void* p) {
     int4 r;
     asm volatile("ld.global.nc" SR_LD_HINT ".v4.s32 {%0,%1,%2,%3}, [%4];"

@@ -328,9 +328,9 @@ static int32_t frag_plan_final_dense(sr_fragment* f) {
         fp.look[L].digit = f->digits[q].as<uint16_t>();
     }
     const size_t smem = f->agg->smem_bytes;
-    SR_CUDA(ctx, cudaFuncSetAttribute(srd::k_frag_final_dense<SR_FINAL_ROWS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(smem, 16)));
+    SR_CUDA(ctx, cudaFuncSetAttribute(srd::k_frag_final_dense<srd::FINAL_ROWS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(smem, 16)));
     int per_sm = 0;
-    SR_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, srd::k_frag_final_dense<SR_FINAL_ROWS>, srd::GATHER_BLOCK, smem));
+    SR_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, srd::k_frag_final_dense<srd::FINAL_ROWS>, srd::GATHER_BLOCK, smem));
     f->final_dense_grid = std::max(per_sm, 1) * ctx->num_sms;
     f->final_dense_ok = true;
     return SR_OK;
@@ -608,16 +608,7 @@ static int32_t frag_push(sr_fragment* f, const sr_chunk_view* fact) {
             const VDesc& d = vt.v[pass.tests[t].value_id];
             if (d.nulls != nullptr || (t < pass.num_vec && (((uintptr_t)d.data) & 15) != 0)) tests = false;
         }
-        static const bool use_tma = getenv("SR_FRAG_STREAM_TMA") != nullptr; // experiment: TMA-staged vector columns
-        if (tests && use_tma && !pass.host_input) {
-            const uint32_t bitmap_bytes = (uint32_t)((f->stream_smem + 127) / 128 * 128);
-            const size_t sm = bitmap_bytes + srd::STREAM_TMA_SMEM;
-            SR_CUDA(ctx, cudaFuncSetAttribute(srd::k_frag_stream_tests_tma<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
-            int per_sm = 1;
-            SR_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, srd::k_frag_stream_tests_tma<false>, srd::STREAM_BLOCK, sm));
-            const int tgrid = (int)std::min<int64_t>((int64_t)std::max(per_sm, 1) * ctx->num_sms, (n + srd::STREAM_TILE - 1) / srd::STREAM_TILE);
-            srd::k_frag_stream_tests_tma<false><<<tgrid, srd::STREAM_BLOCK, sm, ctx->stream>>>(fdev, pass, vt, n, bitmap_bytes, f->sel[0].as<srd::SelEntry>(), cnt);
-        } else if (tests) {
+        if (tests) {
             if (carry)
                 srd::k_frag_stream_tests<true><<<sgrid, srd::STREAM_BLOCK, f->stream_smem, ctx->stream>>>(fdev, pass, vt, n, f->sel[0].as<srd::SelEntry>(), cnt);
             else
@@ -656,7 +647,7 @@ static int32_t frag_push(sr_fragment* f, const sr_chunk_view* fact) {
             fp.gcnt = ah.cnt_star;
             fp.flags = ah.flags;
             fp.rows_passed = f->host.rows_passed;
-            srd::k_frag_final_dense<SR_FINAL_ROWS><<<f->final_dense_grid, srd::GATHER_BLOCK, a->smem_bytes, ctx->stream>>>(fp, f->sel[cur].as<srd::SelEntry>(), cnt + k);
+            srd::k_frag_final_dense<srd::FINAL_ROWS><<<f->final_dense_grid, srd::GATHER_BLOCK, a->smem_bytes, ctx->stream>>>(fp, f->sel[cur].as<srd::SelEntry>(), cnt + k);
         } else if (f->expand)
             srd::k_frag_gather_agg_expand<<<f->final_grid, srd::GATHER_BLOCK, 0, ctx->stream>>>(fdev, (const srd::AggDev*)a->dev.p, pass, vt,
                                                                                        f->sel[cur].as<srd::SelEntry>(), cnt + k, fail_list, fail_count);

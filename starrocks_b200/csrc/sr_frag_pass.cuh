@@ -119,11 +119,7 @@ __device__ __forceinline__ uint32_t join_test_batch(const FragJoinDev& fj, const
             for (int i = 0; i < N; i++) {
                 const uint32_t idx = (uint32_t)keys[i] - umin;
                 const bool p = ((alive >> i) & 1u) && idx <= span;
-#ifdef SR_EXPERIMENT_FAKE_SMEM
-                words[i] = p ? smem[(idx >> 5) & 4095u] : 0u; // timing experiment only: WRONG results
-#else
                 words[i] = ldg_u32_pred(fj.j.bitmap + (idx >> 5), p);
-#endif
             }
 #pragma unroll
             for (int i = 0; i < N; i++) {
@@ -349,7 +345,8 @@ __global__ void __launch_bounds__(STREAM_BLOCK, 2) k_frag_stream(const FragDev* 
 // streamed joins.  The columns of the first one or two tests are read with 128-bit loads prefetched a tile ahead (most
 // of their sectors are needed anyway); every later test loads its column only for the rows still alive (predicated
 // loads, issued back to back).  The host picks this kernel when every test column is int32-class and not nullable
-// (frag_push); anything else takes the generic path of k_frag_stream.
+// (frag_push); anything else takes the generic path of k_frag_stream.  (Staging the vector columns in shared memory with
+// cp.async.bulk instead buys nothing: the pass is issue bound, and every key then costs a shared-memory load as well.)
 template <int N>
 __device__ __forceinline__ uint32_t stream_test(const StreamTest& st, const FragJoinDev* s_joins, const uint32_t* smem, const int32_t (&k)[N], uint32_t alive) {
     if (st.kind == 0) {
@@ -536,158 +533,6 @@ __global__ void __launch_bounds__(STREAM_BLOCK, 2) k_frag_stream_tests(const Fra
     writer.finish();
 }
 
-// ---- the same pass with the vector columns staged by the TMA engine (north_star: "TMA-staged into shared memory") ----
-// The tile's two vector columns (STREAM_TILE x 4 bytes each) are fetched with cp.async.bulk (1-D bulk copy, SASS UBLKCP)
-// into a two-stage ring in shared memory, completion signalled through an mbarrier (complete_tx::bytes); the threads read
-// their eight keys per column with 128-bit shared loads and release the stage through a second mbarrier, on which thread 0
-// waits before it issues the copy of tile + 2.  The register prefetch of k_frag_stream_tests and its LDG.128 / L1TEX tag
-// traffic are gone; the price is 64 KB more shared memory per CTA and two shared loads per column.
-// Opt-in (SR_FRAG_STREAM_TMA=1): the pass is issue bound, so the LDG form stays the default.
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"((uint32_t)__cvta_generic_to_shared(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"((uint32_t)__cvta_generic_to_shared(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"((uint32_t)__cvta_generic_to_shared(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    asm volatile(
-            "{ .reg .pred p;\n"
-            "WAIT_%=:\n"
-            "  mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-            "  @p bra DONE_%=;\n"
-            "  bra WAIT_%=;\n"
-            "DONE_%=: }" ::"r"((uint32_t)__cvta_generic_to_shared(bar)),
-            "r"(parity)
-            : "memory");
-}
-__device__ __forceinline__ void tma_load_1d(void* smem_dst, const void* gmem_src, uint32_t bytes, uint64_t* bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"((uint32_t)__cvta_generic_to_shared(smem_dst)),
-                 "l"(gmem_src), "r"(bytes), "r"((uint32_t)__cvta_generic_to_shared(bar))
-                 : "memory");
-}
-
-constexpr int STREAM_TMA_STAGES = 2;
-constexpr size_t STREAM_TMA_SMEM = (size_t)STREAM_TMA_STAGES * 2 * STREAM_TILE * sizeof(int32_t);
-
-// smem: [bitmaps: bitmap_bytes][stage 0: col0 tile, col1 tile][stage 1: ...]; bitmap_bytes is a multiple of 16
-template <bool CARRY>
-__global__ void __launch_bounds__(STREAM_BLOCK, 2) k_frag_stream_tests_tma(const FragDev* __restrict__ fdp, PassDev pd, const __grid_constant__ VTab vt, int64_t n,
-                                                                           uint32_t bitmap_bytes, SelEntry* __restrict__ sel_out, unsigned long long* __restrict__ counter) {
-    extern __shared__ __align__(128) uint32_t smem_tma[];
-    uint32_t* const smem = smem_tma;
-    __shared__ FragJoinDev s_joins[STREAM_MAX_JOINS];
-    __shared__ StreamTest s_tests[SR_MAX_STREAM_TESTS];
-    __shared__ __align__(8) uint64_t s_full[STREAM_TMA_STAGES], s_empty[STREAM_TMA_STAGES];
-    const FragDev& fd = *fdp;
-    const int SJ = pd.num_stream_joins;
-    const int NT = pd.num_tests;
-    const int NV = pd.num_vec;
-    for (int i = threadIdx.x; i < (int)(sizeof(FragJoinDev) / 4) * SJ; i += blockDim.x) ((uint32_t*)s_joins)[i] = ((const uint32_t*)fd.joins)[i];
-    for (int i = threadIdx.x; i < (int)(sizeof(StreamTest) / 4) * NT; i += blockDim.x) ((uint32_t*)s_tests)[i] = ((const uint32_t*)pd.tests)[i];
-    for (int j = 0; j < SJ; j++) {
-        const FragJoinDev& fj = fd.joins[j];
-        if (fj.smem_off >= 0)
-            for (int w = threadIdx.x; w < fj.bitmap_words; w += blockDim.x) smem[fj.smem_off + w] = fj.j.bitmap[w];
-    }
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < STREAM_TMA_STAGES; s++) {
-            mbar_init(&s_full[s], 1);
-            mbar_init(&s_empty[s], STREAM_BLOCK);
-        }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
-    int32_t* const ring = (int32_t*)((uint8_t*)smem + bitmap_bytes);
-    const int32_t* col0 = (const int32_t*)vt.v[pd.tests[0].value_id].data;
-    const int32_t* col1 = NV > 1 ? (const int32_t*)vt.v[pd.tests[1].value_id].data : nullptr;
-    const int64_t num_tiles = (n + STREAM_TILE - 1) / STREAM_TILE;
-    const int64_t full_tiles = n / STREAM_TILE;
-    const int64_t tiles_per_cta = (num_tiles + gridDim.x - 1) / gridDim.x;
-    const int64_t tile_begin = (int64_t)blockIdx.x * tiles_per_cta;
-    const int64_t tile_end = tile_begin + tiles_per_cta < num_tiles ? tile_begin + tiles_per_cta : num_tiles;
-    const int64_t tma_end = tile_end < full_tiles ? tile_end : full_tiles; // full tiles only; the ragged tail uses predicated loads
-    const uint32_t col_bytes = STREAM_TILE * sizeof(int32_t);
-    auto issue = [&](int64_t tile) { // thread 0 only
-        const int s = (int)((tile - tile_begin) % STREAM_TMA_STAGES);
-        mbar_expect_tx(&s_full[s], col1 ? 2 * col_bytes : col_bytes);
-        tma_load_1d(ring + (size_t)s * 2 * STREAM_TILE, col0 + tile * STREAM_TILE, col_bytes, &s_full[s]);
-        if (col1) tma_load_1d(ring + (size_t)s * 2 * STREAM_TILE + STREAM_TILE, col1 + tile * STREAM_TILE, col_bytes, &s_full[s]);
-    };
-    if (threadIdx.x == 0)
-        for (int64_t t = tile_begin; t < tma_end && t < tile_begin + STREAM_TMA_STAGES; t++) issue(t);
-    WarpSelWriter writer;
-    writer.init(sel_out, counter);
-    for (int64_t tile = tile_begin; tile < tile_end; tile++) {
-        int64_t row0[STREAM_GROUPS];
-#pragma unroll
-        for (int g = 0; g < STREAM_GROUPS; g++)
-            row0[g] = tile * STREAM_TILE + (int64_t)g * (STREAM_BLOCK * STREAM_ROWS) + (int64_t)threadIdx.x * STREAM_ROWS;
-        int32_t carry[8];
-        if (CARRY) {
-#pragma unroll
-            for (int i = 0; i < 8; i++) carry[i] = 0;
-        }
-        uint32_t a8 = 0xFFu;
-        int first_pred = 0;
-        if (tile < tma_end) {
-            const int64_t li = tile - tile_begin;
-            const int s = (int)(li % STREAM_TMA_STAGES);
-            const uint32_t parity = (uint32_t)((li / STREAM_TMA_STAGES) & 1);
-            mbar_wait(&s_full[s], parity);
-            const int32_t* st0 = ring + (size_t)s * 2 * STREAM_TILE;
-            const int4 a0 = *(const int4*)(st0 + threadIdx.x * STREAM_ROWS), a1 = *(const int4*)(st0 + STREAM_BLOCK * STREAM_ROWS + threadIdx.x * STREAM_ROWS);
-            int4 b0 = make_int4(0, 0, 0, 0), b1 = make_int4(0, 0, 0, 0);
-            if (col1) {
-                b0 = *(const int4*)(st0 + STREAM_TILE + threadIdx.x * STREAM_ROWS);
-                b1 = *(const int4*)(st0 + STREAM_TILE + STREAM_BLOCK * STREAM_ROWS + threadIdx.x * STREAM_ROWS);
-            }
-            mbar_arrive(&s_empty[s]); // this thread has its keys in registers
-            if (threadIdx.x == 0 && tile + STREAM_TMA_STAGES < tma_end) {
-                mbar_wait(&s_empty[s], parity); // every thread has read the stage: refill it with tile + 2
-                issue(tile + STREAM_TMA_STAGES);
-            }
-            const int32_t k0[8] = {a0.x, a0.y, a0.z, a0.w, a1.x, a1.y, a1.z, a1.w};
-            const int32_t k1[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
-            a8 = stream_test<8>(s_tests[0], s_joins, smem, k0, 0xFFu);
-            if (CARRY && s_tests[0].kind == 1 && s_tests[0].join == pd.carry_join) {
-#pragma unroll
-                for (int i = 0; i < 8; i++) carry[i] = k0[i];
-            }
-            if (NV > 1) {
-                a8 = stream_test<8>(s_tests[1], s_joins, smem, k1, a8);
-                if (CARRY && s_tests[1].kind == 1 && s_tests[1].join == pd.carry_join) {
-#pragma unroll
-                    for (int i = 0; i < 8; i++) carry[i] = k1[i];
-                }
-            }
-            first_pred = NV;
-        } else { // the ragged last tile: every test through predicated loads
-            a8 = 0;
-#pragma unroll
-            for (int i = 0; i < 8; i++)
-                if (row0[i >> 2] + (i & 3) < n) a8 |= 1u << i;
-        }
-#pragma unroll 1
-        for (int t = first_pred; t < NT; t++) {
-            const StreamTest& st = s_tests[t];
-            const int32_t* col = (const int32_t*)vt.v[st.value_id].data;
-            int32_t kk[8];
-#pragma unroll
-            for (int i = 0; i < 8; i++) kk[i] = ldg_stream_s32_pred(col + row0[i >> 2] + (i & 3), (a8 >> i) & 1u);
-            a8 = stream_test<8>(st, s_joins, smem, kk, a8);
-            if (CARRY && st.kind == 1 && st.join == pd.carry_join) {
-#pragma unroll
-                for (int i = 0; i < 8; i++) carry[i] = kk[i];
-            }
-        }
-        warp_append_rows<CARRY>(a8, row0[0], row0[1], carry, writer);
-    }
-    writer.finish();
-}
-
 constexpr int GATHER_BLOCK = 256;
 
 // the contiguous run [begin, end) of a selection vector of n entries that the calling warp owns (a multiple
@@ -702,11 +547,6 @@ __device__ __forceinline__ void warp_sel_range(unsigned long long n, unsigned lo
     if (begin > n) begin = n;
 }
 
-// the final pass is a chain of dependent gathers per row: latency bound, so resident warps matter more than spills.
-// Five CTAs per SM (48 registers) balance resident warps against spills.
-#ifndef SR_GATHER_AGG_MIN_BLOCKS
-#define SR_GATHER_AGG_MIN_BLOCKS 5
-#endif
 // one selective join on the selected rows: sel_in[0, *n_in) -> sel_out (appended at *counter_out)
 __global__ void __launch_bounds__(GATHER_BLOCK) k_frag_gather_join(const FragDev* __restrict__ fdp, int32_t j, const __grid_constant__ VTab vt,
                                                                     const SelEntry* __restrict__ sel_in, const unsigned long long* __restrict__ n_in_ptr,
@@ -744,10 +584,14 @@ __global__ void __launch_bounds__(GATHER_BLOCK) k_frag_gather_join(const FragDev
     writer.finish();
 }
 
+// the final pass is a chain of dependent gathers per row: latency bound, so resident warps matter more than spills.
+// Five CTAs per SM (48 registers) balance resident warps against spills.
+constexpr int GATHER_AGG_MIN_BLOCKS = 5;
+
 // final pass: remaining joins inline, payload lookups, aggregate update.  SINGLE: no GROUP BY (its register state
 // would only cost the grouped instantiations spills).
 template <bool SMEM_AGG, bool SINGLE = false>
-__global__ void __launch_bounds__(GATHER_BLOCK, SR_GATHER_AGG_MIN_BLOCKS) k_frag_gather_agg(const FragDev* __restrict__ fdp, const AggDev* __restrict__ adp, const __grid_constant__ PassDev pd,
+__global__ void __launch_bounds__(GATHER_BLOCK, GATHER_AGG_MIN_BLOCKS) k_frag_gather_agg(const FragDev* __restrict__ fdp, const AggDev* __restrict__ adp, const __grid_constant__ PassDev pd,
                                                                    const __grid_constant__ VTab vt, const SelEntry* __restrict__ sel_in,
                                                                    const unsigned long long* __restrict__ n_in_ptr, SelEntry* __restrict__ fail_list,
                                                                    unsigned long long* __restrict__ fail_count) {
@@ -898,12 +742,8 @@ constexpr int FINAL_MAX_FKEYS = 2; // group keys that are fact columns
 constexpr int FINAL_MAX_FNS = 4;   // aggregate functions other than COUNT(*)
 // R = 4 rows per lane and batch, three CTAs of 256 threads per SM: 66 registers, no spills (sm_90a).  Four CTAs cap the
 // registers at 64 and spill.
-#ifndef SR_FINAL_ROWS
-#define SR_FINAL_ROWS 4
-#endif
-#ifndef SR_FINAL_MIN_BLOCKS
-#define SR_FINAL_MIN_BLOCKS 3
-#endif
+constexpr int FINAL_ROWS = 4;
+constexpr int FINAL_MIN_BLOCKS = 3;
 
 // Everything k_frag_final_dense reads, in one kernel parameter (the constant bank): no shared descriptor copies, no
 // per-row descriptor loads.  `val` fields index the fact values of `cols`.
@@ -967,7 +807,7 @@ __device__ __forceinline__ uint32_t ldg_u16_pred(const uint16_t* p, bool pred, u
 // R rows, (2) every directory load and bitmap test, (3) the shared-memory updates.  Against k_frag_gather_agg a row
 // waits on two round trips instead of ~8 in a row, and R rows overlap theirs.
 template <int R>
-__global__ void __launch_bounds__(GATHER_BLOCK, SR_FINAL_MIN_BLOCKS) k_frag_final_dense(const __grid_constant__ FinalDense fp, const SelEntry* __restrict__ sel_in,
+__global__ void __launch_bounds__(GATHER_BLOCK, FINAL_MIN_BLOCKS) k_frag_final_dense(const __grid_constant__ FinalDense fp, const SelEntry* __restrict__ sel_in,
                                                                                         const unsigned long long* __restrict__ n_in_ptr) {
     extern __shared__ __align__(16) uint32_t smem[];
     long long* const acc = (long long*)smem;

@@ -33,7 +33,7 @@ def _source_hash():
         h.update(os.path.basename(f).encode())
         with open(f, "rb") as fh:
             h.update(fh.read())
-    h.update(" ".join(NVCC_FLAGS + os.environ.get("SR_NVCC_EXTRA", "").split()).encode())
+    h.update(" ".join(NVCC_FLAGS).encode())
     return h.hexdigest()
 
 
@@ -42,7 +42,6 @@ def build(verbose=False):
     (the ranks of a torchrun job): one process compiles under a file lock into a temporary name and renames it into place."""
     import fcntl
     src = os.path.join(_HERE, "csrc", "sr_gpu.cu")
-    extra = os.environ.get("SR_NVCC_EXTRA", "").split()   # e.g. -DSR_EXPERIMENT_... for timing experiments
     want = _source_hash()
     with open(LIB_PATH + ".lock", "w") as lock:
         fcntl.flock(lock, fcntl.LOCK_EX)
@@ -50,7 +49,7 @@ def build(verbose=False):
             if not verbose and os.path.exists(LIB_PATH) and _recorded_hash() == want:
                 return LIB_PATH                     # another process built it while this one waited for the lock
             tmp = LIB_PATH + ".tmp.%d" % os.getpid()
-            cmd = ["nvcc"] + NVCC_FLAGS + extra + (["-Xptxas", "-v"] if verbose else []) + ["-o", tmp, src]
+            cmd = ["nvcc"] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-o", tmp, src]
             subprocess.check_call(cmd)
             os.replace(tmp, LIB_PATH)
             with open(LIB_PATH + ".srchash", "w") as fh:
