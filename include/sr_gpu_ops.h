@@ -704,16 +704,22 @@ int32_t sr_xchg_hash(sr_xchg* x, const sr_chunk_view* in, uint32_t* hash_values,
  *   FrameOfReferencePageDecoder::next_batch  be/src/storage/rowset/frame_of_reference_page.h:113-222
  *       (ForDecoder, be/src/util/frame_of_reference_coding.cpp:246-352)
  *   PlainPageDecoder::next_batch             be/src/storage/rowset/plain_page.h:135-260
+ * and, for every fixed-width type (widths 1, 2, 4, 8 and 16: BOOLEAN ... LARGEINT, FLOAT, DOUBLE, DECIMAL128 -- the decode
+ * moves bytes and does no arithmetic), the default encoding of those columns:
+ *   BitShufflePageDecoder::next_batch        be/src/storage/rowset/bitshuffle_page.h (bitshuffle + LZ4 blocks)
+ *   For BIT_SHUFFLE, `out` must be aligned to the value width (8 bytes for 16-byte values).
  * `pages`: the BODIES of consecutive data pages of one column (after the page's checksum / null-map handling of
  * page_io.cpp), all in `mem`: SR_MEM_DEVICE, SR_MEM_HOST_PINNED (page-locked mapped memory, e.g. a registered page cache:
  * read in place over PCIe, the decode is the transfer) or SR_MEM_HOST (pageable: staged page by page).  The values of page
  * k follow those of page k - 1 in `out` (device memory, room for out_capacity values); *out_rows receives the total.
- * SR_ERR_INVALID_ARGUMENT for a page that is not well formed (sizes, frame table, bit widths).  Asynchronous on the context
- * stream except for one small read-back of the per-page counts.  BIT_SHUFFLE (bitshuffle + LZ4), RLE and dictionary pages
- * are not covered: SR_ERR_NOT_SUPPORTED. */
+ * SR_ERR_INVALID_ARGUMENT for a page that is not well formed (sizes, frame table, bit widths, the bitshuffle header, block
+ * chain or LZ4 streams).  Asynchronous on the context stream except for one small read-back of the per-page counts and,
+ * for FOR and BIT_SHUFFLE, one of the error flag at the end.  RLE and dictionary pages are not covered:
+ * SR_ERR_NOT_SUPPORTED. */
 typedef enum sr_page_encoding {
-    SR_PAGE_PLAIN = 0, /* EncodingTypePB::PLAIN_ENCODING */
-    SR_PAGE_FOR = 1    /* EncodingTypePB::FOR_ENCODING */
+    SR_PAGE_PLAIN = 0,     /* EncodingTypePB::PLAIN_ENCODING */
+    SR_PAGE_FOR = 1,       /* EncodingTypePB::FOR_ENCODING */
+    SR_PAGE_BITSHUFFLE = 2 /* EncodingTypePB::BIT_SHUFFLE */
 } sr_page_encoding;
 
 typedef struct sr_page_view {

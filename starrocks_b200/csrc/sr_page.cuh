@@ -14,6 +14,22 @@
 // a block scan of 16 * bit_width + sizeof(T)), k_for_decode gives every frame to one warp: the packed bytes are copied to
 // shared memory with coalesced word loads, every lane extracts FOUR CONSECUTIVE values with 64-bit funnel arithmetic (at
 // most 9 bytes of the bit string each), ascending frames take a warp scan, and the lane stores its four values.
+//
+//   BitShufflePageDecoder        be/src/storage/rowset/bitshuffle_page.h (BitshufflePageBuilder::finish writes the page)
+// A bitshuffle page: a 16-byte header of four little-endian uint32s -- num_elements, compressed_size (the whole page, header
+// included), num_elements_after_padding = ALIGN_UP(num_elements, 8) (zero padding, never stored), elem_size_bytes -- then
+// bitshuffle::compress_lz4(values, padded, elem_size, block_size = 0): blocks of bshuf_default_block_size(s) = max(128,
+// (8192 / s) / 8 * 8) = 8192 / s elements (8192 bytes) for s = 1..16, the last one holding padded % block elements when
+// that is non-zero.  Each block is a BIG-endian uint32 compressed length, then one LZ4 block-format stream of the
+// bit-transposed block: 8 * s rows of elems / 8 bytes, row 8 * j + k holding bit k of byte j of every element (element i at
+// bit i % 8 of byte i / 8).  A stream claims at most LZ4_compressBound(8192) = 8240 bytes; the blocks end exactly at
+// compressed_size.  bshuf_oracle/bshuf_oracle.cpp restates the codec on the CPU, with the LZ4 end-of-block rules enforced
+// here (checked against liblz4's verdicts in tests/golden/bitshuffle_lz4.npz).
+// k_page_footers checks the header and counts the blocks, k_bshuf_blocks walks each page's chain of lengths into
+// per-block descriptors, and k_bshuf_decode gives every block to one warp: the compressed block is staged in shared memory
+// with coalesced word loads (in-place reads over PCIe move only the compressed bytes), the LZ4 sequences are parsed serially
+// (warp-uniform) into an 8 KB shared buffer with the literal and match bytes copied across the lanes, and every lane then
+// un-transposes 8 consecutive elements (one 8 x 8 bit transpose per byte position) and stores them.
 #pragma once
 
 namespace srd {
@@ -37,7 +53,10 @@ __device__ __forceinline__ uint32_t page_le32(const uint8_t* p) {
     return (uint32_t)p[0] | (uint32_t)p[1] << 8 | (uint32_t)p[2] << 16 | (uint32_t)p[3] << 24;
 }
 
-// value count and frame count of every page; flags[0] |= 1 when a page cannot be a frame-of-reference / plain page
+constexpr int BSHUF_BLOCK_BYTES = 8192;     // bshuf_default_block_size(s) * s for every width s in 1..16
+constexpr uint32_t BSHUF_MAX_STREAM = 8240; // LZ4_compressBound(8192)
+
+// value count and frame (bitshuffle: block) count of every page; flags[0] |= 1 when a page cannot be a page of `encoding`
 __global__ void __launch_bounds__(256) k_page_footers(const PageDesc* __restrict__ pages, int32_t num_pages, int32_t encoding, int32_t elem_size,
                                                        unsigned long long* __restrict__ counts /* [2 * num_pages]: values, frames */, int32_t* __restrict__ flags) {
     const int p = blockIdx.x * blockDim.x + threadIdx.x;
@@ -51,6 +70,15 @@ __global__ void __launch_bounds__(256) k_page_footers(const PageDesc* __restrict
         } else {
             n = page_le32(pg.data);
             if (pg.size != 4 + (long long)n * elem_size) bad = true;
+        }
+    } else if (encoding == SR_PAGE_BITSHUFFLE) {
+        if (pg.size < 16) {
+            bad = true;
+        } else {
+            n = page_le32(pg.data);
+            const unsigned long long padded = page_le32(pg.data + 8), blk = BSHUF_BLOCK_BYTES / elem_size;
+            if (page_le32(pg.data + 4) != (unsigned long long)pg.size || padded != ((n + 7) & ~7ull) || page_le32(pg.data + 12) != (uint32_t)elem_size) bad = true;
+            frames = (padded + blk - 1) / blk; // blocks
         }
     } else {
         if (pg.size < 5) {
@@ -222,6 +250,203 @@ __global__ void __launch_bounds__(256) k_plain_copy(const PageDesc* __restrict__
     }
 }
 
+struct BshufBlock {
+    const uint8_t* src; // the LZ4 stream (device-visible)
+    long long row;      // output row of the block's first element
+    uint32_t clen;      // stream bytes
+    uint32_t elems;     // elements the stream decodes to (a multiple of 8); 0: skip the block
+    uint32_t n_out;     // elements stored: the rest is padding
+    uint32_t reserved;
+};
+
+__device__ __forceinline__ uint32_t page_be32(const uint8_t* p) {
+    return (uint32_t)p[0] << 24 | (uint32_t)p[1] << 16 | (uint32_t)p[2] << 8 | (uint32_t)p[3];
+}
+
+// one thread per page (headers already checked by k_page_footers): the chain of big-endian block lengths -> descriptors at
+// the page's frame_off.  A chain that overruns the page, claims more than 8240 bytes for a block or does not end at
+// compressed_size raises the flag; blocks from the first bad length on are skipped.
+__global__ void __launch_bounds__(256) k_bshuf_blocks(const PageDesc* __restrict__ pages, int32_t num_pages, int32_t elem_size, BshufBlock* __restrict__ blocks,
+                                                       int32_t* __restrict__ flags) {
+    const int p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= num_pages) return;
+    const PageDesc pg = pages[p];
+    if (pg.size < 16) return;
+    const uint32_t n = page_le32(pg.data), padded = page_le32(pg.data + 8), blk = BSHUF_BLOCK_BYTES / elem_size;
+    const uint32_t nb = (uint32_t)(((unsigned long long)padded + blk - 1) / blk);
+    long long pos = 16;
+    bool bad = false;
+    for (uint32_t b = 0; b < nb; b++) {
+        BshufBlock d;
+        d.src = nullptr;
+        d.row = pg.row_off + (long long)b * blk;
+        d.clen = d.elems = d.n_out = d.reserved = 0;
+        if (!bad && pg.size - pos >= 4) {
+            const uint32_t c = page_be32(pg.data + pos);
+            if (c <= BSHUF_MAX_STREAM && c <= pg.size - pos - 4) {
+                d.src = pg.data + pos + 4;
+                d.clen = c;
+                d.elems = min(blk, padded - b * blk);
+                d.n_out = min(d.elems, n - b * blk); // n > b * blk: padding is < 8 elements and a block holds >= 8
+                pos += 4 + c;
+            } else {
+                bad = true;
+            }
+        } else {
+            bad = true;
+        }
+        blocks[pg.frame_off + b] = d;
+    }
+    if (bad || pos != pg.size) atomicOr(flags, 1);
+}
+
+// 8 x 8 bit matrix transpose: bit k of byte t <-> bit t of byte k (TRANS_BIT_8X8 of the bitshuffle sources)
+__device__ __forceinline__ unsigned long long bshuf_trans8x8(unsigned long long x) {
+    unsigned long long t;
+    t = (x ^ (x >> 7)) & 0x00AA00AA00AA00AAull;
+    x = x ^ t ^ (t << 7);
+    t = (x ^ (x >> 14)) & 0x0000CCCC0000CCCCull;
+    x = x ^ t ^ (t << 14);
+    t = (x ^ (x >> 28)) & 0x00000000F0F0F0F0ull;
+    x = x ^ t ^ (t << 28);
+    return x;
+}
+
+// an LZ4 length nibble of 15, continued in bytes (255: another follows); stops once it passes `limit` (the caller rejects)
+__device__ __forceinline__ bool lz4_len(const uint8_t* in, uint32_t n, uint32_t& ip, uint32_t& v, uint32_t limit) {
+    uint32_t b;
+    do {
+        if (ip >= n) return false;
+        b = in[ip++];
+        v += b;
+    } while (b == 255 && v <= limit);
+    return true;
+}
+
+constexpr int BSHUF_DECODE_WARPS = 2;                                // 2 x 16.1 KB of shared memory per CTA
+constexpr int BSHUF_STAGE_WORDS = (3 + (int)BSHUF_MAX_STREAM + 3) / 4; // the longest stream at the worst byte skew
+
+// one warp per block.  S: value width in bytes.  Every length and offset is checked against the staged input and the
+// block's output before it is used: a corrupt stream raises the flag and stores nothing.
+template <int S>
+__global__ void __launch_bounds__(BSHUF_DECODE_WARPS * 32) k_bshuf_decode(const BshufBlock* __restrict__ blocks, long long num_blocks, uint8_t* __restrict__ out,
+                                                                         int32_t* __restrict__ flags) {
+    __shared__ uint32_t s_in[BSHUF_DECODE_WARPS][BSHUF_STAGE_WORDS];
+    __shared__ uint8_t s_out[BSHUF_DECODE_WARPS][BSHUF_BLOCK_BYTES];
+    constexpr int Q = (S + 7) / 8; // 64-bit words per value
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    uint8_t* o = s_out[wid];
+    const long long stride = (long long)gridDim.x * BSHUF_DECODE_WARPS;
+    for (long long bi = (long long)blockIdx.x * BSHUF_DECODE_WARPS + wid; bi < num_blocks; bi += stride) {
+        const BshufBlock d = blocks[bi];
+        if (d.elems == 0) continue; // (warp-uniform)
+        // the stream -> shared memory: whole words from the aligned address below it (an aligned word never crosses a page
+        // of the host mapping), the byte skew remembered
+        const uintptr_t a0 = (uintptr_t)d.src & ~(uintptr_t)3;
+        const uint32_t skew = (uint32_t)((uintptr_t)d.src - a0);
+        const uint32_t nwords = (skew + d.clen + 3) / 4;
+        __syncwarp();
+        for (uint32_t i = lane; i < nwords; i += 32) s_in[wid][i] = (uint32_t)ldg_stream_s32((const uint32_t*)a0 + i);
+        __syncwarp();
+        const uint8_t* in = (const uint8_t*)s_in[wid] + skew;
+        // LZ4 block decode (the end-of-block rules of bshuf_oracle.cpp).  Control flow depends only on bytes every lane reads
+        // alike, so it is warp-uniform.
+        const uint32_t n = d.clen, E = d.elems * S;
+        uint32_t ip = 0, op = 0;
+        bool ok = false;
+        while (ip < n) {
+            const uint32_t tok = in[ip++];
+            uint32_t lit = tok >> 4;
+            if (lit == 15 && !lz4_len(in, n, ip, lit, n)) break;
+            if (lit > n - ip || lit > E - op) break;
+            for (uint32_t k = lane; k < lit; k += 32) o[op + k] = in[ip + k];
+            ip += lit;
+            op += lit;
+            if (ip == n) {
+                ok = op == E;
+                break;
+            }
+            if (op + 12 > E || n - ip < 2) break; // a match starts at least 12 bytes before the end
+            const uint32_t off = (uint32_t)in[ip] | (uint32_t)in[ip + 1] << 8;
+            ip += 2;
+            if (off == 0 || off > op) break;
+            uint32_t ml = tok & 15;
+            if (ml == 15 && !lz4_len(in, n, ip, ml, E)) break;
+            ml += 4;
+            if (ml + 5 > E - op) break; // ... and ends at least 5 bytes before it
+            __syncwarp();               // the bytes the match reads were written by other lanes
+            // out[op + k] = out[op - off + (k mod off)]: reads only bytes before op, also when the match overlaps itself
+            const uint32_t m0 = op - off;
+            if (off >= ml) {
+                for (uint32_t k = lane; k < ml; k += 32) o[op + k] = o[m0 + k];
+            } else {
+                for (uint32_t k = lane; k < ml; k += 32) o[op + k] = o[m0 + k % off];
+            }
+            op += ml;
+        }
+        if (!ok) {
+            if (lane == 0) atomicOr(flags, 1);
+            continue;
+        }
+        __syncwarp();
+        // un-transpose: lane takes elements [8g, 8g + 8); byte j of them = the 8 x 8 transpose of byte g of rows 8j .. 8j + 7
+        const uint32_t R = d.elems / 8;
+        uint8_t* dst = out + d.row * S;
+        for (uint32_t g = lane; g < R; g += 32) {
+            unsigned long long v[8][Q];
+#pragma unroll
+            for (int t = 0; t < 8; t++)
+#pragma unroll
+                for (int q = 0; q < Q; q++) v[t][q] = 0;
+#pragma unroll
+            for (int j = 0; j < S; j++) {
+                unsigned long long x = 0;
+#pragma unroll
+                for (int k = 0; k < 8; k++) x |= (unsigned long long)o[(8 * j + k) * R + g] << (8 * k);
+                x = bshuf_trans8x8(x);
+#pragma unroll
+                for (int t = 0; t < 8; t++) v[t][j / 8] |= ((x >> (8 * t)) & 0xFF) << (8 * (j % 8));
+            }
+            uint8_t* p = dst + (size_t)8 * g * S;
+            if (8 * g + 8 <= d.n_out && ((uintptr_t)p & 7) == 0) {
+                // the lane's 8 * S bytes as S little-endian 64-bit words; lanes are contiguous, so the warp's stores are too
+                unsigned long long w[S];
+#pragma unroll
+                for (int m = 0; m < S; m++) {
+                    if (S >= 8) {
+                        w[m] = v[m / Q][m % Q];
+                    } else {
+                        w[m] = 0;
+#pragma unroll
+                        for (int q = 0; q < 8 / S; q++) w[m] |= v[m * (8 / S) + q][0] << (8 * S * q);
+                    }
+                }
+                if (S >= 2 && ((uintptr_t)p & 15) == 0) {
+#pragma unroll
+                    for (int m = 0; m + 1 < S; m += 2) ((ulonglong2*)p)[m / 2] = make_ulonglong2(w[m], w[m + 1]);
+                } else {
+#pragma unroll
+                    for (int m = 0; m < S; m++) ((unsigned long long*)p)[m] = w[m];
+                }
+            } else {
+                // a partial group (the page's last), or a row offset that page boundaries left unaligned: value by value
+#pragma unroll
+                for (int t = 0; t < 8; t++) {
+                    if (8 * g + t >= d.n_out) break;
+                    uint8_t* e = p + t * S;
+                    if (S == 1) *e = (uint8_t)v[t][0];
+                    else if (S == 2) *(uint16_t*)e = (uint16_t)v[t][0];
+                    else if (S == 4) *(uint32_t*)e = (uint32_t)v[t][0];
+                    else {
+#pragma unroll
+                        for (int q = 0; q < Q; q++) ((unsigned long long*)e)[q] = v[t][q];
+                    }
+                }
+            }
+        }
+    }
+}
+
 } // namespace srd
 
 // host side ------------------------------------------------------------------------------------------------------------
@@ -233,8 +458,13 @@ struct PageScratch {
 static int32_t pages_decode(sr_ctx* ctx, PageScratch* sc, int32_t encoding, int32_t type, const sr_page_view* pv, int32_t num_pages, int32_t mem, void* out,
                             int64_t out_capacity, int64_t* out_rows) {
     const int w = srd::type_width(type);
-    if ((w != 4 && w != 8) || srd::is_float_class(type)) return sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "page decode of type %d (4- and 8-byte integer-class types)", type);
-    if (encoding != SR_PAGE_PLAIN && encoding != SR_PAGE_FOR) return sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "page encoding %d", encoding);
+    if (encoding == SR_PAGE_BITSHUFFLE) {
+        if (w == 0) return sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "bitshuffle page decode of type %d (fixed-width types)", type);
+        if ((uintptr_t)out % std::min(w, 8)) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "output column not aligned to %d bytes", std::min(w, 8));
+    } else {
+        if ((w != 4 && w != 8) || srd::is_float_class(type)) return sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "page decode of type %d (4- and 8-byte integer-class types)", type);
+        if (encoding != SR_PAGE_PLAIN && encoding != SR_PAGE_FOR) return sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "page encoding %d", encoding);
+    }
     if (num_pages < 0 || (num_pages > 0 && !pv)) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "pages");
     if (mem != SR_MEM_HOST && mem != SR_MEM_DEVICE && mem != SR_MEM_HOST_PINNED) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "unknown memory kind %d", mem);
     *out_rows = 0;
@@ -301,7 +531,8 @@ static int32_t pages_decode(sr_ctx* ctx, PageScratch* sc, int32_t encoding, int3
     SR_CUDA(ctx, cudaMemcpyAsync(hc, sc->counts.p, 16 * (size_t)num_pages, cudaMemcpyDeviceToHost, ctx->stream));
     SR_CUDA(ctx, cudaMemcpyAsync(hc + 2 * (size_t)num_pages, sc->flags.p, 8, cudaMemcpyDeviceToHost, ctx->stream));
     SR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    if (*(const int32_t*)(hc + 2 * (size_t)num_pages)) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "a page is not a well-formed %s page", encoding == SR_PAGE_FOR ? "frame-of-reference" : "plain");
+    if (*(const int32_t*)(hc + 2 * (size_t)num_pages))
+        return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "a page is not a well-formed %s page", encoding == SR_PAGE_FOR ? "frame-of-reference" : encoding == SR_PAGE_PLAIN ? "plain" : "bitshuffle");
     long long rows = 0, frames = 0;
     for (int p = 0; p < num_pages; p++) {
         hp[p].row_off = rows;
@@ -319,6 +550,27 @@ static int32_t pages_decode(sr_ctx* ctx, PageScratch* sc, int32_t encoding, int3
             srd::k_plain_copy<<<dim3(32, std::min(num_pages - p0, 65535)), 256, 0, ctx->stream>>>((const srd::PageDesc*)sc->pages.p + p0, w, (uint8_t*)out);
             SR_LAUNCH_CHECK(ctx);
         }
+        return SR_OK;
+    }
+    if (encoding == SR_PAGE_BITSHUFFLE) {
+        SR_TRY(sc->frames.reserve(ctx, sizeof(srd::BshufBlock) * (size_t)frames));
+        srd::BshufBlock* blocks = (srd::BshufBlock*)sc->frames.p;
+        srd::k_bshuf_blocks<<<grid_for(num_pages, 256), 256, 0, ctx->stream>>>((const srd::PageDesc*)sc->pages.p, num_pages, w, blocks, (int32_t*)sc->flags.p);
+        SR_LAUNCH_CHECK(ctx);
+        const int bgrid = (int)std::min<long long>((frames + srd::BSHUF_DECODE_WARPS - 1) / srd::BSHUF_DECODE_WARPS, (long long)ctx->num_sms * 8);
+        int32_t* flags = (int32_t*)sc->flags.p;
+        switch (w) {
+        case 1: srd::k_bshuf_decode<1><<<bgrid, srd::BSHUF_DECODE_WARPS * 32, 0, ctx->stream>>>(blocks, frames, (uint8_t*)out, flags); break;
+        case 2: srd::k_bshuf_decode<2><<<bgrid, srd::BSHUF_DECODE_WARPS * 32, 0, ctx->stream>>>(blocks, frames, (uint8_t*)out, flags); break;
+        case 4: srd::k_bshuf_decode<4><<<bgrid, srd::BSHUF_DECODE_WARPS * 32, 0, ctx->stream>>>(blocks, frames, (uint8_t*)out, flags); break;
+        case 8: srd::k_bshuf_decode<8><<<bgrid, srd::BSHUF_DECODE_WARPS * 32, 0, ctx->stream>>>(blocks, frames, (uint8_t*)out, flags); break;
+        default: srd::k_bshuf_decode<16><<<bgrid, srd::BSHUF_DECODE_WARPS * 32, 0, ctx->stream>>>(blocks, frames, (uint8_t*)out, flags); break;
+        }
+        SR_LAUNCH_CHECK(ctx);
+        // a block chain that leaves its page (k_bshuf_blocks) or a corrupt LZ4 stream (k_bshuf_decode)
+        SR_CUDA(ctx, cudaMemcpyAsync(hc, sc->flags.p, 8, cudaMemcpyDeviceToHost, ctx->stream));
+        SR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        if (*(const int32_t*)hc) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "a bitshuffle page has a corrupt block chain or LZ4 stream");
         return SR_OK;
     }
     SR_TRY(sc->frames.reserve(ctx, sizeof(srd::FrameDesc) * (size_t)frames));

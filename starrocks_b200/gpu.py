@@ -591,7 +591,7 @@ def chunk_serialize(ctx, chunk, row_begin=0, row_end=None):
 
 
 class PageDecoder:
-    """sr_page_decoder: frame-of-reference / plain data pages -> a device column"""
+    """sr_page_decoder: frame-of-reference / plain / bitshuffle data pages -> a device column"""
 
     def __init__(self, ctx):
         self.ctx = ctx

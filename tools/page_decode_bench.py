@@ -1,10 +1,11 @@
-"""Frame-of-reference page decode on the device (SURVEY.md 8f-4): throughput of sr_pages_decode on SSB-shaped key columns.
+"""Segment page decode on the device (SURVEY.md 8f-4): throughput of sr_pages_decode on SSB-shaped key columns.
 
-    python tools/page_decode_bench.py [--rows 200000000] [--page-rows 65536]
+    python tools/page_decode_bench.py [--rows 50000000] [--page-rows 65536] [--encoding for|bitshuffle|both]
 
-Encodes synthetic lineorder key columns with the (reference-pinned) oracle encoder on the host, then times the decode of the
-resident pages (device memory) and of pages in page-locked host memory (the decode is the PCIe transfer), and checks a
-checksum of every decoded column against the raw values.  Prints one JSON line.
+Encodes synthetic lineorder key columns on the host -- frame-of-reference pages with the (reference-pinned) oracle encoder,
+BIT_SHUFFLE pages (bitshuffle + LZ4, StarRocks' default for these types) with the CPU codec in bshuf_oracle -- then times
+the decode of the resident pages (device memory) and of pages in page-locked host memory (the decode is the PCIe transfer:
+only the encoded bytes cross the bus), and checks every decoded column against the raw values.  Prints one JSON line.
 """
 import argparse
 import json
@@ -16,7 +17,8 @@ import numpy as np
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from oracle import oracle  # noqa: E402  (encoder only: test infrastructure building the input)
+import bshuf_oracle  # noqa: E402  (encoders only: test infrastructure building the input)
+from oracle import oracle  # noqa: E402
 from starrocks_b200 import abi, gpu  # noqa: E402
 
 
@@ -26,6 +28,7 @@ def main():
     ap.add_argument("--page-rows", type=int, default=65_536)
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--repeat", type=int, default=8, help="decode the encoded pages this many times over into one column (amortises the per-call costs without more host encoding)")
+    ap.add_argument("--encoding", choices=["for", "bitshuffle", "both"], default="for")
     args = ap.parse_args()
     n = args.rows
     rng = np.random.default_rng(1)
@@ -34,10 +37,12 @@ def main():
             "lo_revenue int64 (24 bits)": rng.integers(1, 10_000_000, n, dtype=np.int64)}
     ctx = gpu.Context(0)
     dec = gpu.PageDecoder(ctx)
+    encodings = {"for": (abi.PAGE_FOR, oracle.for_encode), "bitshuffle": (abi.PAGE_BITSHUFFLE, bshuf_oracle.bitshuffle_encode)}
     res = []
-    for name, v in cols.items():
+    for (name, v), enc in ((c, e) for c in cols.items() for e in (["for", "bitshuffle"] if args.encoding == "both" else [args.encoding])):
+        code, encode = encodings[enc]
         t0 = time.perf_counter()
-        pages = [oracle.for_encode(v[lo:lo + args.page_rows]) for lo in range(0, n, args.page_rows)]
+        pages = [encode(v[lo:lo + args.page_rows]) for lo in range(0, n, args.page_rows)]
         enc_s = time.perf_counter() - t0
         total = sum(len(p) for p in pages)
         typ = abi.TYPE_INT if v.dtype == np.int32 else abi.TYPE_BIGINT
@@ -47,7 +52,7 @@ def main():
         offs = np.cumsum([0] + [len(p) + (-len(p)) % 16 for p in pages])
         dblob = blob.cuda()
         pblob = blob.pin_memory()
-        line = {"column": name, "rows": n * R, "pages": len(pages) * R, "page_bytes": total * R, "bits_per_value": 8.0 * total / n}
+        line = {"column": name, "encoding": enc, "rows": n * R, "pages": len(pages) * R, "page_bytes": total * R, "bits_per_value": 8.0 * total / n}
         for label, base, mem in (("device", dblob.data_ptr(), abi.MEM_DEVICE), ("pinned_host", pblob.data_ptr(), abi.MEM_HOST_PINNED)):
             views = [(base + int(offs[k]), len(p)) for k, p in enumerate(pages)] * R
             best = 1e9
@@ -55,7 +60,7 @@ def main():
                 e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
                 torch.cuda.synchronize()
                 e0.record()
-                rows = dec.decode(abi.PAGE_FOR, typ, views, out.data_ptr(), n * R, mem=mem)
+                rows = dec.decode(code, typ, views, out.data_ptr(), n * R, mem=mem)
                 e1.record()
                 torch.cuda.synchronize()
                 best = min(best, e0.elapsed_time(e1))
@@ -66,7 +71,9 @@ def main():
         line["host_encode_s"] = enc_s
         res.append(line)
     dec.close()
-    print(json.dumps({"workload": "frame-of-reference page decode (sr_pages_decode)", "page_rows": args.page_rows, "columns": res}))
+    props = torch.cuda.get_device_properties(0)
+    print(json.dumps({"workload": "segment page decode (sr_pages_decode)", "device": props.name, "page_rows": args.page_rows,
+                      "columns": res}))
 
 
 if __name__ == "__main__":
