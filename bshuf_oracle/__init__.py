@@ -150,6 +150,59 @@ def bitshuffle_decode(page, dtype_or_width):
     return got if dt == np.uint8 and isinstance(dtype_or_width, int) else got.view(dt)
 
 
+# ---- dictionary-encoded (DICT_ENCODING) columns: BinaryDictPageBuilder::finish / BinaryPlainPageBuilder::finish ----
+DICT_ENCODING, PLAIN_ENCODING = 5, 2            # EncodingTypePB values of a dictionary data page's mode word
+
+
+def dict_page_encode(codes):
+    """dictionary data page body of int32 codes: the mode word 5, then the BIT_SHUFFLE page of the codes"""
+    c = np.ascontiguousarray(codes, dtype=np.int32)
+    return np.concatenate([np.array([DICT_ENCODING], dtype="<u4").view(np.uint8), bitshuffle_encode(c)])
+
+
+def dict_page_plain_fallback(words):
+    """a data page written after the column's dictionary overflowed: the mode word 2, then a BinaryPlainPage of strings"""
+    return np.concatenate([np.array([PLAIN_ENCODING], dtype="<u4").view(np.uint8), binary_plain_page_encode(words)])
+
+
+def dict_page_decode(page):
+    """dictionary data page body -> int32 codes; CorruptPage for a short page, a mode other than 5 (2 included: strings,
+    not codes) or a bad bitshuffle page"""
+    p = np.ascontiguousarray(page, dtype=np.uint8)
+    if len(p) < 4:
+        raise CorruptPage("dictionary page shorter than its mode word")
+    mode = int(np.frombuffer(p[:4].tobytes(), dtype="<u4")[0])
+    if mode != DICT_ENCODING:
+        raise CorruptPage("dictionary page mode %d" % mode)
+    if len(p) < 20 or int(np.frombuffer(p[16:20].tobytes(), dtype="<u4")[0]) != 4:
+        raise CorruptPage("dictionary codes are not a 4-byte bitshuffle page")
+    return bitshuffle_decode(p[4:], np.int32)
+
+
+def binary_plain_page_encode(words):
+    """BinaryPlainPage of byte strings: the words back to back, one uint32 LE start offset per word, the uint32 LE count"""
+    words = [bytes(w) for w in words]
+    offs = np.cumsum([0] + [len(w) for w in words[:-1]]).astype("<u4") if words else np.zeros(0, dtype="<u4")
+    return np.concatenate([np.frombuffer(b"".join(words), dtype=np.uint8), offs.view(np.uint8),
+                           np.array([len(words)], dtype="<u4").view(np.uint8)])
+
+
+def binary_plain_page_decode(page):
+    """BinaryPlainPage -> list of bytes (BinaryPlainPageDecoder::init); CorruptPage for a count that does not fit, or
+    offsets that decrease or pass the offset array.  Word i runs to offset[i + 1], the last one to the offset array."""
+    p = np.ascontiguousarray(page, dtype=np.uint8).tobytes()
+    if len(p) < 4:
+        raise CorruptPage("binary plain page shorter than its count")
+    n = int.from_bytes(p[-4:], "little")
+    start = len(p) - 4 - 4 * n
+    if start < 0:
+        raise CorruptPage("word count %d" % n)
+    offs = [int.from_bytes(p[start + 4 * i:start + 4 * i + 4], "little") for i in range(n)] + [start]
+    if any(a > b for a, b in zip(offs, offs[1:])):
+        raise CorruptPage("word offsets")
+    return [p[offs[i]:offs[i + 1]] for i in range(n)]
+
+
 def system_lz4():
     """the system liblz4 (ctypes: LZ4_compress_default, LZ4_decompress_safe, LZ4_compressBound), or None when absent"""
     for name in ("liblz4.so.1", ctypes.util.find_library("lz4")):

@@ -712,14 +712,23 @@ int32_t sr_xchg_hash(sr_xchg* x, const sr_chunk_view* in, uint32_t* hash_values,
  * page_io.cpp), all in `mem`: SR_MEM_DEVICE, SR_MEM_HOST_PINNED (page-locked mapped memory, e.g. a registered page cache:
  * read in place over PCIe, the decode is the transfer) or SR_MEM_HOST (pageable: staged page by page).  The values of page
  * k follow those of page k - 1 in `out` (device memory, room for out_capacity values); *out_rows receives the total.
+ * And, for TYPE_INT only, the data pages of a dictionary-encoded (DICT_ENCODING: CHAR / VARCHAR) column, decoded
+ * straight into ids -- the low-cardinality global dictionary's scan step (GlobalDictCodeColumnIterator):
+ *   BinaryDictPageDecoder::next_batch        be/src/storage/rowset/binary_dict_page.{h,cpp}
+ *   A data page is a 4-byte little-endian mode word (EncodingTypePB) and, with mode 5 (DICT_ENCODING), a BIT_SHUFFLE page
+ *   of int32 codes.  Code k is stored as values[k] of the last sr_page_decoder_set_dict (SR_ERR_STATE when there is
+ *   none); a code >= num_words is a corrupt page.  Mode 2 (PLAIN_ENCODING: the dictionary overflowed and the column
+ *   fell back to plain string pages) gives SR_ERR_NOT_SUPPORTED when no page of the call is malformed.  `out` must be
+ *   4-byte aligned.
  * SR_ERR_INVALID_ARGUMENT for a page that is not well formed (sizes, frame table, bit widths, the bitshuffle header, block
- * chain or LZ4 streams).  Asynchronous on the context stream except for one small read-back of the per-page counts and,
- * for FOR and BIT_SHUFFLE, one of the error flag at the end.  RLE and dictionary pages are not covered:
- * SR_ERR_NOT_SUPPORTED. */
+ * chain or LZ4 streams, the dictionary mode word or codes).  Asynchronous on the context stream except for one small
+ * read-back of the per-page counts and, for FOR, BIT_SHUFFLE and DICT, one of the error flag at the end.  RLE pages and
+ * plain-mode string pages are not covered: SR_ERR_NOT_SUPPORTED. */
 typedef enum sr_page_encoding {
-    SR_PAGE_PLAIN = 0,     /* EncodingTypePB::PLAIN_ENCODING */
-    SR_PAGE_FOR = 1,       /* EncodingTypePB::FOR_ENCODING */
-    SR_PAGE_BITSHUFFLE = 2 /* EncodingTypePB::BIT_SHUFFLE */
+    SR_PAGE_PLAIN = 0,      /* EncodingTypePB::PLAIN_ENCODING */
+    SR_PAGE_FOR = 1,        /* EncodingTypePB::FOR_ENCODING */
+    SR_PAGE_BITSHUFFLE = 2, /* EncodingTypePB::BIT_SHUFFLE */
+    SR_PAGE_DICT = 3        /* EncodingTypePB::DICT_ENCODING */
 } sr_page_encoding;
 
 typedef struct sr_page_view {
@@ -732,6 +741,13 @@ sr_page_decoder* sr_page_decoder_create(sr_ctx* ctx);
 void sr_page_decoder_destroy(sr_page_decoder* dec);
 int32_t sr_pages_decode(sr_page_decoder* dec, int32_t encoding, int32_t type, const sr_page_view* pages, int32_t num_pages, int32_t mem, void* out,
                         int64_t out_capacity, int64_t* out_rows);
+/* The code -> value table of SR_PAGE_DICT pages (BinaryDictPageDecoder::set_dict_decoder): values[k] is what code k
+ * decodes to -- for a low-cardinality column, the segment's local -> global id table (the global id of word k of the
+ * segment's dictionary page, 0 for an empty word the global dictionary lacks: build_code_convert_map).  `values` (num_words
+ * int32 in `mem`: SR_MEM_HOST, SR_MEM_HOST_PINNED or SR_MEM_DEVICE) is copied into the decoder; the caller may free it
+ * when the call returns (it synchronises the context stream).  A later call replaces the table: one table per segment, so
+ * a caller decoding several segments into one column sets each segment's table and advances `out`. */
+int32_t sr_page_decoder_set_dict(sr_page_decoder* dec, const int32_t* values, int64_t num_words, int32_t mem);
 
 /* ---------------------------------------------------------------------------------------
  * exchange wire format (SURVEY.md 8f-3): the bytes of ChunkPB.data as ProtobufChunkSerde::serialize_without_meta writes

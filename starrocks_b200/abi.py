@@ -120,7 +120,7 @@ class sr_join_desc(C.Structure):
                 ("other_conjunct", sr_expr)]
 
 
-PAGE_PLAIN, PAGE_FOR, PAGE_BITSHUFFLE = 0, 1, 2
+PAGE_PLAIN, PAGE_FOR, PAGE_BITSHUFFLE, PAGE_DICT = 0, 1, 2, 3
 
 
 class sr_page_view(C.Structure):

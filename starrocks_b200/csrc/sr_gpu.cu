@@ -1635,6 +1635,8 @@ int32_t sr_chunk_deserialize(sr_serde* h, const void* src, int64_t bytes, int32_
 struct sr_page_decoder {
     sr_ctx* ctx = nullptr;
     PageScratch scratch;
+    DevBuf dict;                // sr_page_decoder_set_dict's table: what each code of a dictionary data page decodes to
+    long long dict_words = -1;  // -1: no table set
 };
 
 sr_page_decoder* sr_page_decoder_create(sr_ctx* ctx) {
@@ -1656,7 +1658,21 @@ int32_t sr_pages_decode(sr_page_decoder* d, int32_t encoding, int32_t type, cons
                         int64_t out_capacity, int64_t* out_rows) {
     if (!d || !out_rows) return SR_ERR_INVALID_ARGUMENT;
     SR_BIND(d->ctx);
-    return pages_decode(d->ctx, &d->scratch, encoding, type, pages, num_pages, mem, out, out_capacity, out_rows);
+    return pages_decode(d->ctx, &d->scratch, encoding, type, pages, num_pages, mem, out, out_capacity, out_rows, (const int32_t*)d->dict.p, d->dict_words);
+}
+
+int32_t sr_page_decoder_set_dict(sr_page_decoder* d, const int32_t* values, int64_t num_words, int32_t mem) {
+    if (!d) return SR_ERR_INVALID_ARGUMENT;
+    SR_BIND(d->ctx);
+    sr_ctx* ctx = d->ctx;
+    if (num_words < 0 || num_words > INT32_MAX || (num_words > 0 && !values)) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "sr_page_decoder_set_dict: %lld words", (long long)num_words);
+    if (mem != SR_MEM_HOST && mem != SR_MEM_DEVICE && mem != SR_MEM_HOST_PINNED) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "unknown memory kind %d", mem);
+    d->dict_words = -1; // a failed call leaves no table
+    SR_TRY(d->dict.reserve(ctx, 4 * (size_t)num_words + 4));
+    if (num_words > 0) SR_CUDA(ctx, cudaMemcpyAsync(d->dict.p, values, 4 * (size_t)num_words, cudaMemcpyDefault, ctx->stream));
+    SR_CUDA(ctx, cudaStreamSynchronize(ctx->stream)); // the caller may free `values` on return
+    d->dict_words = num_words;
+    return SR_OK;
 }
 
 int32_t sr_flush_l2(sr_ctx* ctx) {

@@ -30,6 +30,13 @@
 // with coalesced word loads (in-place reads over PCIe move only the compressed bytes), the LZ4 sequences are parsed serially
 // (warp-uniform) into an 8 KB shared buffer with the literal and match bytes copied across the lanes, and every lane then
 // un-transposes 8 consecutive elements (one 8 x 8 bit transpose per byte position) and stores them.
+//
+//   BinaryDictPageDecoder        be/src/storage/rowset/binary_dict_page.{h,cpp} (BinaryDictPageBuilder::finish writes the page)
+// A data page of a dictionary-encoded column: a 4-byte little-endian mode word (EncodingTypePB: 5 DICT_ENCODING, 2
+// PLAIN_ENCODING once the dictionary overflowed), then with mode 5 a bitshuffle page of int32 codes, a code being a position
+// in the segment's dictionary page.  k_page_footers checks the mode word and the embedded header, the host moves the page
+// descriptors past the mode word, and k_bshuf_decode_dict is k_bshuf_decode<4> with the store translating every code
+// through the decoder's table (sr_page_decoder_set_dict): the id column comes out in HBM.
 #pragma once
 
 namespace srd {
@@ -56,7 +63,8 @@ __device__ __forceinline__ uint32_t page_le32(const uint8_t* p) {
 constexpr int BSHUF_BLOCK_BYTES = 8192;     // bshuf_default_block_size(s) * s for every width s in 1..16
 constexpr uint32_t BSHUF_MAX_STREAM = 8240; // LZ4_compressBound(8192)
 
-// value count and frame (bitshuffle: block) count of every page; flags[0] |= 1 when a page cannot be a page of `encoding`
+// value count and frame (bitshuffle: block) count of every page; flags[0] |= 1 when a page cannot be a page of `encoding`,
+// |= 2 for a dictionary-column page in plain mode (the column's dictionary overflowed: a page of strings, not codes)
 __global__ void __launch_bounds__(256) k_page_footers(const PageDesc* __restrict__ pages, int32_t num_pages, int32_t encoding, int32_t elem_size,
                                                        unsigned long long* __restrict__ counts /* [2 * num_pages]: values, frames */, int32_t* __restrict__ flags) {
     const int p = blockIdx.x * blockDim.x + threadIdx.x;
@@ -71,13 +79,20 @@ __global__ void __launch_bounds__(256) k_page_footers(const PageDesc* __restrict
             n = page_le32(pg.data);
             if (pg.size != 4 + (long long)n * elem_size) bad = true;
         }
-    } else if (encoding == SR_PAGE_BITSHUFFLE) {
-        if (pg.size < 16) {
+    } else if (encoding == SR_PAGE_BITSHUFFLE || encoding == SR_PAGE_DICT) {
+        // a dictionary data page: a 4-byte mode word (EncodingTypePB: 5 dictionary codes, 2 plain strings), then with mode
+        // 5 a bitshuffle page of int32 codes
+        const int hdr = encoding == SR_PAGE_DICT ? 4 : 0;
+        const uint8_t* b = pg.data + hdr;
+        const long long size = pg.size - hdr;
+        if (hdr && pg.size >= 4 && page_le32(pg.data) == 2) {
+            atomicOr(flags, 2);
+        } else if (size < 16 || (hdr && page_le32(pg.data) != 5)) {
             bad = true;
         } else {
-            n = page_le32(pg.data);
-            const unsigned long long padded = page_le32(pg.data + 8), blk = BSHUF_BLOCK_BYTES / elem_size;
-            if (page_le32(pg.data + 4) != (unsigned long long)pg.size || padded != ((n + 7) & ~7ull) || page_le32(pg.data + 12) != (uint32_t)elem_size) bad = true;
+            n = page_le32(b);
+            const unsigned long long padded = page_le32(b + 8), blk = BSHUF_BLOCK_BYTES / elem_size;
+            if (page_le32(b + 4) != (unsigned long long)size || padded != ((n + 7) & ~7ull) || page_le32(b + 12) != (uint32_t)elem_size) bad = true;
             frames = (padded + blk - 1) / blk; // blocks
         }
     } else {
@@ -327,10 +342,11 @@ constexpr int BSHUF_DECODE_WARPS = 2;                                // 2 x 16.1
 constexpr int BSHUF_STAGE_WORDS = (3 + (int)BSHUF_MAX_STREAM + 3) / 4; // the longest stream at the worst byte skew
 
 // one warp per block.  S: value width in bytes.  Every length and offset is checked against the staged input and the
-// block's output before it is used: a corrupt stream raises the flag and stores nothing.
-template <int S>
-__global__ void __launch_bounds__(BSHUF_DECODE_WARPS * 32) k_bshuf_decode(const BshufBlock* __restrict__ blocks, long long num_blocks, uint8_t* __restrict__ out,
-                                                                         int32_t* __restrict__ flags) {
+// block's output before it is used: a corrupt stream raises the flag and stores nothing.  DICT (S = 4, dictionary data
+// pages): every decoded value is a code; it is checked against dict_size and replaced by dict[code] before the store.
+template <int S, bool DICT>
+__device__ __forceinline__ void bshuf_decode_blocks(const BshufBlock* __restrict__ blocks, long long num_blocks, uint8_t* __restrict__ out,
+                                                    int32_t* __restrict__ flags, const int32_t* __restrict__ dict, uint32_t dict_size) {
     __shared__ uint32_t s_in[BSHUF_DECODE_WARPS][BSHUF_STAGE_WORDS];
     __shared__ uint8_t s_out[BSHUF_DECODE_WARPS][BSHUF_BLOCK_BYTES];
     constexpr int Q = (S + 7) / 8; // 64-bit words per value
@@ -392,6 +408,7 @@ __global__ void __launch_bounds__(BSHUF_DECODE_WARPS * 32) k_bshuf_decode(const 
         // un-transpose: lane takes elements [8g, 8g + 8); byte j of them = the 8 x 8 transpose of byte g of rows 8j .. 8j + 7
         const uint32_t R = d.elems / 8;
         uint8_t* dst = out + d.row * S;
+        bool bad = false;
         for (uint32_t g = lane; g < R; g += 32) {
             unsigned long long v[8][Q];
 #pragma unroll
@@ -406,6 +423,17 @@ __global__ void __launch_bounds__(BSHUF_DECODE_WARPS * 32) k_bshuf_decode(const 
                 x = bshuf_trans8x8(x);
 #pragma unroll
                 for (int t = 0; t < 8; t++) v[t][j / 8] |= ((x >> (8 * t)) & 0xFF) << (8 * (j % 8));
+            }
+            if (DICT) {
+                // code -> dict[code] through the read-only path (a low-cardinality table is <= 1 KB and stays in L1).  A code
+                // outside the dictionary is a corrupt page: the reference's CPU decode would write 0 there silently.
+#pragma unroll
+                for (int t = 0; t < 8; t++) {
+                    const uint32_t c = (uint32_t)v[t][0];
+                    const bool in = c < dict_size;
+                    if (!in && 8 * g + t < d.n_out) bad = true; // padding is never stored
+                    v[t][0] = in ? (uint32_t)__ldg(dict + c) : 0u;
+                }
             }
             uint8_t* p = dst + (size_t)8 * g * S;
             if (8 * g + 8 <= d.n_out && ((uintptr_t)p & 7) == 0) {
@@ -444,7 +472,20 @@ __global__ void __launch_bounds__(BSHUF_DECODE_WARPS * 32) k_bshuf_decode(const 
                 }
             }
         }
+        if (DICT && __any_sync(SR_FULL_MASK, bad) && lane == 0) atomicOr(flags, 1); // (the block loop is warp-uniform)
     }
+}
+
+template <int S>
+__global__ void __launch_bounds__(BSHUF_DECODE_WARPS * 32) k_bshuf_decode(const BshufBlock* __restrict__ blocks, long long num_blocks, uint8_t* __restrict__ out,
+                                                                         int32_t* __restrict__ flags) {
+    bshuf_decode_blocks<S, false>(blocks, num_blocks, out, flags, nullptr, 0);
+}
+
+// dictionary data pages: the bitshuffle blocks of int32 codes, each code translated through dict[0, dict_size)
+__global__ void __launch_bounds__(BSHUF_DECODE_WARPS * 32) k_bshuf_decode_dict(const BshufBlock* __restrict__ blocks, long long num_blocks, int32_t* __restrict__ out,
+                                                                              int32_t* __restrict__ flags, const int32_t* __restrict__ dict, uint32_t dict_size) {
+    bshuf_decode_blocks<4, true>(blocks, num_blocks, (uint8_t*)out, flags, dict, dict_size);
 }
 
 } // namespace srd
@@ -455,10 +496,15 @@ struct PageScratch {
     PinnedBuf host_pages, host_counts;
 };
 
+// dict / dict_words: the decoder's code -> value table (device memory; dict_words < 0: none set), read by SR_PAGE_DICT only
 static int32_t pages_decode(sr_ctx* ctx, PageScratch* sc, int32_t encoding, int32_t type, const sr_page_view* pv, int32_t num_pages, int32_t mem, void* out,
-                            int64_t out_capacity, int64_t* out_rows) {
+                            int64_t out_capacity, int64_t* out_rows, const int32_t* dict, long long dict_words) {
     const int w = srd::type_width(type);
-    if (encoding == SR_PAGE_BITSHUFFLE) {
+    if (encoding == SR_PAGE_DICT) {
+        if (type != SR_TYPE_INT) return sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "dictionary page decode of type %d (TYPE_INT ids)", type);
+        if (dict_words < 0) return sr_fail(ctx, SR_ERR_STATE, "dictionary pages decoded before sr_page_decoder_set_dict");
+        if ((uintptr_t)out % 4) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "output column not aligned to 4 bytes");
+    } else if (encoding == SR_PAGE_BITSHUFFLE) {
         if (w == 0) return sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "bitshuffle page decode of type %d (fixed-width types)", type);
         if ((uintptr_t)out % std::min(w, 8)) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "output column not aligned to %d bytes", std::min(w, 8));
     } else {
@@ -531,10 +577,17 @@ static int32_t pages_decode(sr_ctx* ctx, PageScratch* sc, int32_t encoding, int3
     SR_CUDA(ctx, cudaMemcpyAsync(hc, sc->counts.p, 16 * (size_t)num_pages, cudaMemcpyDeviceToHost, ctx->stream));
     SR_CUDA(ctx, cudaMemcpyAsync(hc + 2 * (size_t)num_pages, sc->flags.p, 8, cudaMemcpyDeviceToHost, ctx->stream));
     SR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    if (*(const int32_t*)(hc + 2 * (size_t)num_pages))
-        return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "a page is not a well-formed %s page", encoding == SR_PAGE_FOR ? "frame-of-reference" : encoding == SR_PAGE_PLAIN ? "plain" : "bitshuffle");
+    const int32_t hflags = *(const int32_t*)(hc + 2 * (size_t)num_pages);
+    if (hflags & 1)
+        return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "a page is not a well-formed %s page",
+                       encoding == SR_PAGE_FOR ? "frame-of-reference" : encoding == SR_PAGE_PLAIN ? "plain" : encoding == SR_PAGE_DICT ? "dictionary data" : "bitshuffle");
+    if (hflags & 2) return sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "a dictionary data page in plain mode: the column fell back to plain pages");
     long long rows = 0, frames = 0;
     for (int p = 0; p < num_pages; p++) {
+        if (encoding == SR_PAGE_DICT) { // past the mode word: the bitshuffle page of codes (k_bshuf_blocks reads it as is)
+            hp[p].data += 4;
+            hp[p].size -= 4;
+        }
         hp[p].row_off = rows;
         hp[p].frame_off = frames;
         rows += (long long)hc[2 * p];
@@ -552,25 +605,31 @@ static int32_t pages_decode(sr_ctx* ctx, PageScratch* sc, int32_t encoding, int3
         }
         return SR_OK;
     }
-    if (encoding == SR_PAGE_BITSHUFFLE) {
+    if (encoding == SR_PAGE_BITSHUFFLE || encoding == SR_PAGE_DICT) {
         SR_TRY(sc->frames.reserve(ctx, sizeof(srd::BshufBlock) * (size_t)frames));
         srd::BshufBlock* blocks = (srd::BshufBlock*)sc->frames.p;
         srd::k_bshuf_blocks<<<grid_for(num_pages, 256), 256, 0, ctx->stream>>>((const srd::PageDesc*)sc->pages.p, num_pages, w, blocks, (int32_t*)sc->flags.p);
         SR_LAUNCH_CHECK(ctx);
         const int bgrid = (int)std::min<long long>((frames + srd::BSHUF_DECODE_WARPS - 1) / srd::BSHUF_DECODE_WARPS, (long long)ctx->num_sms * 8);
         int32_t* flags = (int32_t*)sc->flags.p;
-        switch (w) {
-        case 1: srd::k_bshuf_decode<1><<<bgrid, srd::BSHUF_DECODE_WARPS * 32, 0, ctx->stream>>>(blocks, frames, (uint8_t*)out, flags); break;
-        case 2: srd::k_bshuf_decode<2><<<bgrid, srd::BSHUF_DECODE_WARPS * 32, 0, ctx->stream>>>(blocks, frames, (uint8_t*)out, flags); break;
-        case 4: srd::k_bshuf_decode<4><<<bgrid, srd::BSHUF_DECODE_WARPS * 32, 0, ctx->stream>>>(blocks, frames, (uint8_t*)out, flags); break;
-        case 8: srd::k_bshuf_decode<8><<<bgrid, srd::BSHUF_DECODE_WARPS * 32, 0, ctx->stream>>>(blocks, frames, (uint8_t*)out, flags); break;
-        default: srd::k_bshuf_decode<16><<<bgrid, srd::BSHUF_DECODE_WARPS * 32, 0, ctx->stream>>>(blocks, frames, (uint8_t*)out, flags); break;
+        if (encoding == SR_PAGE_DICT) {
+            srd::k_bshuf_decode_dict<<<bgrid, srd::BSHUF_DECODE_WARPS * 32, 0, ctx->stream>>>(blocks, frames, (int32_t*)out, flags, dict, (uint32_t)dict_words);
+        } else {
+            switch (w) {
+            case 1: srd::k_bshuf_decode<1><<<bgrid, srd::BSHUF_DECODE_WARPS * 32, 0, ctx->stream>>>(blocks, frames, (uint8_t*)out, flags); break;
+            case 2: srd::k_bshuf_decode<2><<<bgrid, srd::BSHUF_DECODE_WARPS * 32, 0, ctx->stream>>>(blocks, frames, (uint8_t*)out, flags); break;
+            case 4: srd::k_bshuf_decode<4><<<bgrid, srd::BSHUF_DECODE_WARPS * 32, 0, ctx->stream>>>(blocks, frames, (uint8_t*)out, flags); break;
+            case 8: srd::k_bshuf_decode<8><<<bgrid, srd::BSHUF_DECODE_WARPS * 32, 0, ctx->stream>>>(blocks, frames, (uint8_t*)out, flags); break;
+            default: srd::k_bshuf_decode<16><<<bgrid, srd::BSHUF_DECODE_WARPS * 32, 0, ctx->stream>>>(blocks, frames, (uint8_t*)out, flags); break;
+            }
         }
         SR_LAUNCH_CHECK(ctx);
         // a block chain that leaves its page (k_bshuf_blocks) or a corrupt LZ4 stream (k_bshuf_decode)
         SR_CUDA(ctx, cudaMemcpyAsync(hc, sc->flags.p, 8, cudaMemcpyDeviceToHost, ctx->stream));
         SR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        if (*(const int32_t*)hc) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "a bitshuffle page has a corrupt block chain or LZ4 stream");
+        if (*(const int32_t*)hc)
+            return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, encoding == SR_PAGE_DICT ? "a dictionary data page has a corrupt block chain or LZ4 stream, or a code outside the dictionary"
+                                                                                : "a bitshuffle page has a corrupt block chain or LZ4 stream");
         return SR_OK;
     }
     SR_TRY(sc->frames.reserve(ctx, sizeof(srd::FrameDesc) * (size_t)frames));

@@ -167,6 +167,7 @@ def lib():
         "sr_page_decoder_create": (vp, [vp]),
         "sr_page_decoder_destroy": (None, [vp]),
         "sr_pages_decode": (i32, [vp, i32, i32, vp, i32, i32, vp, i64, vp]),
+        "sr_page_decoder_set_dict": (i32, [vp, vp, i64, i32]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)
@@ -192,7 +193,7 @@ EXPORTED_SYMBOLS = [
     "sr_xchg_destroy", "sr_xchg_partition", "sr_xchg_hash", "sr_gather", "sr_memcpy", "sr_abi_sizeof", "sr_bandwidth_probe", "sr_flush_l2",
     "sr_chunk_serialized_size", "sr_chunk_serialize", "sr_serde_create", "sr_serde_destroy", "sr_chunk_deserialize",
     "sr_host_alloc", "sr_host_free", "sr_event_create", "sr_event_destroy", "sr_event_record", "sr_event_query", "sr_event_sync",
-    "sr_page_decoder_create", "sr_page_decoder_destroy", "sr_pages_decode",
+    "sr_page_decoder_create", "sr_page_decoder_destroy", "sr_pages_decode", "sr_page_decoder_set_dict",
 ]
 
 
@@ -591,7 +592,7 @@ def chunk_serialize(ctx, chunk, row_begin=0, row_end=None):
 
 
 class PageDecoder:
-    """sr_page_decoder: frame-of-reference / plain / bitshuffle data pages -> a device column"""
+    """sr_page_decoder: frame-of-reference / plain / bitshuffle data pages -> a device column; dictionary data pages -> ids"""
 
     def __init__(self, ctx):
         self.ctx = ctx
@@ -616,6 +617,16 @@ class PageDecoder:
         rows = C.c_int64(0)
         self.ctx.check(lib().sr_pages_decode(self.h, encoding, typ, views, len(pages), mem, out_ptr, out_capacity, C.byref(rows)))
         return rows.value
+
+    def set_dict(self, values, mem=abi.MEM_HOST):
+        """the code -> value table of PAGE_DICT pages (one per segment; replaces the last): a host int32 array, or a
+        (pointer, number of words) pair in `mem`.  The decoder keeps its own copy."""
+        if isinstance(values, tuple):
+            ptr, n = values
+        else:
+            a = np.ascontiguousarray(values, dtype=np.int32)
+            ptr, n = (a.ctypes.data if a.size else None), a.size
+        self.ctx.check(lib().sr_page_decoder_set_dict(self.h, ptr, n, mem))
 
 
 class Serde:

@@ -6,6 +6,7 @@
 //   be/src/runtime/global_dict/fragment_dict_state.cpp:44-67   the maps built from the plan's (strings, ids) lists
 //   be/src/storage/rowset/dictcode_column_iterator.cpp:53-128  segment-local codes -> global ids (the scan side)
 //   be/src/runtime/global_dict/decoder.cpp:104-176         GlobalDictDecoder::decode_string
+//   be/src/storage/rowset/binary_plain_page.h              BinaryPlainPageBuilder / Decoder: a segment's dictionary page
 //   be/src/exec/pipeline/dict_decode_operator.{h,cpp}      DictDecodeOperator / DictDecodeOperatorFactory
 // Host-only: no kernel is involved; the id columns these classes produce are what make_chunk_view hands to libsr_gpu.
 #pragma once
@@ -121,6 +122,12 @@ public:
         return out;
     }
     int dict_size() const { return _dict_size; }
+    // the table in code order (without the slot of index -1): global_ids()[k] is the global id of local word k.  What
+    // sr_page_decoder_set_dict takes to decode this segment's dictionary data pages into ids on the device.
+    std::vector<int32_t> global_ids() const {
+        if (_table.empty()) return {};
+        return std::vector<int32_t>(_table.begin() + 1, _table.begin() + 1 + _dict_size);
+    }
 
 private:
     std::vector<int16_t> _table;
@@ -144,6 +151,40 @@ inline void encode_local_dict(const BinaryColumn& column, BinaryColumn* local_wo
     }
     local_words->reset_column();
     for (const auto& w : order) local_words->append_string(w);
+}
+
+// A segment's dictionary page (BinaryPlainPage): the words' bytes back to back, one uint32 LE start offset per word, then
+// the uint32 LE word count.  Word i runs from offset[i] to offset[i + 1], the last word to the start of the offset array.
+// The parse of BinaryPlainPageDecoder::init, rejecting a count that does not fit the page and offsets that decrease or
+// pass the offset array.
+inline Status decode_binary_plain_page(const uint8_t* data, size_t size, BinaryColumn* words) {
+    if (size < 4) return Status::InvalidArgument("binary plain page: shorter than its word count");
+    uint32_t n = 0;
+    memcpy(&n, data + size - 4, 4);
+    if ((size - 4) / 4 < n) return Status::InvalidArgument("binary plain page: " + std::to_string(n) + " words do not fit");
+    const size_t start = size - 4 - 4 * (size_t)n;
+    if (start > 0xFFFFFFFFull) return Status::InvalidArgument("binary plain page: more than 4 GiB of words");
+    std::vector<uint32_t> offs(n + 1);
+    if (n) memcpy(offs.data(), data + start, 4 * (size_t)n);
+    offs[n] = (uint32_t)start;
+    for (uint32_t i = 0; i < n; i++)
+        if (offs[i] > offs[i + 1]) return Status::InvalidArgument("binary plain page: word offsets decrease or pass the offset array");
+    words->reset_column();
+    for (uint32_t i = 0; i < n; i++) words->append(Slice(data + offs[i], offs[i + 1] - offs[i]));
+    return Status::OK();
+}
+
+// BinaryPlainPageBuilder::finish of `words` (e.g. encode_local_dict's): the dictionary page a segment stores.  Test /
+// benchmark helper.
+inline std::vector<uint8_t> encode_binary_plain_page(const BinaryColumn& words) {
+    const auto& bytes = words.get_bytes();
+    std::vector<uint8_t> page(bytes.begin(), bytes.end());
+    auto put32 = [&page](uint32_t v) {
+        for (int k = 0; k < 4; k++) page.push_back((uint8_t)(v >> (8 * k)));
+    };
+    for (size_t i = 0; i < words.size(); i++) put32(words.get_offset()[i]);
+    put32((uint32_t)words.size());
+    return page;
 }
 
 // GlobalDictDecoder::decode_string for a plain or nullable TYPE_INT id column -> BinaryColumn / Nullable(BinaryColumn)

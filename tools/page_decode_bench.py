@@ -1,11 +1,15 @@
 """Segment page decode on the device (SURVEY.md 8f-4): throughput of sr_pages_decode on SSB-shaped key columns.
 
-    python tools/page_decode_bench.py [--rows 50000000] [--page-rows 65536] [--encoding for|bitshuffle|both]
+    python tools/page_decode_bench.py [--rows 50000000] [--page-rows 65536] [--encoding for|bitshuffle|both|dict]
 
 Encodes synthetic lineorder key columns on the host -- frame-of-reference pages with the (reference-pinned) oracle encoder,
 BIT_SHUFFLE pages (bitshuffle + LZ4, StarRocks' default for these types) with the CPU codec in bshuf_oracle -- then times
 the decode of the resident pages (device memory) and of pages in page-locked host memory (the decode is the PCIe transfer:
 only the encoded bytes cross the bus), and checks every decoded column against the raw values.  Prints one JSON line.
+
+--encoding dict: low-cardinality string columns (7, 25 and 256 words, codes drawn uniformly) written as dictionary data
+pages (mode word + bitshuffle page of int32 codes) and decoded into global ids through a per-segment table, timed next to
+BIT_SHUFFLE pages of the same codes decoded as plain int32 -- the difference is the mode word and the translation.
 """
 import argparse
 import json
@@ -28,8 +32,10 @@ def main():
     ap.add_argument("--page-rows", type=int, default=65_536)
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--repeat", type=int, default=8, help="decode the encoded pages this many times over into one column (amortises the per-call costs without more host encoding)")
-    ap.add_argument("--encoding", choices=["for", "bitshuffle", "both"], default="for")
+    ap.add_argument("--encoding", choices=["for", "bitshuffle", "both", "dict"], default="for")
     args = ap.parse_args()
+    if args.encoding == "dict":
+        return dict_bench(args)
     n = args.rows
     rng = np.random.default_rng(1)
     cols = {"lo_custkey (22 bits)": rng.integers(1, 3_000_000, n, dtype=np.int32), "lo_suppkey (18 bits)": rng.integers(1, 200_000, n, dtype=np.int32),
@@ -74,6 +80,61 @@ def main():
     props = torch.cuda.get_device_properties(0)
     print(json.dumps({"workload": "segment page decode (sr_pages_decode)", "device": props.name, "page_rows": args.page_rows,
                       "columns": res}))
+
+
+def _time(dec, code, views, out, rows, mem, reps):
+    best = 1e9
+    for _ in range(reps):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        torch.cuda.synchronize()
+        e0.record()
+        got = dec.decode(code, abi.TYPE_INT, views, out.data_ptr(), rows, mem=mem)
+        e1.record()
+        torch.cuda.synchronize()
+        best = min(best, e0.elapsed_time(e1))
+    assert got == rows
+    return best
+
+
+def dict_bench(args):
+    import subprocess
+    n, R = args.rows, args.repeat
+    rng = np.random.default_rng(2)
+    ctx = gpu.Context(0)
+    dec = gpu.PageDecoder(ctx)
+    out = torch.empty(n * R, dtype=torch.int32, device="cuda")
+    res = []
+    for words in (7, 25, 256):
+        codes = rng.integers(0, words, n, dtype=np.int32)
+        ids = (rng.permutation(words) + 1).astype(np.int32)            # a segment's local -> global id table
+        dec.set_dict(ids)
+        want = {"dict": ids[codes], "bitshuffle": codes}
+        line = {"column": "%d words" % words, "rows": n * R}
+        for enc, code, encode in (("dict", abi.PAGE_DICT, bshuf_oracle.dict_page_encode), ("bitshuffle", abi.PAGE_BITSHUFFLE, bshuf_oracle.bitshuffle_encode)):
+            pages = [encode(codes[lo:lo + args.page_rows]) for lo in range(0, n, args.page_rows)]
+            total = sum(len(p) for p in pages)
+            blob = torch.from_numpy(np.concatenate([np.pad(p, (0, (-len(p)) % 16)) for p in pages]))
+            offs = np.cumsum([0] + [len(p) + (-len(p)) % 16 for p in pages])
+            dblob, pblob = blob.cuda(), blob.pin_memory()
+            e = {"pages": len(pages) * R, "page_bytes": total * R, "bits_per_value": 8.0 * total / n}
+            for label, base, mem in (("device", dblob.data_ptr(), abi.MEM_DEVICE), ("pinned_host", pblob.data_ptr(), abi.MEM_HOST_PINNED)):
+                views = [(base + int(offs[k]), len(p)) for k, p in enumerate(pages)] * R
+                out.fill_(-1)
+                ms = _time(dec, code, views, out, n * R, mem, args.reps)
+                ok = bool((out.view(R, n).cpu().numpy() == want[enc][None, :]).all())
+                e[label] = {"ms": ms, "g_values_per_s": n * R / ms / 1e6, "page_gbs": total * R / ms / 1e6, "bit_exact": ok}
+            line[enc] = e
+            del dblob, pblob
+        res.append(line)
+    dec.close()
+    props = torch.cuda.get_device_properties(0)
+    try:
+        power = subprocess.run(["nvidia-smi", "-i", str(torch.cuda.current_device()), "--query-gpu=power.limit", "--format=csv,noheader"],
+                               capture_output=True, text=True, timeout=30).stdout.strip()
+    except OSError:
+        power = "unknown"
+    print(json.dumps({"workload": "dictionary page decode into global ids (sr_pages_decode, SR_PAGE_DICT)", "device": props.name,
+                      "power_limit": power, "page_rows": args.page_rows, "columns": res}))
 
 
 if __name__ == "__main__":
