@@ -294,8 +294,11 @@ __device__ __forceinline__ long long agg_find_slot(const AggDev& a, Loader& ld) 
                     idx = 0;
                     bad |= !a.key_nullable[k];
                 } else {
-                    idx = v - a.dense_min[k] + (a.key_nullable[k] ? 1 : 0);
-                    bad |= (v < a.dense_min[k]) || (idx >= a.dense_extent[k]);
+                    // unsigned offset against the non-NULL span: a key near the int64 extremes cannot wrap into the range
+                    const long long nn = a.key_nullable[k] ? 1 : 0;
+                    const unsigned long long off = (unsigned long long)v - (unsigned long long)a.dense_min[k];
+                    bad |= off >= (unsigned long long)(a.dense_extent[k] - nn);
+                    idx = (long long)off + nn;
                 }
                 slot += idx * a.dense_stride[k];
             }

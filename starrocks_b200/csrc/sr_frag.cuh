@@ -415,19 +415,8 @@ static int32_t frag_plan(sr_fragment* f, const VTab& vt, int64_t n) {
             auto int32_class = [&](int id) { return srd::type_width(f->reg.types[id]) == 4 && !srd::is_float_class(f->reg.types[id]); };
             for (int p = 0; p < h.num_preds && ok; p++) {
                 const srd::CPred& cp = h.preds[p];
-                long long lo = INT32_MIN, hi = INT32_MAX;
-                switch (cp.op) {
-                case SR_PRED_EQ: lo = hi = cp.ilo; break;
-                case SR_PRED_LT: hi = cp.ilo - 1; break;
-                case SR_PRED_LE: hi = cp.ilo; break;
-                case SR_PRED_GT: lo = cp.ilo + 1; break;
-                case SR_PRED_GE: lo = cp.ilo; break;
-                case SR_PRED_BETWEEN: lo = cp.ilo; hi = cp.ihi; break;
-                default: ok = false; break;
-                }
-                lo = std::max<long long>(lo, INT32_MIN);
-                hi = std::min<long long>(hi, INT32_MAX);
-                if (cp.is_double || !int32_class(cp.value_id) || lo > hi) ok = false;
+                long long lo, hi;
+                ok = pred_int32_range(cp, &lo, &hi) && int32_class(cp.value_id);
                 if (!ok) break;
                 srd::StreamTest& st = f->pass.tests[nt++];
                 st.kind = 0;

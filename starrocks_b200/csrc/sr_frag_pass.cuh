@@ -725,8 +725,9 @@ __global__ void __launch_bounds__(256) k_frag_build_digits(const uint32_t* __res
                     bad |= !d.nullable;
                 } else {
                     const int64_t v = load_int(d.data, d.type, b);
-                    idx = v - d.min + d.nullable;
-                    bad |= (v < d.min) || (idx >= d.extent);
+                    const unsigned long long off = (unsigned long long)v - (unsigned long long)d.min; // as agg_find_slot
+                    bad |= off >= (unsigned long long)(d.extent - d.nullable);
+                    idx = (long long)off + d.nullable;
                 }
                 slot += idx * d.stride;
             }

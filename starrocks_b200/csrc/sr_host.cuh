@@ -486,6 +486,31 @@ static int32_t compile_pred(sr_ctx* ctx, const sr_pred* p, VReg* reg, slot_type_
     return SR_OK;
 }
 
+// The int32 values [lo, hi] an integer EQ / LT / LE / GT / GE / BETWEEN conjunct selects: the "range form" of the scan
+// and streaming-pass tests.  False when the conjunct has no such form or selects no int32 value (the generic form then
+// evaluates it).  The constants are clamped to one past the int32 range first, so that LT INT64_MIN and GT INT64_MAX
+// cannot overflow into a range that selects every row.
+static bool pred_int32_range(const srd::CPred& cp, long long* lo_out, long long* hi_out) {
+    const auto clamp = [](long long c) { return std::min<long long>(std::max<long long>(c, (long long)INT32_MIN - 1), (long long)INT32_MAX + 1); };
+    const long long a = clamp(cp.ilo), b = clamp(cp.ihi);
+    long long lo = INT32_MIN, hi = INT32_MAX;
+    switch (cp.op) {
+    case SR_PRED_EQ: lo = hi = a; break;
+    case SR_PRED_LT: hi = a - 1; break;
+    case SR_PRED_LE: hi = a; break;
+    case SR_PRED_GT: lo = a + 1; break;
+    case SR_PRED_GE: lo = a; break;
+    case SR_PRED_BETWEEN: lo = a; hi = b; break;
+    default: return false;
+    }
+    lo = std::max<long long>(lo, INT32_MIN);
+    hi = std::min<long long>(hi, INT32_MAX);
+    if (cp.is_double || lo > hi) return false;
+    *lo_out = lo;
+    *hi_out = hi;
+    return true;
+}
+
 // fill a VTab from a staged chunk for the slots registered in reg
 static int32_t bind_vtab(sr_ctx* ctx, const VReg& reg, const Staged& st, VTab* vt) {
     vt->n = (int32_t)reg.slots.size();

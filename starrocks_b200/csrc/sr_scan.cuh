@@ -464,20 +464,9 @@ static int32_t scan_compile(sr_scan* s) {
         bool ok = s->exprs.empty() && !s->preds.empty() && s->preds.size() <= SR_MAX_SCAN_RANGE_TESTS;
         for (size_t k = 0; k < s->preds.size() && ok; k++) {
             const srd::CPred& cp = hp->preds[k];
-            long long lo = INT32_MIN, hi = INT32_MAX;
-            switch (cp.op) {
-            case SR_PRED_EQ: lo = hi = cp.ilo; break;
-            case SR_PRED_LT: hi = cp.ilo - 1; break;
-            case SR_PRED_LE: hi = cp.ilo; break;
-            case SR_PRED_GT: lo = cp.ilo + 1; break;
-            case SR_PRED_GE: lo = cp.ilo; break;
-            case SR_PRED_BETWEEN: lo = cp.ilo; hi = cp.ihi; break;
-            default: ok = false; break;
-            }
-            lo = std::max<long long>(lo, INT32_MIN);
-            hi = std::min<long long>(hi, INT32_MAX);
+            long long lo, hi;
             const int32_t t = s->reg.types[cp.value_id];
-            if (cp.is_double || srd::type_width(t) != 4 || srd::is_float_class(t) || lo > hi) ok = false;
+            ok = pred_int32_range(cp, &lo, &hi) && srd::type_width(t) == 4 && !srd::is_float_class(t);
             if (!ok) break;
             s->tests.t[k] = srd::RangeTest{cp.value_id, (uint32_t)(int32_t)lo, (uint32_t)(hi - lo)};
         }
