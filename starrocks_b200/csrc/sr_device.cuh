@@ -553,4 +553,33 @@ __device__ __forceinline__ uint32_t block_excl_scan(uint32_t v, uint32_t* smem, 
     return res;
 }
 
+// the same in 64 bits: for counts whose sum may pass 2^32 (output sizes the host must see exactly to refuse them)
+__device__ __forceinline__ unsigned long long warp_incl_scan64(unsigned long long v) {
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const unsigned long long t = __shfl_up_sync(SR_FULL_MASK, v, o);
+        if (lane_id() >= (uint32_t)o) v += t;
+    }
+    return v;
+}
+template <int BLOCK>
+__device__ __forceinline__ unsigned long long block_excl_scan64(unsigned long long v, unsigned long long* smem, unsigned long long* total) {
+    const unsigned long long incl = warp_incl_scan64(v);
+    const int w = threadIdx.x >> 5;
+    if (lane_id() == 31) smem[w] = incl;
+    __syncthreads();
+    if (w == 0) {
+        const int nw = BLOCK / 32;
+        const unsigned long long x = (int)lane_id() < nw ? smem[lane_id()] : 0;
+        const unsigned long long xi = warp_incl_scan64(x);
+        if ((int)lane_id() < nw) smem[lane_id()] = xi - x;
+        if ((int)lane_id() == nw - 1) smem[nw] = xi;
+    }
+    __syncthreads();
+    const unsigned long long res = incl - v + smem[w];
+    *total = smem[BLOCK / 32];
+    __syncthreads();
+    return res;
+}
+
 } // namespace srd

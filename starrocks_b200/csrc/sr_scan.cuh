@@ -33,18 +33,20 @@ struct ScanProg {
     CExpr exprs[8];
 };
 
-// single-block exclusive scan of `n` uint32 counts into uint64 offsets; total -> *total
+// single-block exclusive scan of `n` uint32 counts into uint64 offsets; total -> *total.  The scan is 64-bit inside each
+// 1024-count step as well: 1024 counts can sum past 2^32 (the probe blocks of a join with long chains), and a total that
+// wrapped would let the host size the output too small instead of refusing it.
 __global__ void __launch_bounds__(1024) k_scan_counts(const uint32_t* __restrict__ counts, int64_t n, uint64_t* __restrict__ offsets,
                                                        uint64_t* __restrict__ total) {
-    __shared__ uint32_t s_scan[1024 / 32 + 1];
+    __shared__ unsigned long long s_scan[1024 / 32 + 1];
     __shared__ uint64_t s_running;
     if (threadIdx.x == 0) s_running = 0;
     __syncthreads();
     for (int64_t base = 0; base < n; base += 1024) {
         const int64_t i = base + threadIdx.x;
         const uint32_t v = i < n ? counts[i] : 0;
-        uint32_t tot;
-        const uint32_t ex = block_excl_scan<1024>(v, s_scan, &tot);
+        unsigned long long tot;
+        const unsigned long long ex = block_excl_scan64<1024>(v, s_scan, &tot);
         const uint64_t run = s_running;
         if (i < n) offsets[i] = run + ex;
         __syncthreads();
@@ -199,15 +201,27 @@ __global__ void __launch_bounds__(SCANW_BLOCK) k_scan_mask(const ScanProg* __res
     }
 }
 
-// exclusive scan inside blocks of 1024 counts; block_sums[b] = total of block b
+// exclusive scan inside blocks of 1024 counts; block_sums[b] = total of block b.  SAT_SUM: the total is summed in 64 bits
+// and stored saturated at 0xFFFFFFFF, so that counts passing 2^32 in one block cannot wrap to a small total (scan_counts:
+// the host refuses such an output, and the wrapped offsets inside the block are never used)
+template <bool SAT_SUM>
 __global__ void __launch_bounds__(1024) k_scan_lvl1(const uint32_t* __restrict__ counts, int64_t n, uint32_t* __restrict__ local_excl, uint32_t* __restrict__ block_sums) {
     __shared__ uint32_t s_scan[1024 / 32 + 1];
+    __shared__ unsigned long long s_sum;
     const int64_t i = (int64_t)blockIdx.x * 1024 + threadIdx.x;
     const uint32_t v = i < n ? counts[i] : 0;
+    if (SAT_SUM && threadIdx.x == 0) s_sum = 0;
     uint32_t tot;
-    const uint32_t ex = block_excl_scan<1024>(v, s_scan, &tot);
+    const uint32_t ex = block_excl_scan<1024>(v, s_scan, &tot); // (synchronises the block: s_sum is initialised)
     if (i < n) local_excl[i] = ex;
-    if (threadIdx.x == 0) block_sums[blockIdx.x] = tot;
+    if (SAT_SUM) {
+        const unsigned long long ws = warp_sum((unsigned long long)v);
+        if (lane_id() == 0) atomicAdd(&s_sum, ws);
+        __syncthreads();
+        if (threadIdx.x == 0) block_sums[blockIdx.x] = s_sum > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)s_sum;
+    } else if (threadIdx.x == 0) {
+        block_sums[blockIdx.x] = tot;
+    }
 }
 
 // offsets[i] = base of i's 1024-block + position inside the block (second half of the two-level scan)
@@ -399,7 +413,7 @@ static int32_t scan_counts(sr_ctx* ctx, ScanScratch* sc, const uint32_t* counts,
     SR_TRY(sc->local.reserve(ctx, sizeof(uint32_t) * (size_t)n));
     SR_TRY(sc->sums.reserve(ctx, sizeof(uint32_t) * (size_t)nblk));
     SR_TRY(sc->bases.reserve(ctx, sizeof(uint64_t) * (size_t)nblk));
-    srd::k_scan_lvl1<<<(int)nblk, 1024, 0, ctx->stream>>>(counts, n, sc->local.as<uint32_t>(), sc->sums.as<uint32_t>());
+    srd::k_scan_lvl1<true><<<(int)nblk, 1024, 0, ctx->stream>>>(counts, n, sc->local.as<uint32_t>(), sc->sums.as<uint32_t>());
     SR_LAUNCH_CHECK(ctx);
     srd::k_scan_counts<<<1, 1024, 0, ctx->stream>>>(sc->sums.as<uint32_t>(), nblk, sc->bases.as<uint64_t>(), ctx->dscratch);
     SR_LAUNCH_CHECK(ctx);
@@ -552,7 +566,7 @@ static int32_t scan_select(sr_scan* s, const sr_chunk_view* in, bool want_counts
     }
     if (want_counts) {
         if (n > 0) {
-            srd::k_scan_lvl1<<<(int)nblk, 1024, 0, ctx->stream>>>(s->tile_counts.as<uint32_t>(), tiles, s->local_excl.as<uint32_t>(), s->block_sums.as<uint32_t>());
+            srd::k_scan_lvl1<false><<<(int)nblk, 1024, 0, ctx->stream>>>(s->tile_counts.as<uint32_t>(), tiles, s->local_excl.as<uint32_t>(), s->block_sums.as<uint32_t>());
             SR_LAUNCH_CHECK(ctx);
             srd::k_scan_counts<<<1, 1024, 0, ctx->stream>>>(s->block_sums.as<uint32_t>(), nblk, s->block_offsets.as<uint64_t>(), ctx->dscratch);
             SR_LAUNCH_CHECK(ctx);
