@@ -438,7 +438,9 @@ static int32_t frag_plan(sr_fragment* f, const VTab& vt, int64_t n) {
             }
             f->pass.num_tests = ok ? nt : 0;
             // the second test's column is streamed with vector loads as well when >= 8 % of the rows reach it
-            // (most of its 64-byte DRAM bursts would be touched anyway, and the loads do not wait for test 0)
+            // (most of its 64-byte DRAM bursts would be touched anyway, and the loads do not wait for test 0).  HBM does
+            // move 64 bytes per access: on H100, reading every other 32-byte sector of a column costs 1.03x reading all of
+            // it (scripts/hbm_sector_probe.cu), so fetching this column by the sector for the rows test 0 passed saves nothing
             double reach1 = 1.0;
             if (ok && nt > 1) reach1 = f->pass.tests[0].kind == 0 ? (double)counts[16] / (double)std::max<int64_t>(sample, 1) : f->pred_rate * f->pass_rate[ord[0]];
             f->pass.num_vec = (ok && nt > 1 && reach1 >= 0.08) ? 2 : 1;
@@ -461,9 +463,10 @@ static int32_t frag_plan(sr_fragment* f, const VTab& vt, int64_t n) {
         }
         f->gather_joins.clear();
         for (int q = ns; q < ff; q++) f->gather_joins.push_back(q);
-        // streaming pass shared memory: bitmaps of the streamed joins only
+        // streaming pass shared memory: bitmaps of the streamed joins only (less the carried-key stash of
+        // k_frag_stream_tests<true>, so that two CTAs still fit on an SM)
         size_t sw = 0;
-        const size_t sbudget = (100 * 1024) / 4;
+        const size_t sbudget = (100 * 1024 - (f->pass.carry_join >= 0 ? sizeof(int4) * srd::STREAM_GROUPS * srd::STREAM_BLOCK : 0)) / 4;
         for (int q = 0; q < f->num_joins; q++) {
             srd::FragJoinDev& fj = h.joins[q];
             fj.smem_off = -1;
@@ -473,6 +476,29 @@ static int32_t frag_plan(sr_fragment* f, const VTab& vt, int64_t n) {
             }
         }
         f->stream_smem = sw * 4;
+        for (int v = 0; v < 2 && f->pass.num_tests > 0; v++) {
+            const srd::StreamTest& st = f->pass.tests[v < f->pass.num_vec ? v : 0];
+            srd::VecTest& t = f->pass.vec[v];
+            t.kind = st.kind == 0 ? 0 : 3;
+            t.lo = st.lo;
+            t.span = st.span;
+            t.smem_off = -1;
+            t.bm = nullptr;
+            if (st.kind == 1) {
+                const srd::FragJoinDev& fj = h.joins[st.join];
+                if (fj.use_bitmap && fj.idx32) {
+                    t.lo = (uint32_t)(int32_t)fj.j.min_value;
+                    t.span = (uint32_t)(fj.j.max_value - fj.j.min_value);
+                    if (fj.smem_off >= 0 && t.span != 0xFFFFFFFFu) {
+                        t.kind = 1;
+                        t.smem_off = fj.smem_off;
+                    } else {
+                        t.kind = 2;
+                        t.bm = fj.j.bitmap;
+                    }
+                }
+            }
+        }
         f->smem_agg = f->agg->smem_bytes > 0;
         f->smem_bytes = f->agg->smem_bytes;
         f->queue_word_off = 0;
@@ -578,11 +604,8 @@ static int32_t frag_push(sr_fragment* f, const sr_chunk_view* fact) {
         const size_t slack = (size_t)srd::SEL_CHUNK * ((size_t)f->stream_grid * (srd::STREAM_BLOCK / 32) + (size_t)f->grid * (srd::GATHER_BLOCK / 32));
         SR_TRY(f->sel[0].reserve(ctx, sizeof(srd::SelEntry) * ((size_t)n + slack)));
         if (!f->gather_joins.empty()) SR_TRY(f->sel[1].reserve(ctx, sizeof(srd::SelEntry) * ((size_t)n + slack)));
-        // this push's pass parameters: the carried key (planned in f->pass) is only used for host-resident input
-        srd::PassDev pass = f->pass;
-        pass.host_input = fact->mem == SR_MEM_HOST_PINNED ? 1 : 0;
-        const bool carry = pass.host_input && pass.carry_join >= 0; // (HBM input: the register cost in the stream pass outweighs the saved re-read)
-        if (!carry) pass.carry_join = pass.carry_value_id = -1;
+        const srd::PassDev& pass = f->pass;
+        const bool carry = pass.carry_join >= 0;
         unsigned long long* cnt = f->pass_counters.as<unsigned long long>();
         SR_CUDA(ctx, cudaMemsetAsync(cnt, 0, 16 * sizeof(uint64_t), ctx->stream));
         const int sgrid = (int)std::min<int64_t>(f->stream_grid, (n + srd::STREAM_TILE - 1) / srd::STREAM_TILE);

@@ -30,9 +30,23 @@ struct StreamTest {
 };
 #define SR_MAX_STREAM_TESTS 6
 
+// How k_frag_stream_tests runs one of its two vector-column tests, planned on the host (frag_plan) and read from the kernel
+// parameter: nothing of it occupies a register of the issue-bound, register-capped kernel, and nothing is re-read from
+// shared memory per tile.  kind: 0 = range conjunct, 1 = bitmap in shared memory at word smem_off (int32 index arithmetic,
+// zero GUARD bit at index span + 1: an out-of-range key is clamped onto it, so the test needs neither a predicate nor a
+// select), 2 = bitmap in global memory at bm (predicated word fetches, issued back to back), 3 = anything else (falls back
+// to stream_test).  lo / span: the range, or the join table's [min, min + span].
+struct VecTest {
+    uint32_t kind;
+    uint32_t lo, span;
+    int32_t smem_off;
+    const uint32_t* bm;
+};
+
 struct PassDev {
     int32_t num_tests; // > 0: the streaming pass can run as k_frag_stream_tests (subject to the batch's nullability)
     int32_t num_vec;   // its first num_vec (1 or 2) tests read their column with prefetched 128-bit loads
+    VecTest vec[2];    // tests 0 and (num_vec > 1 ? 1 : 0) in the form k_frag_stream_tests runs them
     StreamTest tests[SR_MAX_STREAM_TESTS];
     int32_t num_stream_joins; // joins [0, num_stream_joins) are tested by the streaming pass
     int32_t final_first_join; // joins [final_first_join, S) are tested inline by the final pass
@@ -40,12 +54,11 @@ struct PassDev {
     // depends on them)
     int8_t final_vals[8];  // value ids, -1 = unused
     int8_t num_final_vals; // how many the final pass needs (may exceed 8: then only the generic final pass applies)
-    int8_t host_input; // the fact columns of this push live in pinned host memory (SR_MEM_HOST_PINNED)
     // the int32 key of one streamed join whose build row the final pass needs travels in the upper half of the
     // selection-vector entries, so the final pass does not gather it from the fact table again
     int8_t carry_join;     // index of that join among the streamed joins, -1 = none
     int8_t carry_value_id; // its key's value id
-    int8_t pad[1];
+    int8_t pad[2];
 };
 
 // selection-vector entry: row id (low 32 bits) + carried key (high 32 bits)
@@ -199,41 +212,30 @@ struct WarpSelWriter {
     }
 };
 
-// append the rows flagged in `alive` (bit i -> row base_i + (i & 3)) with their carried keys to the selection vector
-template <bool CARRY>
-__device__ __forceinline__ void warp_append_rows(uint32_t alive_all, int64_t row0_g0, int64_t row0_g1,
-                                                 const int32_t (&carry)[STREAM_GROUPS * STREAM_ROWS], WarpSelWriter& w) {
+// append the rows flagged in `alive` (bit i -> row base_i + (i & 3)) with their carried keys (key_at(i), i not a
+// compile-time constant) to the selection vector
+template <bool CARRY, typename KeyAt>
+__device__ __forceinline__ void warp_append_rows(uint32_t alive_all, int64_t row0_g0, int64_t row0_g1, KeyAt key_at, WarpSelWriter& w) {
     const uint32_t cnt = __popc(alive_all);
     const uint32_t incl = warp_incl_scan(cnt);
     const uint32_t total = __shfl_sync(SR_FULL_MASK, incl, 31);
     if (total == 0) return;
     SelEntry* __restrict__ sel_out = w.out + (w.reserve(total) + incl - cnt);
-    if (CARRY) {
-        uint32_t pos = 0;
-#pragma unroll
-        for (int i = 0; i < STREAM_GROUPS * STREAM_ROWS; i++) {
-            if ((alive_all >> i) & 1u) {
-                const int64_t row = (i < STREAM_ROWS ? row0_g0 : row0_g1) + (i & (STREAM_ROWS - 1));
-                sel_out[pos++] = sel_make((uint32_t)row, carry[i]);
-            }
-        }
-    } else {
-        // few rows survive (a lane holds 0..2 of its 8): walk the set bits instead of testing all eight
-        const uint32_t r0 = (uint32_t)row0_g0, r1 = (uint32_t)row0_g1 - STREAM_ROWS;
-        uint32_t m = alive_all, pos = 0;
-        while (m) {
-            const uint32_t i = (uint32_t)__ffs((int)m) - 1u;
-            m &= m - 1u;
-            sel_out[pos++] = (SelEntry)((i < STREAM_ROWS ? r0 : r1) + i);
-        }
+    // few rows survive (a lane holds 0..2 of its 8): walk the set bits instead of testing all eight
+    const uint32_t r0 = (uint32_t)row0_g0, r1 = (uint32_t)row0_g1 - STREAM_ROWS;
+    uint32_t m = alive_all, pos = 0;
+    while (m) {
+        const uint32_t i = (uint32_t)__ffs((int)m) - 1u;
+        m &= m - 1u;
+        const uint32_t row = (i < STREAM_ROWS ? r0 : r1) + i;
+        sel_out[pos++] = CARRY ? sel_make(row, key_at(i)) : (SelEntry)row;
     }
 }
 
-// CARRY: the key of streamed join pd.carry_join rides in the upper half of the entries.  Only instantiated for
-// host-resident input: holding the tile's keys in registers through the append costs the streaming kernel ~25 %
-// when it runs at HBM speed (register spills; re-reading the key for the survivors instead was worse still, it puts
-// an L2 round trip on every tile's critical path) but nothing when the kernel waits on PCIe, and there every sector
-// the final pass does not have to fetch is worth ~2.5 ns of bus time.
+// CARRY: the key of streamed join pd.carry_join rides in the upper half of the entries, so the final pass does not
+// gather it from the fact table again (one random 32-byte sector per surviving row from HBM, ~2.5 ns of bus time per
+// sector from pinned host memory).  (Re-reading the key for the survivors in this pass instead puts an L2 round trip
+// on every tile's critical path.)
 template <bool CARRY>
 __global__ void __launch_bounds__(STREAM_BLOCK, 2) k_frag_stream(const FragDev* __restrict__ fdp, PassDev pd, const __grid_constant__ VTab vt, int64_t n,
                                                                  SelEntry* __restrict__ sel_out, unsigned long long* __restrict__ counter) {
@@ -335,7 +337,13 @@ __global__ void __launch_bounds__(STREAM_BLOCK, 2) k_frag_stream(const FragDev* 
             }
         }
         static_assert(STREAM_GROUPS == 2, "two groups of alive bits are packed into one word");
-        warp_append_rows<CARRY>(alive[0] | (alive[1] << STREAM_ROWS), row0[0], row0[1], carry, writer);
+        auto key_at = [&](uint32_t i) { // a select chain: indexing the register array with i would put it in local memory
+            int32_t v = carry[0];
+#pragma unroll
+            for (int k = 1; k < STREAM_GROUPS * STREAM_ROWS; k++) v = i == (uint32_t)k ? carry[k] : v;
+            return v;
+        };
+        warp_append_rows<CARRY>(alive[0] | (alive[1] << STREAM_ROWS), row0[0], row0[1], key_at, writer);
     }
     writer.finish();
 }
@@ -358,45 +366,10 @@ __device__ __forceinline__ uint32_t stream_test(const StreamTest& st, const Frag
     return join_test_batch<N>(s_joins[st.join], smem, k, alive);
 }
 
-// The two vector-column tests of k_frag_stream_tests with their parameters held in REGISTERS for the whole kernel.  The
-// kernel is issue bound, and otherwise re-reads the warp-uniform test descriptors from shared memory on every call (the
-// compiler cannot hoist them over the selection-vector stores) next to the shared-memory bitmap test.  kind: 0 = range conjunct, 1 = bitmap in shared memory (int32 index
-// arithmetic, zero GUARD bit at index span + 1: an out-of-range key is clamped onto it, so the test needs neither a
-// predicate nor a select), 2 = bitmap in global memory (predicated word fetches, issued back to back), 3 = anything else
-// (falls back to stream_test).
-struct TestReg {
-    uint32_t kind;
-    uint32_t lo, span;
-    const uint32_t* bm;
-};
-
-__device__ __forceinline__ TestReg make_test_reg(const StreamTest& st, const FragJoinDev* s_joins, const uint32_t* smem) {
-    TestReg t;
-    t.kind = 3;
-    t.lo = st.lo;
-    t.span = st.span;
-    t.bm = nullptr;
-    if (st.kind == 0) {
-        t.kind = 0;
-    } else {
-        const FragJoinDev& fj = s_joins[st.join];
-        if (fj.use_bitmap && fj.idx32) {
-            t.lo = (uint32_t)(int32_t)fj.j.min_value;
-            t.span = (uint32_t)(fj.j.max_value - fj.j.min_value);
-            if (fj.smem_off >= 0 && t.span != 0xFFFFFFFFu) {
-                t.kind = 1;
-                t.bm = smem + fj.smem_off;
-            } else {
-                t.kind = 2;
-                t.bm = fj.j.bitmap;
-            }
-        }
-    }
-    return t;
-}
-
+// one of the two vector-column tests of k_frag_stream_tests in the form the host planned (VecTest); sbm = smem +
+// t.smem_off
 template <int N>
-__device__ __forceinline__ uint32_t stream_test_reg(const TestReg& t, const StreamTest& st, const FragJoinDev* s_joins, const uint32_t* smem,
+__device__ __forceinline__ uint32_t stream_test_reg(const VecTest& t, const uint32_t* sbm, const StreamTest& st, const FragJoinDev* s_joins, const uint32_t* smem,
                                                     const int32_t (&k)[N], uint32_t alive) {
     uint32_t out = 0;
     if (t.kind == 1) {
@@ -404,7 +377,7 @@ __device__ __forceinline__ uint32_t stream_test_reg(const TestReg& t, const Stre
 #pragma unroll
         for (int i = 0; i < N; i++) {
             const uint32_t idx = min((uint32_t)k[i] - t.lo, guard);
-            const uint32_t word = t.bm[idx >> 5];
+            const uint32_t word = sbm[idx >> 5];
             out |= __funnelshift_r(word, word, idx - (uint32_t)i) & (1u << i);
         }
         return out & alive;
@@ -431,12 +404,17 @@ __device__ __forceinline__ uint32_t stream_test_reg(const TestReg& t, const Stre
     return stream_test<N>(st, s_joins, smem, k, alive);
 }
 
+// CARRY: the carried keys wait for the append in a per-thread STASH in shared memory (16 KB per CTA), not in registers.
+// At two 512-thread CTAs per SM the kernel has 64 registers, and eight more live from the carried test to the append
+// spilled: the spill stores of the prefetched vectors then waited on their loads on every tile.  Two 128-bit shared stores
+// per tile instead, and a shared load per surviving row.
 template <bool CARRY>
-__global__ void __launch_bounds__(STREAM_BLOCK, 2) k_frag_stream_tests(const FragDev* __restrict__ fdp, PassDev pd, const __grid_constant__ VTab vt, int64_t n,
+__global__ void __launch_bounds__(STREAM_BLOCK, 2) k_frag_stream_tests(const FragDev* __restrict__ fdp, const __grid_constant__ PassDev pd, const __grid_constant__ VTab vt, int64_t n,
                                                                        SelEntry* __restrict__ sel_out, unsigned long long* __restrict__ counter) {
     extern __shared__ __align__(16) uint32_t smem[];
     __shared__ FragJoinDev s_joins[STREAM_MAX_JOINS];
     __shared__ StreamTest s_tests[SR_MAX_STREAM_TESTS];
+    __shared__ int4 s_carry[CARRY ? STREAM_GROUPS * STREAM_BLOCK : 1]; // [group][thread]: the keys of the thread's 4 rows
     const FragDev& fd = *fdp;
     const int SJ = pd.num_stream_joins;
     const int NT = pd.num_tests;
@@ -449,8 +427,10 @@ __global__ void __launch_bounds__(STREAM_BLOCK, 2) k_frag_stream_tests(const Fra
             for (int w = threadIdx.x; w <= fj.bitmap_words; w += blockDim.x) smem[fj.smem_off + w] = w < fj.bitmap_words ? fj.j.bitmap[w] : 0u;
     }
     __syncthreads();
-    const TestReg t0 = make_test_reg(s_tests[0], s_joins, smem);
-    const TestReg t1 = make_test_reg(s_tests[NV > 1 ? 1 : 0], s_joins, smem);
+    const VecTest& t0 = pd.vec[0];
+    const VecTest& t1 = pd.vec[1];
+    const uint32_t* sbm0 = smem + (t0.kind == 1 ? t0.smem_off : 0);
+    const uint32_t* sbm1 = smem + (t1.kind == 1 ? t1.smem_off : 0);
     const bool carry0 = CARRY && s_tests[0].kind == 1 && s_tests[0].join == pd.carry_join;
     const bool carry1 = CARRY && NV > 1 && s_tests[1].kind == 1 && s_tests[1].join == pd.carry_join;
     const int32_t* col0 = (const int32_t*)vt.v[pd.tests[0].value_id].data;
@@ -485,29 +465,19 @@ __global__ void __launch_bounds__(STREAM_BLOCK, 2) k_frag_stream_tests(const Fra
 #pragma unroll
         for (int g = 0; g < STREAM_GROUPS; g++)
             row0[g] = tile * STREAM_TILE + (int64_t)g * (STREAM_BLOCK * STREAM_ROWS) + (int64_t)threadIdx.x * STREAM_ROWS;
-        int32_t carry[8];
-        if (CARRY) {
-#pragma unroll
-            for (int i = 0; i < 8; i++) carry[i] = 0;
-        }
         uint32_t a8 = 0xFFu;
         int first_pred = 0; // tests [first_pred, NT) load their column for the live rows only
         if (tile < full_tiles) {
+#pragma unroll
+            for (int g = 0; g < STREAM_GROUPS; g++) {
+                if (carry0) s_carry[g * STREAM_BLOCK + threadIdx.x] = pk[0][g];
+                if (carry1) s_carry[g * STREAM_BLOCK + threadIdx.x] = pk[1][g];
+            }
             const int32_t k0[8] = {pk[0][0].x, pk[0][0].y, pk[0][0].z, pk[0][0].w, pk[0][1].x, pk[0][1].y, pk[0][1].z, pk[0][1].w};
             const int32_t k1[8] = {pk[1][0].x, pk[1][0].y, pk[1][0].z, pk[1][0].w, pk[1][1].x, pk[1][1].y, pk[1][1].z, pk[1][1].w};
             prefetch(tile + 1); // the next tile's vector columns stay in flight while this tile is tested
-            a8 = stream_test_reg<8>(t0, s_tests[0], s_joins, smem, k0, 0xFFu);
-            if (carry0) {
-#pragma unroll
-                for (int i = 0; i < 8; i++) carry[i] = k0[i];
-            }
-            if (NV > 1) {
-                a8 = stream_test_reg<8>(t1, s_tests[1], s_joins, smem, k1, a8);
-                if (carry1) {
-#pragma unroll
-                    for (int i = 0; i < 8; i++) carry[i] = k1[i];
-                }
-            }
+            a8 = stream_test_reg<8>(t0, sbm0, s_tests[0], s_joins, smem, k0, 0xFFu);
+            if (NV > 1) a8 = stream_test_reg<8>(t1, sbm1, s_tests[1], s_joins, smem, k1, a8);
             first_pred = NV;
         } else { // the ragged last tile: every test through predicated loads
             a8 = 0;
@@ -525,10 +495,11 @@ __global__ void __launch_bounds__(STREAM_BLOCK, 2) k_frag_stream_tests(const Fra
             a8 = stream_test<8>(st, s_joins, smem, kk, a8);
             if (CARRY && st.kind == 1 && st.join == pd.carry_join) {
 #pragma unroll
-                for (int i = 0; i < 8; i++) carry[i] = kk[i];
+                for (int g = 0; g < STREAM_GROUPS; g++) s_carry[g * STREAM_BLOCK + threadIdx.x] = make_int4(kk[4 * g], kk[4 * g + 1], kk[4 * g + 2], kk[4 * g + 3]);
             }
         }
-        warp_append_rows<CARRY>(a8, row0[0], row0[1], carry, writer);
+        const int32_t* stash = (const int32_t*)s_carry + STREAM_ROWS * threadIdx.x;
+        warp_append_rows<CARRY>(a8, row0[0], row0[1], [&](uint32_t i) { return stash[(i >> 2) * (STREAM_ROWS * STREAM_BLOCK) + (i & 3)]; }, writer);
     }
     writer.finish();
 }
@@ -571,6 +542,8 @@ __global__ void __launch_bounds__(GATHER_BLOCK) k_frag_gather_join(const FragDev
         if (i < n_in) entry = sel_in[i];
         const uint32_t row = sel_row(entry);
         if (row != SEL_INVALID) {
+            // (an L2::evict_first policy on this single-use load, and on the final pass's fact loads, to keep bitmaps and
+            // directories resident changed neither pass on H100: 0.569 / 0.752 ms against 0.569 / 0.748 ms)
             const int64_t key = load_int(d.data, d.type, (int64_t)row);
             const bool nul = d.nulls != nullptr && d.nulls[row] != 0;
             hit = !nul && join_hit_global(fj, key); // global bitmap copy: L1/L2 resident
