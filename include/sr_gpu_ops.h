@@ -88,7 +88,11 @@ int32_t sr_type_width(int32_t type);
 typedef enum sr_mem { SR_MEM_HOST = 0, SR_MEM_DEVICE = 1, SR_MEM_HOST_PINNED = 2 } sr_mem;
 
 /* mirrors FixedLengthColumn / NullableColumn raw buffers (be/src/column/nullable_column.h:32:
- * data column + uint8 null column, 1 = null). nulls == NULL means "not nullable / no nulls". */
+ * data column + uint8 null column, 1 = null). nulls == NULL means "not nullable / no nulls".
+ * Alignment: a column the kernels read in place (SR_MEM_DEVICE, and SR_MEM_HOST_PINNED where it is read in place) must be
+ * naturally aligned: `data` a multiple of the value width, of 8 bytes for 16-byte values (so row k of a larger column
+ * qualifies).  Such a column that is not is refused with SR_ERR_INVALID_ARGUMENT before any launch.  SR_MEM_HOST columns
+ * are copied and may have any alignment. */
 typedef struct sr_col_view {
     const void* data;
     const uint8_t* nulls;
@@ -420,7 +424,8 @@ void sr_rf_destroy(sr_rf* rf);
 int32_t sr_rf_get_info(sr_rf* rf, sr_rf_info* info);
 /* bloom directory: copy out (bytes = 32 << log_num_buckets) / merge another filter in: OR of the directories
  * (SimdBlockFilter::merge; `mem` says where `directory` lives; NULL when `other` has no bloom part) and union of
- * min/max/has_null/num_inserted taken from `other` -- the wire-compatible parts of serialize / merge. */
+ * min/max/has_null/num_inserted taken from `other` -- the wire-compatible parts of serialize / merge.  A SR_MEM_DEVICE
+ * directory is read in place and must be 4-byte aligned, else SR_ERR_INVALID_ARGUMENT. */
 int32_t sr_rf_copy_directory(sr_rf* rf, void* dst, int64_t bytes, int32_t mem);
 int32_t sr_rf_merge_directory(sr_rf* rf, const void* directory, int64_t bytes, int32_t mem, const sr_rf_info* other);
 /* RuntimeFilter::evaluate on one column of a chunk: selection[i] = has_null for NULL rows, else min <= v <= max and
@@ -693,7 +698,9 @@ void sr_xchg_destroy(sr_xchg* x);
  * hash of the partition columns, Shuffler::exchange_shuffle (shuffler.h:72-89), per-channel row index lists.
  * Partition one batch.  out: DEVICE buffers, all columns of `in` reordered so that the rows
  * of channel c occupy [offsets[c], offsets[c+1]) in input order (stable, like the reference's
- * counting sort).  channel_offsets_host: num_channels + 1 int64 written on return (syncs). */
+ * counting sort).  channel_offsets_host: num_channels + 1 int64 written on return (syncs).  A batch of zero rows gives
+ * zero-row columns whose `data` may be NULL; a nullable input column still gets a non-NULL (empty) `nulls`, so every
+ * batch's output, and every channel's ChunkPB, has the same null columns. */
 int32_t sr_xchg_partition(sr_xchg* x, const sr_chunk_view* in, sr_chunk_out* out, int64_t* channel_offsets_host);
 /* hash values + channel ids only (device or host arrays of num_rows uint32, per `mem`). */
 int32_t sr_xchg_hash(sr_xchg* x, const sr_chunk_view* in, uint32_t* hash_values, uint32_t* channel_ids, int32_t mem);
@@ -780,7 +787,10 @@ int32_t sr_chunk_serialize(sr_ctx* ctx, const sr_chunk_view* chunk, int64_t row_
                            int32_t dst_mem, sr_chunk_pb_meta* meta);
 /* Parse ChunkPB.data (src in src_mem) described by `meta` (num_cols, slot_ids, types, is_nulls) into device columns owned by
  * `handle` (valid until its next deserialize / destroy); checks version, sizes and bounds like the reference's
- * deserialize (SR_ERR_INVALID_ARGUMENT on a malformed payload). */
+ * deserialize (SR_ERR_INVALID_ARGUMENT on a malformed payload).  The payload must be exactly the columns `meta` describes:
+ * bytes == meta->serialized_size, header num_rows == meta->num_rows and no bytes after the last column, else
+ * SR_ERR_INVALID_ARGUMENT.  A const column (meta->is_consts[k] != 0) gives SR_ERR_NOT_SUPPORTED.  A refused payload
+ * leaves no copy queued. */
 typedef struct sr_serde sr_serde;
 sr_serde* sr_serde_create(sr_ctx* ctx);
 void sr_serde_destroy(sr_serde* handle);
@@ -788,7 +798,8 @@ int32_t sr_chunk_deserialize(sr_serde* handle, const void* src, int64_t bytes, i
 
 /* ---------------------------------------------------------------------------------------
  * K11: Column::append_selective gather (be/src/column/fixed_length_column_base.cpp:54):
- * dst[j] = src[index[j]] for one column; all pointers in `mem`.
+ * dst[j] = src[index[j]] for one column; all pointers in `mem` (SR_MEM_DEVICE only) and naturally aligned (see
+ * sr_col_view), else SR_ERR_INVALID_ARGUMENT.
  * ------------------------------------------------------------------------------------- */
 int32_t sr_gather(sr_ctx* ctx, const void* src, int32_t type, const uint32_t* index, int64_t n, void* dst,
                   int32_t mem);

@@ -391,7 +391,8 @@ int32_t sr_scan_filter(sr_scan* s, const sr_chunk_view* in, sr_chunk_out* out) {
         if (c < 0) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "chunk misses output slot %d", s->out_slots[k]);
         const srd::DCol& dc = s->staged.cols[c];
         SR_TRY(s->out_bufs[2 * k].reserve(ctx, (size_t)std::max<int64_t>(total, 1) * dc.width));
-        ca.c[ca.n++] = srd::CompactCol{dc.data, s->out_bufs[2 * k].p, dc.width, 0};
+        const int32_t vec16 = dc.width == 16 && (((uintptr_t)dc.data | (uintptr_t)s->out_bufs[2 * k].p) & 15) == 0 ? 1 : 0;
+        ca.c[ca.n++] = srd::CompactCol{dc.data, s->out_bufs[2 * k].p, dc.width, vec16};
         out->cols[k].data = s->out_bufs[2 * k].p;
         out->cols[k].nulls = nullptr;
         out->cols[k].type = dc.type;
@@ -668,6 +669,7 @@ int32_t sr_rf_merge_directory(sr_rf* rf, const void* directory, int64_t bytes, i
     if (other->log_num_buckets != rf->log_num_buckets) // SimdBlockFilter::merge DCHECKs equal sizes
         return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "bloom directories of different size (2^%d vs 2^%d buckets)", rf->log_num_buckets, other->log_num_buckets);
     if (bytes != (int64_t)rf->dir_bytes() || (bytes > 0 && !directory)) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "directory is %zu bytes, caller passed %lld", rf->dir_bytes(), (long long)bytes);
+    if (mem == SR_MEM_DEVICE && !col_aligned(directory, 4)) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "device directory at %p is not 4-byte aligned", directory);
     rf->stats_valid = false;
     if (bytes > 0) {
         DevBuf tmp;
@@ -758,6 +760,8 @@ int32_t sr_join_key_hash(sr_ctx* ctx, const void* keys, int32_t key_type, int64_
     if ((w != 4 && w != 8) || srd::is_float_class(key_type)) return sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "sr_join_key_hash: 4- or 8-byte integer keys only");
     if (log_bucket_size < 1 || log_bucket_size > 31) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "log_bucket_size %u", log_bucket_size);
     if (n <= 0) return SR_OK;
+    if (mem != SR_MEM_HOST && (!col_aligned(keys, w) || !col_aligned(buckets, 4)))
+        return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "sr_join_key_hash: device keys or buckets are not naturally aligned");
     DevBuf kin, kout;
     const void* dk = keys;
     uint32_t* dout = buckets;
@@ -1194,8 +1198,7 @@ int32_t sr_agg_push_selective(sr_agg* a, const sr_chunk_view* chunk, sr_chunk_ou
         out->cols[k].nulls = g.dst_nulls;
         ga.c[ga.n++] = g;
     }
-    srd::k_gather<<<dim3(std::min(grid_for(m, 256), ctx->num_sms * 16), ga.n), 256, 0, ctx->stream>>>(a->sel_index.as<uint32_t>(), m, ga);
-    SR_LAUNCH_CHECK(ctx);
+    SR_TRY(launch_gather(ctx, a->sel_index.as<uint32_t>(), m, ga));
     if (chunk->mem != SR_MEM_DEVICE) SR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     return SR_OK;
 }
@@ -1472,9 +1475,16 @@ int32_t sr_xchg_partition(sr_xchg* x, const sr_chunk_view* in, sr_chunk_out* out
         for (size_t i = 0; i < x->out_bufs.size(); i++) std::swap(nb[i], x->out_bufs[i]);
         x->out_bufs.swap(nb);
     }
-    if (n <= 0) {
+    if (n <= 0) { // zero rows of every column; a nullable column keeps a (zero-row) null column
         for (int c = 0; c <= nch; c++) channel_offsets_host[c] = 0;
-        for (int k = 0; k < in->num_cols; k++) out->cols[k] = sr_col_out{nullptr, nullptr, in->cols[k].type, in->cols[k].slot_id};
+        for (int k = 0; k < in->num_cols; k++) {
+            uint8_t* nulls = nullptr;
+            if (in->cols[k].nulls) {
+                SR_TRY(x->out_bufs[2 * k + 1].reserve(ctx, 16));
+                nulls = (uint8_t*)x->out_bufs[2 * k + 1].p;
+            }
+            out->cols[k] = sr_col_out{nullptr, nulls, in->cols[k].type, in->cols[k].slot_id};
+        }
         return SR_OK;
     }
     const int tiles = grid_for(n, srd::PART_TILE);
@@ -1512,8 +1522,7 @@ int32_t sr_xchg_partition(sr_xchg* x, const sr_chunk_view* in, sr_chunk_out* out
         ga.c[ga.n++] = g;
         out->cols[k] = sr_col_out{g.dst, g.dst_nulls, dc.type, x->staged.slots[k]};
     }
-    srd::k_gather<<<dim3(std::min(grid_for(n, 256), ctx->num_sms * 16), ga.n), 256, 0, ctx->stream>>>(x->row_index.as<uint32_t>(), n, ga);
-    SR_LAUNCH_CHECK(ctx);
+    SR_TRY(launch_gather(ctx, x->row_index.as<uint32_t>(), n, ga));
     SR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     for (int c = 0; c < nch; c++) channel_offsets_host[c] = (int64_t)starts[c];
     channel_offsets_host[nch] = n;
@@ -1527,12 +1536,12 @@ int32_t sr_gather(sr_ctx* ctx, const void* src, int32_t type, const uint32_t* in
     if (w == 0) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "unknown type %d", type);
     if (mem != SR_MEM_DEVICE) return sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "sr_gather takes device pointers");
     if (n <= 0) return SR_OK;
+    if (!col_aligned(src, w) || !col_aligned(dst, w) || !col_aligned(index, 4))
+        return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "sr_gather: a device pointer is not naturally aligned for width %d", w);
     srd::GatherArgs ga;
     ga.n = 1;
-    ga.c[0] = srd::GatherCol{src, nullptr, dst, nullptr, w, 0};
-    srd::k_gather<<<dim3(std::min(grid_for(n, 256), ctx->num_sms * 16), 1), 256, 0, ctx->stream>>>(index, n, ga);
-    SR_LAUNCH_CHECK(ctx);
-    return SR_OK;
+    ga.c[0] = srd::GatherCol{src, nullptr, dst, nullptr, w, 0, 0};
+    return launch_gather(ctx, index, n, ga);
 }
 
 int32_t sr_abi_sizeof(int32_t which) {

@@ -198,8 +198,14 @@ static inline const sr_col_view* find_col(const sr_chunk_view* c, int32_t slot) 
     return nullptr;
 }
 
+// natural alignment of a column the kernels read in place: its value width, 8 bytes for 16-byte values
+static inline bool col_aligned(const void* p, int width) {
+    return ((uintptr_t)p & (uintptr_t)(std::min(width, 8) - 1)) == 0;
+}
+
 // A chunk made resident on the device: host chunks are staged (H2D on the ctx stream) into
-// buffers owned by `Staged`; device chunks are referenced in place.
+// buffers owned by `Staged`; device chunks (and pinned ones read in place) are referenced in place and must be
+// naturally aligned.
 struct Staged {
     std::vector<DevBuf> bufs; // 2 per column (data, nulls)
     std::vector<srd::DCol> cols;
@@ -238,9 +244,13 @@ struct Staged {
             d.type = c.type;
             d.width = w;
             if (in->mem == SR_MEM_DEVICE) {
+                if (!col_aligned(c.data, w))
+                    return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "slot %d: device column at %p is not %d-byte aligned", c.slot_id, c.data, std::min(w, 8));
                 d.data = c.data;
                 d.nulls = c.nulls;
             } else if (in->mem == SR_MEM_HOST_PINNED && in_place_pinned && in->num_rows > 0) {
+                if (!col_aligned(c.data, w))
+                    return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "slot %d: pinned column at %p is not %d-byte aligned", c.slot_id, c.data, std::min(w, 8));
                 const void* p = nullptr;
                 SR_TRY(mapped_alias(ctx, c.data, c.slot_id, &p));
                 d.data = p;

@@ -1014,10 +1014,7 @@ static int32_t join_probe_remain(sr_join* j, sr_chunk_out* out) {
         out->cols[k].slot_id = slot;
         ga.c[ga.n++] = g;
     }
-    if (total > 0 && ga.n > 0) {
-        srd::k_gather<<<dim3(std::min(grid_for(total, 256), ctx->num_sms * 16), ga.n), 256, 0, ctx->stream>>>(j->remain_index.as<uint32_t>(), total, ga);
-        SR_LAUNCH_CHECK(ctx);
-    }
+    if (total > 0 && ga.n > 0) SR_TRY(launch_gather(ctx, j->remain_index.as<uint32_t>(), total, ga));
     return SR_OK;
 }
 
@@ -1240,15 +1237,8 @@ static int32_t join_probe(sr_join* j, int32_t prober_id, const sr_chunk_view* pr
             ga_b.c[ga_b.n++] = g;
     }
     if (total > 0) {
-        const int gx = std::min(grid_for(total, 256), ctx->num_sms * 16);
-        if (ga_p.n > 0) {
-            srd::k_gather<<<dim3(gx, ga_p.n), 256, 0, ctx->stream>>>(ps.probe_index.as<uint32_t>(), total, ga_p);
-            SR_LAUNCH_CHECK(ctx);
-        }
-        if (ga_b.n > 0) {
-            srd::k_gather<<<dim3(gx, ga_b.n), 256, 0, ctx->stream>>>(ps.build_index.as<uint32_t>(), total, ga_b);
-            SR_LAUNCH_CHECK(ctx);
-        }
+        if (ga_p.n > 0) SR_TRY(launch_gather(ctx, ps.probe_index.as<uint32_t>(), total, ga_p));
+        if (ga_b.n > 0) SR_TRY(launch_gather(ctx, ps.build_index.as<uint32_t>(), total, ga_b));
     }
     return SR_OK;
 }

@@ -60,7 +60,11 @@ struct CompactCol {
     const void* src;
     void* dst;
     int32_t width;
-    int32_t pad;
+    int32_t vec16; // width 16 with src and dst 16-byte aligned: one int4 per value
+};
+// a 16-byte value that need only be 8-byte aligned: copied as two 8-byte words
+struct Words16 {
+    unsigned long long lo, hi;
 };
 struct CompactArgs {
     CompactCol c[2 * SR_MAX_OUT_COLS];
@@ -336,7 +340,10 @@ __global__ void __launch_bounds__(SCANW_BLOCK) k_scan_compact(const uint8_t* __r
                 compact_rows<uint64_t>(col.src, col.dst, base, m, out_pos);
                 break;
             default:
-                compact_rows<int4>(col.src, col.dst, base, m, out_pos);
+                if (col.vec16)
+                    compact_rows<int4>(col.src, col.dst, base, m, out_pos);
+                else
+                    compact_rows<Words16>(col.src, col.dst, base, m, out_pos);
                 break;
             }
         }
@@ -357,6 +364,7 @@ struct GatherCol {
     uint8_t* dst_nulls;
     int32_t width;
     int32_t zero_is_null; // build side of an outer join
+    int32_t vec16;        // width 16 with src and dst 16-byte aligned: one int4 per value (set by launch_gather)
 };
 struct GatherArgs {
     GatherCol c[SR_MAX_OUT_COLS];
@@ -380,8 +388,13 @@ __global__ void __launch_bounds__(256) k_gather(const uint32_t* __restrict__ ind
         case 8:
             copy_elem<uint64_t>(col.src, col.dst, s, i);
             break;
-        default:
-            copy_elem<int4>(col.src, col.dst, s, i);
+        default: // 16-byte values need only be 8-byte aligned
+            if (col.vec16) {
+                copy_elem<int4>(col.src, col.dst, s, i);
+            } else {
+                copy_elem<uint64_t>(col.src, col.dst, 2 * s, 2 * i);
+                copy_elem<uint64_t>(col.src, col.dst, 2 * s + 1, 2 * i + 1);
+            }
             break;
         }
         if (col.dst_nulls) {
@@ -418,6 +431,17 @@ static int32_t scan_counts(sr_ctx* ctx, ScanScratch* sc, const uint32_t* counts,
     srd::k_scan_counts<<<1, 1024, 0, ctx->stream>>>(sc->sums.as<uint32_t>(), nblk, sc->bases.as<uint64_t>(), ctx->dscratch);
     SR_LAUNCH_CHECK(ctx);
     srd::k_scan_add_base<<<(int)nblk, 1024, 0, ctx->stream>>>(sc->local.as<uint32_t>(), sc->bases.as<uint64_t>(), n, offsets);
+    SR_LAUNCH_CHECK(ctx);
+    return SR_OK;
+}
+
+// K11 over ga.n columns (n > 0, ga.n > 0): dst rows [0, n) from src rows index[0, n)
+static int32_t launch_gather(sr_ctx* ctx, const uint32_t* index, int64_t n, srd::GatherArgs& ga) {
+    for (int k = 0; k < ga.n; k++) {
+        srd::GatherCol& g = ga.c[k];
+        g.vec16 = g.width == 16 && (((uintptr_t)g.src | (uintptr_t)g.dst) & 15) == 0 ? 1 : 0;
+    }
+    srd::k_gather<<<dim3(std::min(grid_for(n, 256), ctx->num_sms * 16), ga.n), 256, 0, ctx->stream>>>(index, n, ga);
     SR_LAUNCH_CHECK(ctx);
     return SR_OK;
 }

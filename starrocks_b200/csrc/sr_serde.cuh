@@ -111,10 +111,17 @@ static int32_t serde_serialize(sr_ctx* ctx, const sr_chunk_view* c, int64_t r0, 
     return SR_OK;
 }
 
+// The payload must be exactly what serde_serialize writes for `meta`: a const column (ConstColumnSerde) is refused, and
+// so are a header num_rows other than meta->num_rows, a size other than meta->serialized_size and bytes left after the
+// last column.  The whole layout is checked before the first column is copied, so a refused payload queues no copy.
 static int32_t serde_deserialize(sr_serde* h, const void* src, int64_t bytes, int32_t src_mem, const sr_chunk_pb_meta* meta, sr_chunk_out* out) {
     sr_ctx* ctx = h->ctx;
     if (meta->num_cols < 0 || meta->num_cols > SR_MAX_OUT_COLS) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "%d columns", meta->num_cols);
+    for (int k = 0; k < meta->num_cols; k++)
+        if (meta->is_consts[k]) return sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "column %d is a const column: ConstColumnSerde payloads are not parsed", k);
     if (bytes < 8) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "payload of %lld bytes has no header", (long long)bytes);
+    if (bytes != meta->serialized_size)
+        return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "payload of %lld bytes, meta.serialized_size %lld", (long long)bytes, (long long)meta->serialized_size);
     // the header words and the per-column sizes steer the parse: read them on the host (device payload: the first pass
     // copies the whole payload's size words one by one -- at most 2 per column)
     const bool src_dev = src_mem == SR_MEM_DEVICE;
@@ -135,40 +142,52 @@ static int32_t serde_deserialize(sr_serde* h, const void* src, int64_t bytes, in
     SR_TRY(read32(0, &version));
     SR_TRY(read32(4, &rows));
     if (version != 1) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "ChunkPB.data version %u (expected 1)", version);
-    if (h->bufs.size() < 2 * (size_t)meta->num_cols) {
-        std::vector<DevBuf> nb(2 * (size_t)meta->num_cols);
-        for (size_t i = 0; i < h->bufs.size(); i++) std::swap(nb[i], h->bufs[i]);
-        h->bufs.swap(nb);
-    }
-    const cudaMemcpyKind kind = src_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+    if ((int64_t)rows != meta->num_rows)
+        return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "payload header says %u rows, meta.num_rows %lld", rows, (long long)meta->num_rows);
+    int64_t null_off[SR_MAX_OUT_COLS], data_off[SR_MAX_OUT_COLS], data_size[SR_MAX_OUT_COLS];
     int64_t off = 8;
-    out->num_cols = meta->num_cols;
-    out->mem = SR_MEM_DEVICE;
-    out->num_rows = rows;
     for (int k = 0; k < meta->num_cols; k++) {
         const int w = srd::type_width(meta->types[k]);
         if (w == 0) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "unknown column type %d", meta->types[k]);
-        out->cols[k].type = meta->types[k];
-        out->cols[k].slot_id = meta->slot_ids[k];
-        out->cols[k].nulls = nullptr;
         uint32_t sz = 0;
+        null_off[k] = -1;
         if (meta->is_nulls[k]) {
             SR_TRY(read32(off, &sz));
             off += 4;
             if (sz != rows || off + sz > bytes) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "column %d: null column of %u bytes for %u rows", k, sz, rows);
-            SR_TRY(h->bufs[2 * k + 1].reserve(ctx, (size_t)std::max<uint32_t>(sz, 1)));
-            if (sz) SR_CUDA(ctx, cudaMemcpyAsync(h->bufs[2 * k + 1].p, in + off, sz, kind, ctx->stream));
-            out->cols[k].nulls = (uint8_t*)h->bufs[2 * k + 1].p;
+            null_off[k] = off;
             off += sz;
         }
         SR_TRY(read32(off, &sz));
         off += 4;
         if ((int64_t)sz != (int64_t)rows * w || off + sz > bytes)
             return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "column %d: %u bytes for %u rows of width %d", k, sz, rows, w);
-        SR_TRY(h->bufs[2 * k].reserve(ctx, (size_t)std::max<uint32_t>(sz, 1)));
-        if (sz) SR_CUDA(ctx, cudaMemcpyAsync(h->bufs[2 * k].p, in + off, sz, kind, ctx->stream));
-        out->cols[k].data = h->bufs[2 * k].p;
+        data_off[k] = off;
+        data_size[k] = sz;
         off += sz;
+    }
+    if (off != bytes) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "%lld bytes after the last column", (long long)(bytes - off));
+    if (h->bufs.size() < 2 * (size_t)meta->num_cols) {
+        std::vector<DevBuf> nb(2 * (size_t)meta->num_cols);
+        for (size_t i = 0; i < h->bufs.size(); i++) std::swap(nb[i], h->bufs[i]);
+        h->bufs.swap(nb);
+    }
+    const cudaMemcpyKind kind = src_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+    out->num_cols = meta->num_cols;
+    out->mem = SR_MEM_DEVICE;
+    out->num_rows = rows;
+    for (int k = 0; k < meta->num_cols; k++) {
+        out->cols[k].type = meta->types[k];
+        out->cols[k].slot_id = meta->slot_ids[k];
+        out->cols[k].nulls = nullptr;
+        if (null_off[k] >= 0) {
+            SR_TRY(h->bufs[2 * k + 1].reserve(ctx, (size_t)std::max<uint32_t>(rows, 1)));
+            if (rows) SR_CUDA(ctx, cudaMemcpyAsync(h->bufs[2 * k + 1].p, in + null_off[k], rows, kind, ctx->stream));
+            out->cols[k].nulls = (uint8_t*)h->bufs[2 * k + 1].p;
+        }
+        SR_TRY(h->bufs[2 * k].reserve(ctx, (size_t)std::max<int64_t>(data_size[k], 1)));
+        if (data_size[k]) SR_CUDA(ctx, cudaMemcpyAsync(h->bufs[2 * k].p, in + data_off[k], (size_t)data_size[k], kind, ctx->stream));
+        out->cols[k].data = h->bufs[2 * k].p;
     }
     if (!src_dev) SR_CUDA(ctx, cudaStreamSynchronize(ctx->stream)); // the caller's host buffer may go away
     return SR_OK;
