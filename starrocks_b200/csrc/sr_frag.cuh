@@ -26,6 +26,10 @@
 //    the table is small, flushed once per CTA;
 //  * join order: pass rates measured on a sample of the first batch (adaptive), most selective
 //    first, smaller table first on a tie -- inner joins commute, the result is order independent.
+//
+// Host side: frag_plan chooses the mode on the first batch and plans it (frag_plan_passes: the selection-vector passes
+// of sr_frag_pass.cuh, frag_plan_cascade: k_fragment); frag_push runs it on every batch, the final pass of the
+// selection-vector passes through frag_launch_final.
 #pragma once
 
 #include "sr_agg.cuh"
@@ -50,15 +54,16 @@ struct sr_fragment {
     srd::FragDev host;
     DevBuf dev, counters;
     Staged staged;
-    size_t smem_bytes = 0;
-    int32_t queue_word_off = 0;
     bool smem_agg = false;
-    int grid = 0;
     int order[SR_MAX_FRAG_JOINS];
     double pass_rate[SR_MAX_FRAG_JOINS];
     double pred_rate = 1.0;
-    // selective mode (sr_frag_pass.cuh): streaming pass -> gather passes -> final pass
     int force_mode = 0; // 0 = choose from the sampled pass rates, 1 = fused cascade kernel, 2 = selection-vector passes
+    // cascade mode (k_fragment), planned by frag_plan_cascade
+    size_t cascade_smem = 0;
+    int32_t queue_word_off = 0;
+    int cascade_grid = 0;
+    // selective mode (sr_frag_pass.cuh): streaming pass -> gather passes -> final pass, planned by frag_plan_passes
     bool selective = false;
     bool expand = false; // some INNER join has duplicate build keys: selection-vector passes + k_frag_gather_agg_expand
     srd::PassDev pass;
@@ -67,6 +72,7 @@ struct sr_fragment {
     double est_rate = 1.0; // sampled fraction of the fact rows that reaches the aggregate
     size_t stream_smem = 0;
     int stream_grid = 0;
+    int gather_grid = 0; // k_frag_gather_join
     int final_grid = 0;
     // the batched final pass (k_frag_final_dense): planned when the shape allows it, used by a push whose fact columns
     // are all plain int32 and whose aggregate still accumulates in shared memory
@@ -88,30 +94,32 @@ struct FragTypeCtx {
     sr_fragment* f;
 };
 
+// the first join (hint order) that carries `slot` as a payload, and its build column; join = -1 when none does
+struct FragPayload {
+    const BuildCol* col;
+    int join;
+};
+static FragPayload frag_find_payload(const sr_fragment* f, int32_t slot) {
+    for (int j = 0; j < f->num_joins; j++)
+        for (int p = 0; p < f->joins[j].num_payload; p++)
+            if (f->joins[j].payload_build_slots[p] == slot) return FragPayload{f->joins[j].join->find_col(slot), j};
+    return FragPayload{nullptr, -1};
+}
+
 // slot type: fact chunk first, then payload columns of the joins
 static int32_t frag_slot_type(void* user, int32_t slot) {
     sr_fragment* f = ((FragTypeCtx*)user)->f;
     const int k = f->staged.find(slot);
     if (k >= 0) return f->staged.cols[k].type;
-    for (int j = 0; j < f->num_joins; j++)
-        for (int p = 0; p < f->joins[j].num_payload; p++)
-            if (f->joins[j].payload_build_slots[p] == slot) {
-                const BuildCol* bc = f->joins[j].join->find_col(slot);
-                return bc ? bc->type : 0;
-            }
-    return 0;
+    const BuildCol* bc = frag_find_payload(f, slot).col;
+    return bc ? bc->type : 0;
 }
 static bool frag_slot_nullable(void* user, int32_t slot) {
     sr_fragment* f = ((FragTypeCtx*)user)->f;
     const int k = f->staged.find(slot);
     if (k >= 0) return f->staged.cols[k].nulls != nullptr;
-    for (int j = 0; j < f->num_joins; j++)
-        for (int p = 0; p < f->joins[j].num_payload; p++)
-            if (f->joins[j].payload_build_slots[p] == slot) {
-                const BuildCol* bc = f->joins[j].join->find_col(slot);
-                return bc && bc->nullable;
-            }
-    return false;
+    const BuildCol* bc = frag_find_payload(f, slot).col;
+    return bc && bc->nullable;
 }
 
 static int32_t frag_bind_vtab(sr_fragment* f, VTab* vt) {
@@ -201,16 +209,11 @@ static int32_t frag_compile(sr_fragment* f) {
     f->value_col.assign(f->reg.slots.size(), nullptr);
     for (size_t k = 0; k < f->reg.slots.size(); k++) {
         if (f->staged.find(f->reg.slots[k]) >= 0) continue;
-        bool found = false;
-        for (int j = 0; j < f->num_joins && !found; j++)
-            for (int p = 0; p < f->joins[j].num_payload && !found; p++)
-                if (f->joins[j].payload_build_slots[p] == f->reg.slots[k]) {
-                    f->value_src[k] = j;
-                    f->value_col[k] = f->joins[j].join->find_col(f->reg.slots[k]);
-                    h.joins[j].need_head = 1;
-                    found = true;
-                }
-        if (!found) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "slot %d is neither a fact column nor a join payload", f->reg.slots[k]);
+        const FragPayload pl = frag_find_payload(f, f->reg.slots[k]);
+        if (pl.join < 0) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "slot %d is neither a fact column nor a join payload", f->reg.slots[k]);
+        f->value_src[k] = pl.join;
+        f->value_col[k] = pl.col;
+        h.joins[pl.join].need_head = 1;
     }
     SR_TRY(f->counters.reserve(ctx, 256));
     SR_CUDA(ctx, cudaMemsetAsync(f->counters.p, 0, 256, ctx->stream));
@@ -336,17 +339,229 @@ static int32_t frag_plan_final_dense(sr_fragment* f) {
     return SR_OK;
 }
 
-// sample pass rates, order the joins, assign shared-memory bitmaps, upload, pick the grid
+// ---- selection-vector mode (sr_frag_pass.cuh) ----
+
+// which joins the streaming pass, the gather passes and the final pass test, and the streamed join that carries its key
+static void frag_plan_stream_joins(sr_fragment* f) {
+    const srd::FragDev& h = f->host;
+    const int* ord = f->order;
+    // joins whose key column is streamed: the first one, and the second when >= 8 % of the rows reach it
+    int ns = f->num_joins > 0 ? 1 : 0;
+    if (f->num_joins > 1 && f->pred_rate * f->pass_rate[ord[0]] >= 0.08) ns = 2;
+    // trailing joins that filter (almost) nothing are tested inline by the final pass
+    int ff = f->num_joins;
+    while (ff > ns && f->pass_rate[ord[ff - 1]] >= 0.9) ff--;
+    f->pass.num_stream_joins = ns;
+    f->pass.final_first_join = ff;
+    f->gather_joins.clear();
+    for (int q = ns; q < ff; q++) f->gather_joins.push_back(q);
+    // a streamed join whose build row the final pass looks up (payload) hands its int32 key over through the
+    // selection vector: one random fact-sector read less per surviving row
+    f->pass.carry_join = -1;
+    f->pass.carry_value_id = -1;
+    for (int q = 0; q < ns; q++) {
+        const int id = h.joins[q].key_value_id;
+        const int32_t kt = f->reg.types[id];
+        if (h.joins[q].need_head && srd::type_width(kt) == 4 && !srd::is_float_class(kt) && id < 127) {
+            f->pass.carry_join = (int8_t)q;
+            f->pass.carry_value_id = (int8_t)id;
+            break;
+        }
+    }
+}
+
+// streaming pass shared memory: bitmaps of the streamed joins only (less the carried-key stash of
+// k_frag_stream_tests<true>, so that two CTAs still fit on an SM)
+static void frag_plan_stream_smem(sr_fragment* f) {
+    srd::FragDev& h = f->host;
+    size_t sw = 0;
+    const size_t sbudget = (100 * 1024 - (f->pass.carry_join >= 0 ? sizeof(int4) * srd::STREAM_GROUPS * srd::STREAM_BLOCK : 0)) / 4;
+    for (int q = 0; q < f->num_joins; q++) {
+        srd::FragJoinDev& fj = h.joins[q];
+        fj.smem_off = -1;
+        if (q < f->pass.num_stream_joins && fj.use_bitmap && sw + (size_t)fj.bitmap_words + 1 <= sbudget) {
+            fj.smem_off = (int32_t)sw;
+            sw += ((size_t)fj.bitmap_words + 1 + 3) & ~(size_t)3; // + one zero guard word (stream_test_reg kind 1)
+        }
+    }
+    f->stream_smem = sw * 4;
+}
+
+// the streaming pass in "tests" form (k_frag_stream_tests): every scan conjunct must reduce to an int32 range
+// and every streamed column must be int32-class; otherwise the generic streaming kernel runs.  reach_pred0: the
+// sampled fraction of the rows that pass scan conjunct 0.
+static void frag_plan_stream_tests(sr_fragment* f, double reach_pred0) {
+    const srd::FragDev& h = f->host;
+    const int ns = f->pass.num_stream_joins;
+    bool ok = h.num_exprs == 0 && h.num_preds + ns > 0 && h.num_preds + ns <= SR_MAX_STREAM_TESTS;
+    int nt = 0;
+    auto int32_class = [&](int id) { return srd::type_width(f->reg.types[id]) == 4 && !srd::is_float_class(f->reg.types[id]); };
+    for (int p = 0; p < h.num_preds && ok; p++) {
+        const srd::CPred& cp = h.preds[p];
+        long long lo, hi;
+        ok = pred_int32_range(cp, &lo, &hi) && int32_class(cp.value_id);
+        if (!ok) break;
+        srd::StreamTest& st = f->pass.tests[nt++];
+        st.kind = 0;
+        st.value_id = cp.value_id;
+        st.join = -1;
+        st.lo = (uint32_t)(int32_t)lo;
+        st.span = (uint32_t)(hi - lo);
+    }
+    for (int q = 0; q < ns && ok; q++) {
+        if (!int32_class(h.joins[q].key_value_id)) {
+            ok = false;
+            break;
+        }
+        srd::StreamTest& st = f->pass.tests[nt++];
+        st.kind = 1;
+        st.value_id = h.joins[q].key_value_id;
+        st.join = q;
+        st.lo = st.span = 0;
+    }
+    f->pass.num_tests = ok ? nt : 0;
+    // the second test's column is streamed with vector loads as well when >= 8 % of the rows reach it
+    // (most of its 64-byte DRAM bursts would be touched anyway, and the loads do not wait for test 0).  HBM does
+    // move 64 bytes per access: on H100, reading every other 32-byte sector of a column costs 1.03x reading all of
+    // it (scripts/hbm_sector_probe.cu), so fetching this column by the sector for the rows test 0 passed saves nothing
+    double reach1 = 1.0;
+    if (ok && nt > 1) reach1 = f->pass.tests[0].kind == 0 ? reach_pred0 : f->pred_rate * f->pass_rate[f->order[0]];
+    f->pass.num_vec = (ok && nt > 1 && reach1 >= 0.08) ? 2 : 1;
+    // the vector-column tests in the form k_frag_stream_tests runs them, with the bitmaps where frag_plan_stream_smem put them
+    for (int v = 0; v < 2 && f->pass.num_tests > 0; v++) {
+        const srd::StreamTest& st = f->pass.tests[v < f->pass.num_vec ? v : 0];
+        srd::VecTest& t = f->pass.vec[v];
+        t.kind = st.kind == 0 ? 0 : 3;
+        t.lo = st.lo;
+        t.span = st.span;
+        t.smem_off = -1;
+        t.bm = nullptr;
+        if (st.kind == 1) {
+            const srd::FragJoinDev& fj = h.joins[st.join];
+            if (fj.use_bitmap && fj.idx32) {
+                t.lo = (uint32_t)(int32_t)fj.j.min_value;
+                t.span = (uint32_t)(fj.j.max_value - fj.j.min_value);
+                if (fj.smem_off >= 0 && t.span != 0xFFFFFFFFu) {
+                    t.kind = 1;
+                    t.smem_off = fj.smem_off;
+                } else {
+                    t.kind = 2;
+                    t.bm = fj.j.bitmap;
+                }
+            }
+        }
+    }
+}
+
+// fact values the final pass reads: keys of the joins it looks up or tests, group keys, aggregate inputs
+static void frag_plan_final_vals(sr_fragment* f) {
+    const srd::FragDev& h = f->host;
+    std::vector<int> need;
+    auto want = [&](int id) {
+        if (id >= 0 && id < (int)f->value_src.size() && f->value_src[id] < 0 && std::find(need.begin(), need.end(), id) == need.end()) need.push_back(id);
+    };
+    for (int q = 0; q < f->num_joins; q++)
+        if (h.joins[q].need_head || q >= f->pass.final_first_join) want(h.joins[q].key_value_id);
+    const srd::AggDev& ah = f->agg->host;
+    for (int k = 0; k < ah.num_keys; k++) want(ah.key_value_id[k]);
+    for (int q = 0; q < ah.num_fns; q++)
+        for (int k = 0; k < ah.fns[q].input.num_nodes; k++)
+            if (ah.fns[q].input.nodes[k].op == srd::C_LOAD_I || ah.fns[q].input.nodes[k].op == srd::C_LOAD_D) want(ah.fns[q].input.nodes[k].arg);
+    for (int k = 0; k < SR_FINAL_PREFETCH; k++) f->pass.final_vals[k] = k < (int)need.size() ? (int8_t)need[k] : (int8_t)-1;
+    f->pass.num_final_vals = (int8_t)std::min<size_t>(need.size(), 127);
+}
+
+// launch grids of the passes (and the dynamic shared-memory limit of the streaming kernels)
+static int32_t frag_plan_pass_grids(sr_fragment* f) {
+    sr_ctx* ctx = f->ctx;
+    const int stream_smem_limit = (int)std::max<size_t>(f->stream_smem, 16);
+    SR_CUDA(ctx, cudaFuncSetAttribute(srd::k_frag_stream<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, stream_smem_limit));
+    SR_CUDA(ctx, cudaFuncSetAttribute(srd::k_frag_stream<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, stream_smem_limit));
+    SR_CUDA(ctx, cudaFuncSetAttribute(srd::k_frag_stream_tests<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, stream_smem_limit));
+    SR_CUDA(ctx, cudaFuncSetAttribute(srd::k_frag_stream_tests<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, stream_smem_limit));
+    int per_sm = 0;
+    SR_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, srd::k_frag_stream<false>, srd::STREAM_BLOCK, f->stream_smem));
+    if (per_sm < 1) return sr_fail(ctx, SR_ERR_CUDA, "streaming pass does not fit on an SM (smem %zu)", f->stream_smem);
+    f->stream_grid = per_sm * ctx->num_sms;
+    // gather passes: exactly one wave of resident CTAs (grid-stride loops; a partial second wave only adds a tail)
+    int gj = 0, ga = 0;
+    SR_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&gj, srd::k_frag_gather_join, srd::GATHER_BLOCK, 0));
+    if (f->expand)
+        SR_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ga, srd::k_frag_gather_agg_expand, srd::GATHER_BLOCK, 0));
+    else if (f->agg->host.num_keys == 0)
+        SR_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ga, srd::k_frag_gather_agg<false, true>, srd::GATHER_BLOCK, 0));
+    else if (f->smem_agg)
+        SR_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ga, srd::k_frag_gather_agg<true>, srd::GATHER_BLOCK, f->agg->smem_bytes));
+    else
+        SR_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ga, srd::k_frag_gather_agg<false>, srd::GATHER_BLOCK, 0));
+    f->gather_grid = std::max(gj, 1) * ctx->num_sms;
+    f->final_grid = std::max(ga, 1) * ctx->num_sms;
+    return SR_OK;
+}
+
+// slots of pass_counters (64-bit words): the entry count of every selection vector a push writes (the streaming pass's,
+// then one per gather pass), and the two fail counters of the final pass's hash-table retries (live and spare)
+constexpr int PASS_CNT_SEL = 0;
+constexpr int PASS_CNT_FAIL = 8;
+constexpr int PASS_CNT_WORDS = 16;
+static_assert(PASS_CNT_SEL + SR_MAX_FRAG_JOINS <= PASS_CNT_FAIL && PASS_CNT_FAIL + 2 <= PASS_CNT_WORDS, "pass counter layout");
+
+// selection-vector mode; reach_pred0: the sampled fraction of the rows that pass scan conjunct 0
+static int32_t frag_plan_passes(sr_fragment* f, double reach_pred0) {
+    memset(&f->pass, 0, sizeof(f->pass));
+    frag_plan_stream_joins(f);
+    frag_plan_stream_smem(f);
+    frag_plan_stream_tests(f, reach_pred0);
+    frag_plan_final_vals(f);
+    SR_TRY(frag_plan_pass_grids(f));
+    SR_TRY(frag_plan_final_dense(f));
+    return f->pass_counters.reserve(f->ctx, PASS_CNT_WORDS * sizeof(uint64_t));
+}
+
+// ---- cascade mode (k_fragment) ----
+static int32_t frag_plan_cascade(sr_fragment* f) {
+    sr_ctx* ctx = f->ctx;
+    srd::FragDev& h = f->host;
+    // dynamic shared memory: [aggregate accumulators | bitmaps | per-warp queues]
+    size_t words = 0;
+    if (f->smem_agg) words += (f->agg->smem_bytes + 15) / 16 * 4;
+    const size_t budget_words = (96 * 1024) / 4; // keeps 2 CTAs of 512 threads resident per SM
+    const size_t queue_words = (size_t)srd::FRAG_WARPS * srd::FRAG_WARP_QWORDS;
+    for (int q = 0; q < f->num_joins; q++) {
+        srd::FragJoinDev& fj = h.joins[q];
+        fj.smem_off = -1;
+        if (fj.use_bitmap && words + (size_t)fj.bitmap_words + queue_words <= budget_words) {
+            fj.smem_off = (int32_t)words;
+            words += (size_t)fj.bitmap_words;
+            words = (words + 3) & ~(size_t)3;
+        }
+    }
+    f->queue_word_off = (int32_t)words;
+    words += queue_words;
+    f->cascade_smem = words * 4;
+    // occupancy-sized persistent grid
+    int per_sm = 0;
+    SR_CUDA(ctx, cudaFuncSetAttribute(srd::k_fragment<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)f->cascade_smem));
+    SR_CUDA(ctx, cudaFuncSetAttribute(srd::k_fragment<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)f->cascade_smem));
+    if (f->smem_agg)
+        SR_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, srd::k_fragment<true>, srd::FRAG_BLOCK, f->cascade_smem));
+    else
+        SR_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, srd::k_fragment<false>, srd::FRAG_BLOCK, f->cascade_smem));
+    if (per_sm < 1) return sr_fail(ctx, SR_ERR_CUDA, "fragment kernel does not fit on an SM (smem %zu)", f->cascade_smem);
+    f->cascade_grid = per_sm * ctx->num_sms;
+    return SR_OK;
+}
+
+// sample pass rates, order the joins, choose the mode and plan it, upload
 static int32_t frag_plan(sr_fragment* f, const VTab& vt, int64_t n) {
     sr_ctx* ctx = f->ctx;
     srd::FragDev& h = f->host;
     SR_TRY(f->dev.reserve(ctx, sizeof(srd::FragDev)));
     SR_CUDA(ctx, cudaMemcpyAsync(f->dev.p, &h, sizeof(h), cudaMemcpyHostToDevice, ctx->stream));
     const int64_t sample = std::min<int64_t>(n, 1 << 16);
-    unsigned long long counts[24] = {0}; // [0, 6): joins, [6]: all conjuncts, [16 + p]: conjuncts 0..p
-    static_assert(SR_MAX_FRAG_JOINS + 1 <= 16, "sample counter layout");
-    counts[SR_MAX_FRAG_JOINS] = (unsigned long long)sample;
-    for (int p = 0; p < 8; p++) counts[16 + p] = (unsigned long long)sample;
+    unsigned long long counts[srd::SAMPLE_COUNTERS] = {0};
+    counts[srd::SAMPLE_ALL_PREDS] = (unsigned long long)sample;
+    for (int p = srd::SAMPLE_PREDS_UPTO; p < srd::SAMPLE_COUNTERS; p++) counts[p] = (unsigned long long)sample;
     if (sample > 0 && (f->num_joins > 0 || h.num_preds > 0 || h.num_exprs > 0)) {
         unsigned long long* dcounts = f->counters.as<unsigned long long>() + 8;
         SR_CUDA(ctx, cudaMemsetAsync(dcounts, 0, sizeof(counts), ctx->stream));
@@ -356,7 +571,7 @@ static int32_t frag_plan(sr_fragment* f, const VTab& vt, int64_t n) {
         SR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     }
     for (int j = 0; j < f->num_joins; j++) f->pass_rate[j] = sample > 0 ? (double)counts[j] / (double)sample : 1.0;
-    f->pred_rate = sample > 0 ? (double)counts[SR_MAX_FRAG_JOINS] / (double)sample : 1.0;
+    f->pred_rate = sample > 0 ? (double)counts[srd::SAMPLE_ALL_PREDS] / (double)sample : 1.0;
     std::vector<int> ord(f->num_joins);
     for (int j = 0; j < f->num_joins; j++) ord[j] = j;
     // most selective first; pass rates within 15 % of each other count as a tie -> smaller table first
@@ -384,183 +599,53 @@ static int32_t frag_plan(sr_fragment* f, const VTab& vt, int64_t n) {
     for (int q = 0; q < f->num_joins; q++) total_rate *= f->pass_rate[ord[q]];
     f->est_rate = total_rate;
     f->selective = f->expand || f->force_mode == 2 || (f->force_mode == 0 && total_rate < 0.25 && n >= (1 << 16));
-    if (f->selective) {
-        // joins whose key column is streamed: the first one, and the second when >= 8 % of the rows reach it
-        int ns = f->num_joins > 0 ? 1 : 0;
-        if (f->num_joins > 1 && f->pred_rate * f->pass_rate[ord[0]] >= 0.08) ns = 2;
-        // trailing joins that filter (almost) nothing are tested inline by the final pass
-        int ff = f->num_joins;
-        while (ff > ns && f->pass_rate[ord[ff - 1]] >= 0.9) ff--;
-        memset(&f->pass, 0, sizeof(f->pass));
-        f->pass.num_stream_joins = ns;
-        f->pass.final_first_join = ff;
-        // a streamed join whose build row the final pass looks up (payload) hands its int32 key over through the
-        // selection vector: one random fact-sector read less per surviving row
-        f->pass.carry_join = -1;
-        f->pass.carry_value_id = -1;
-        for (int q = 0; q < ns; q++) {
-            const int id = h.joins[q].key_value_id;
-            const int32_t kt = f->reg.types[id];
-            if (h.joins[q].need_head && srd::type_width(kt) == 4 && !srd::is_float_class(kt) && id < 127) {
-                f->pass.carry_join = (int8_t)q;
-                f->pass.carry_value_id = (int8_t)id;
-                break;
-            }
-        }
-        // the streaming pass in "tests" form (k_frag_stream_tests): every scan conjunct must reduce to an int32 range
-        // and every streamed column must be int32-class; otherwise the generic streaming kernel runs
-        {
-            bool ok = h.num_exprs == 0 && h.num_preds + ns > 0 && h.num_preds + ns <= SR_MAX_STREAM_TESTS;
-            int nt = 0;
-            auto int32_class = [&](int id) { return srd::type_width(f->reg.types[id]) == 4 && !srd::is_float_class(f->reg.types[id]); };
-            for (int p = 0; p < h.num_preds && ok; p++) {
-                const srd::CPred& cp = h.preds[p];
-                long long lo, hi;
-                ok = pred_int32_range(cp, &lo, &hi) && int32_class(cp.value_id);
-                if (!ok) break;
-                srd::StreamTest& st = f->pass.tests[nt++];
-                st.kind = 0;
-                st.value_id = cp.value_id;
-                st.join = -1;
-                st.lo = (uint32_t)(int32_t)lo;
-                st.span = (uint32_t)(hi - lo);
-            }
-            for (int q = 0; q < ns && ok; q++) {
-                if (!int32_class(h.joins[q].key_value_id)) {
-                    ok = false;
-                    break;
-                }
-                srd::StreamTest& st = f->pass.tests[nt++];
-                st.kind = 1;
-                st.value_id = h.joins[q].key_value_id;
-                st.join = q;
-                st.lo = st.span = 0;
-            }
-            f->pass.num_tests = ok ? nt : 0;
-            // the second test's column is streamed with vector loads as well when >= 8 % of the rows reach it
-            // (most of its 64-byte DRAM bursts would be touched anyway, and the loads do not wait for test 0).  HBM does
-            // move 64 bytes per access: on H100, reading every other 32-byte sector of a column costs 1.03x reading all of
-            // it (scripts/hbm_sector_probe.cu), so fetching this column by the sector for the rows test 0 passed saves nothing
-            double reach1 = 1.0;
-            if (ok && nt > 1) reach1 = f->pass.tests[0].kind == 0 ? (double)counts[16] / (double)std::max<int64_t>(sample, 1) : f->pred_rate * f->pass_rate[ord[0]];
-            f->pass.num_vec = (ok && nt > 1 && reach1 >= 0.08) ? 2 : 1;
-        }
-        // fact values the final pass reads: keys of the joins it looks up or tests, group keys, aggregate inputs
-        {
-            std::vector<int> need;
-            auto want = [&](int id) {
-                if (id >= 0 && id < (int)f->value_src.size() && f->value_src[id] < 0 && std::find(need.begin(), need.end(), id) == need.end()) need.push_back(id);
-            };
-            for (int q = 0; q < f->num_joins; q++)
-                if (h.joins[q].need_head || q >= ff) want(h.joins[q].key_value_id);
-            const srd::AggDev& ah = f->agg->host;
-            for (int k = 0; k < ah.num_keys; k++) want(ah.key_value_id[k]);
-            for (int q = 0; q < ah.num_fns; q++)
-                for (int k = 0; k < ah.fns[q].input.num_nodes; k++)
-                    if (ah.fns[q].input.nodes[k].op == srd::C_LOAD_I || ah.fns[q].input.nodes[k].op == srd::C_LOAD_D) want(ah.fns[q].input.nodes[k].arg);
-            for (int k = 0; k < SR_FINAL_PREFETCH; k++) f->pass.final_vals[k] = k < (int)need.size() ? (int8_t)need[k] : (int8_t)-1;
-            f->pass.num_final_vals = (int8_t)std::min<size_t>(need.size(), 127);
-        }
-        f->gather_joins.clear();
-        for (int q = ns; q < ff; q++) f->gather_joins.push_back(q);
-        // streaming pass shared memory: bitmaps of the streamed joins only (less the carried-key stash of
-        // k_frag_stream_tests<true>, so that two CTAs still fit on an SM)
-        size_t sw = 0;
-        const size_t sbudget = (100 * 1024 - (f->pass.carry_join >= 0 ? sizeof(int4) * srd::STREAM_GROUPS * srd::STREAM_BLOCK : 0)) / 4;
-        for (int q = 0; q < f->num_joins; q++) {
-            srd::FragJoinDev& fj = h.joins[q];
-            fj.smem_off = -1;
-            if (q < ns && fj.use_bitmap && sw + (size_t)fj.bitmap_words + 1 <= sbudget) {
-                fj.smem_off = (int32_t)sw;
-                sw += ((size_t)fj.bitmap_words + 1 + 3) & ~(size_t)3; // + one zero guard word (stream_test_reg kind 1)
-            }
-        }
-        f->stream_smem = sw * 4;
-        for (int v = 0; v < 2 && f->pass.num_tests > 0; v++) {
-            const srd::StreamTest& st = f->pass.tests[v < f->pass.num_vec ? v : 0];
-            srd::VecTest& t = f->pass.vec[v];
-            t.kind = st.kind == 0 ? 0 : 3;
-            t.lo = st.lo;
-            t.span = st.span;
-            t.smem_off = -1;
-            t.bm = nullptr;
-            if (st.kind == 1) {
-                const srd::FragJoinDev& fj = h.joins[st.join];
-                if (fj.use_bitmap && fj.idx32) {
-                    t.lo = (uint32_t)(int32_t)fj.j.min_value;
-                    t.span = (uint32_t)(fj.j.max_value - fj.j.min_value);
-                    if (fj.smem_off >= 0 && t.span != 0xFFFFFFFFu) {
-                        t.kind = 1;
-                        t.smem_off = fj.smem_off;
-                    } else {
-                        t.kind = 2;
-                        t.bm = fj.j.bitmap;
-                    }
-                }
-            }
-        }
-        f->smem_agg = f->agg->smem_bytes > 0;
-        f->smem_bytes = f->agg->smem_bytes;
-        f->queue_word_off = 0;
-        SR_CUDA(ctx, cudaMemcpyAsync(f->dev.p, &h, sizeof(h), cudaMemcpyHostToDevice, ctx->stream));
-        SR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        int per_sm = 0;
-        SR_CUDA(ctx, cudaFuncSetAttribute(srd::k_frag_stream<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(f->stream_smem, 16)));
-        SR_CUDA(ctx, cudaFuncSetAttribute(srd::k_frag_stream<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(f->stream_smem, 16)));
-        SR_CUDA(ctx, cudaFuncSetAttribute(srd::k_frag_stream_tests<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(f->stream_smem, 16)));
-        SR_CUDA(ctx, cudaFuncSetAttribute(srd::k_frag_stream_tests<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(f->stream_smem, 16)));
-        SR_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, srd::k_frag_stream<false>, srd::STREAM_BLOCK, f->stream_smem));
-        if (per_sm < 1) return sr_fail(ctx, SR_ERR_CUDA, "streaming pass does not fit on an SM (smem %zu)", f->stream_smem);
-        f->stream_grid = per_sm * ctx->num_sms;
-        // gather passes: exactly one wave of resident CTAs (grid-stride loops; a partial second wave only adds a tail)
-        int gj = 0, ga = 0;
-        SR_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&gj, srd::k_frag_gather_join, srd::GATHER_BLOCK, 0));
-        if (f->expand)
-            SR_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ga, srd::k_frag_gather_agg_expand, srd::GATHER_BLOCK, 0));
-        else if (f->agg->host.num_keys == 0)
-            SR_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ga, srd::k_frag_gather_agg<false, true>, srd::GATHER_BLOCK, 0));
-        else if (f->smem_agg)
-            SR_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ga, srd::k_frag_gather_agg<true>, srd::GATHER_BLOCK, f->agg->smem_bytes));
-        else
-            SR_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ga, srd::k_frag_gather_agg<false>, srd::GATHER_BLOCK, 0));
-        f->grid = std::max(gj, 1) * ctx->num_sms;
-        f->final_grid = std::max(ga, 1) * ctx->num_sms;
-        SR_TRY(frag_plan_final_dense(f));
-        SR_TRY(f->pass_counters.reserve(ctx, 16 * sizeof(uint64_t)));
-        f->compiled = true;
-        return SR_OK;
-    }
-    // dynamic shared memory: [aggregate accumulators | bitmaps | per-warp queues]
-    size_t words = 0;
     f->smem_agg = f->agg->smem_bytes > 0;
-    if (f->smem_agg) words += (f->agg->smem_bytes + 15) / 16 * 4;
-    const size_t budget_words = (96 * 1024) / 4; // keeps 2 CTAs of 512 threads resident per SM
-    const size_t queue_words = (size_t)srd::FRAG_WARPS * srd::FRAG_WARP_QWORDS;
-    for (int q = 0; q < f->num_joins; q++) {
-        srd::FragJoinDev& fj = h.joins[q];
-        fj.smem_off = -1;
-        if (fj.use_bitmap && words + (size_t)fj.bitmap_words + queue_words <= budget_words) {
-            fj.smem_off = (int32_t)words;
-            words += (size_t)fj.bitmap_words;
-            words = (words + 3) & ~(size_t)3;
-        }
-    }
-    f->queue_word_off = (int32_t)words;
-    words += queue_words;
-    f->smem_bytes = words * 4;
+    if (f->selective)
+        SR_TRY(frag_plan_passes(f, (double)counts[srd::SAMPLE_PREDS_UPTO] / (double)std::max<int64_t>(sample, 1)));
+    else
+        SR_TRY(frag_plan_cascade(f));
+    // the kernels read the shared-memory offsets of the bitmaps the mode's plan assigned
     SR_CUDA(ctx, cudaMemcpyAsync(f->dev.p, &h, sizeof(h), cudaMemcpyHostToDevice, ctx->stream));
     SR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    // occupancy-sized persistent grid
-    int per_sm = 0;
-    SR_CUDA(ctx, cudaFuncSetAttribute(srd::k_fragment<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)f->smem_bytes));
-    SR_CUDA(ctx, cudaFuncSetAttribute(srd::k_fragment<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)f->smem_bytes));
-    if (f->smem_agg)
-        SR_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, srd::k_fragment<true>, srd::FRAG_BLOCK, f->smem_bytes));
-    else
-        SR_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, srd::k_fragment<false>, srd::FRAG_BLOCK, f->smem_bytes));
-    if (per_sm < 1) return sr_fail(ctx, SR_ERR_CUDA, "fragment kernel does not fit on an SM (smem %zu)", f->smem_bytes);
-    f->grid = per_sm * ctx->num_sms;
     f->compiled = true;
+    return SR_OK;
+}
+
+// The final pass of selective mode over the selection vector `in` (its entry count at `in_count`).  A hash aggregate is
+// neither dense nor kept in shared memory and has group keys, so it always runs k_frag_gather_agg_expand or
+// k_frag_gather_agg<false>: the two that append the rows its table refuses to `fail_list` (counted at `fail_count`).
+static int32_t frag_launch_final(sr_fragment* f, const VTab& vt, const srd::SelEntry* in, const unsigned long long* in_count, srd::SelEntry* fail_list,
+                                 unsigned long long* fail_count) {
+    sr_ctx* ctx = f->ctx;
+    sr_agg* a = f->agg;
+    const srd::AggDev& ah = a->host;
+    const srd::FragDev* fdev = (const srd::FragDev*)f->dev.p;
+    const srd::AggDev* adev = (const srd::AggDev*)a->dev.p;
+    const srd::PassDev& pass = f->pass;
+    // the batched final pass needs plain int32 fact columns and the shared-memory accumulators it was planned for
+    // (a push whose aggregate input turned nullable switches the aggregate to global accumulation)
+    const bool dense_final = f->final_dense_ok && vt.plain32 && f->smem_agg && a->smem_bytes > 0;
+    f->final_pass = dense_final ? SR_FINAL_PASS_DENSE : f->expand ? SR_FINAL_PASS_EXPAND : SR_FINAL_PASS_GENERIC;
+    if (dense_final) {
+        srd::FinalDense fp = f->final_dense;
+        for (int c = 0; c < fp.num_vals; c++) {
+            fp.cols[c] = (const int32_t*)vt.v[pass.final_vals[c]].data;
+            if (pass.carry_join >= 0 && pass.final_vals[c] == pass.carry_value_id) fp.carry_val = c;
+        }
+        for (int q = 0; q < fp.num_fns; q++) fp.fn[q].gacc = ah.fns[f->final_fn_src[q]].acc0;
+        fp.gcnt = ah.cnt_star;
+        fp.flags = ah.flags;
+        fp.rows_passed = f->host.rows_passed;
+        srd::k_frag_final_dense<srd::FINAL_ROWS><<<f->final_dense_grid, srd::GATHER_BLOCK, a->smem_bytes, ctx->stream>>>(fp, in, in_count);
+    } else if (f->expand)
+        srd::k_frag_gather_agg_expand<<<f->final_grid, srd::GATHER_BLOCK, 0, ctx->stream>>>(fdev, adev, pass, vt, in, in_count, fail_list, fail_count);
+    else if (ah.num_keys == 0)
+        srd::k_frag_gather_agg<false, true><<<f->final_grid, srd::GATHER_BLOCK, 0, ctx->stream>>>(fdev, adev, pass, vt, in, in_count, nullptr, nullptr);
+    else if (f->smem_agg)
+        srd::k_frag_gather_agg<true><<<f->final_grid, srd::GATHER_BLOCK, a->smem_bytes, ctx->stream>>>(fdev, adev, pass, vt, in, in_count, nullptr, nullptr);
+    else
+        srd::k_frag_gather_agg<false><<<f->final_grid, srd::GATHER_BLOCK, 0, ctx->stream>>>(fdev, adev, pass, vt, in, in_count, fail_list, fail_count);
+    SR_LAUNCH_CHECK(ctx);
     return SR_OK;
 }
 
@@ -601,13 +686,14 @@ static int32_t frag_push(sr_fragment* f, const sr_chunk_view* fact) {
     if (f->selective) {
         const srd::FragDev* fdev = (const srd::FragDev*)f->dev.p;
         // worst case every row survives, plus one partly used chunk per warp of the writing pass
-        const size_t slack = (size_t)srd::SEL_CHUNK * ((size_t)f->stream_grid * (srd::STREAM_BLOCK / 32) + (size_t)f->grid * (srd::GATHER_BLOCK / 32));
+        const size_t slack = (size_t)srd::SEL_CHUNK * ((size_t)f->stream_grid * (srd::STREAM_BLOCK / 32) + (size_t)f->gather_grid * (srd::GATHER_BLOCK / 32));
         SR_TRY(f->sel[0].reserve(ctx, sizeof(srd::SelEntry) * ((size_t)n + slack)));
         if (!f->gather_joins.empty()) SR_TRY(f->sel[1].reserve(ctx, sizeof(srd::SelEntry) * ((size_t)n + slack)));
         const srd::PassDev& pass = f->pass;
         const bool carry = pass.carry_join >= 0;
         unsigned long long* cnt = f->pass_counters.as<unsigned long long>();
-        SR_CUDA(ctx, cudaMemsetAsync(cnt, 0, 16 * sizeof(uint64_t), ctx->stream));
+        SR_CUDA(ctx, cudaMemsetAsync(cnt, 0, PASS_CNT_WORDS * sizeof(uint64_t), ctx->stream));
+        unsigned long long* sel_count = cnt + PASS_CNT_SEL; // [k]: entries of the selection vector after k gather passes
         const int sgrid = (int)std::min<int64_t>(f->stream_grid, (n + srd::STREAM_TILE - 1) / srd::STREAM_TILE);
         // pass boundaries are bracketed with CUDA events (bench.py reads them back as per-kernel durations)
         if (!f->ev[0])
@@ -622,20 +708,20 @@ static int32_t frag_push(sr_fragment* f, const sr_chunk_view* fact) {
         }
         if (tests) {
             if (carry)
-                srd::k_frag_stream_tests<true><<<sgrid, srd::STREAM_BLOCK, f->stream_smem, ctx->stream>>>(fdev, pass, vt, n, f->sel[0].as<srd::SelEntry>(), cnt);
+                srd::k_frag_stream_tests<true><<<sgrid, srd::STREAM_BLOCK, f->stream_smem, ctx->stream>>>(fdev, pass, vt, n, f->sel[0].as<srd::SelEntry>(), sel_count);
             else
-                srd::k_frag_stream_tests<false><<<sgrid, srd::STREAM_BLOCK, f->stream_smem, ctx->stream>>>(fdev, pass, vt, n, f->sel[0].as<srd::SelEntry>(), cnt);
+                srd::k_frag_stream_tests<false><<<sgrid, srd::STREAM_BLOCK, f->stream_smem, ctx->stream>>>(fdev, pass, vt, n, f->sel[0].as<srd::SelEntry>(), sel_count);
         } else if (carry) {
-            srd::k_frag_stream<true><<<sgrid, srd::STREAM_BLOCK, f->stream_smem, ctx->stream>>>(fdev, pass, vt, n, f->sel[0].as<srd::SelEntry>(), cnt);
+            srd::k_frag_stream<true><<<sgrid, srd::STREAM_BLOCK, f->stream_smem, ctx->stream>>>(fdev, pass, vt, n, f->sel[0].as<srd::SelEntry>(), sel_count);
         } else {
-            srd::k_frag_stream<false><<<sgrid, srd::STREAM_BLOCK, f->stream_smem, ctx->stream>>>(fdev, pass, vt, n, f->sel[0].as<srd::SelEntry>(), cnt);
+            srd::k_frag_stream<false><<<sgrid, srd::STREAM_BLOCK, f->stream_smem, ctx->stream>>>(fdev, pass, vt, n, f->sel[0].as<srd::SelEntry>(), sel_count);
         }
         SR_LAUNCH_CHECK(ctx);
         SR_CUDA(ctx, cudaEventRecord(f->ev[1], ctx->stream));
         int cur = 0, k = 0;
         for (int q : f->gather_joins) {
-            srd::k_frag_gather_join<<<f->grid, srd::GATHER_BLOCK, 0, ctx->stream>>>(fdev, q, vt, f->sel[cur].as<srd::SelEntry>(), cnt + k,
-                                                                                  f->sel[cur ^ 1].as<srd::SelEntry>(), cnt + k + 1);
+            srd::k_frag_gather_join<<<f->gather_grid, srd::GATHER_BLOCK, 0, ctx->stream>>>(fdev, q, vt, f->sel[cur].as<srd::SelEntry>(), sel_count + k,
+                                                                                         f->sel[cur ^ 1].as<srd::SelEntry>(), sel_count + k + 1);
             SR_LAUNCH_CHECK(ctx);
             cur ^= 1;
             k++;
@@ -643,44 +729,16 @@ static int32_t frag_push(sr_fragment* f, const sr_chunk_view* fact) {
         SR_CUDA(ctx, cudaEventRecord(f->ev[2], ctx->stream));
         // hash table: rows it refuses go to the other selection buffer (free by now) and are retried after a growth
         if (hash) SR_TRY(f->sel[cur ^ 1].reserve(ctx, sizeof(srd::SelEntry) * ((size_t)n + slack)));
-        srd::SelEntry* fail_list = hash ? f->sel[cur ^ 1].as<srd::SelEntry>() : nullptr;
-        unsigned long long* fail_count = cnt + 8;
-        // the batched final pass needs plain int32 fact columns and the shared-memory accumulators it was planned for
-        // (a push whose aggregate input turned nullable switches the aggregate to global accumulation)
-        const bool dense_final = f->final_dense_ok && vt.plain32 && f->smem_agg && a->smem_bytes > 0;
-        f->final_pass = dense_final ? SR_FINAL_PASS_DENSE : f->expand ? SR_FINAL_PASS_EXPAND : SR_FINAL_PASS_GENERIC;
-        if (dense_final) {
-            srd::FinalDense fp = f->final_dense;
-            for (int c = 0; c < fp.num_vals; c++) {
-                fp.cols[c] = (const int32_t*)vt.v[pass.final_vals[c]].data;
-                if (pass.carry_join >= 0 && pass.final_vals[c] == pass.carry_value_id) fp.carry_val = c;
-            }
-            for (int q = 0; q < fp.num_fns; q++) fp.fn[q].gacc = ah.fns[f->final_fn_src[q]].acc0;
-            fp.gcnt = ah.cnt_star;
-            fp.flags = ah.flags;
-            fp.rows_passed = f->host.rows_passed;
-            srd::k_frag_final_dense<srd::FINAL_ROWS><<<f->final_dense_grid, srd::GATHER_BLOCK, a->smem_bytes, ctx->stream>>>(fp, f->sel[cur].as<srd::SelEntry>(), cnt + k);
-        } else if (f->expand)
-            srd::k_frag_gather_agg_expand<<<f->final_grid, srd::GATHER_BLOCK, 0, ctx->stream>>>(fdev, (const srd::AggDev*)a->dev.p, pass, vt,
-                                                                                       f->sel[cur].as<srd::SelEntry>(), cnt + k, fail_list, fail_count);
-        else if (ah.num_keys == 0)
-            srd::k_frag_gather_agg<false, true><<<f->final_grid, srd::GATHER_BLOCK, 0, ctx->stream>>>(fdev, (const srd::AggDev*)a->dev.p, pass, vt,
-                                                                                              f->sel[cur].as<srd::SelEntry>(), cnt + k, nullptr, nullptr);
-        else if (f->smem_agg)
-            srd::k_frag_gather_agg<true><<<f->final_grid, srd::GATHER_BLOCK, a->smem_bytes, ctx->stream>>>(fdev, (const srd::AggDev*)a->dev.p, pass, vt,
-                                                                                                   f->sel[cur].as<srd::SelEntry>(), cnt + k, nullptr, nullptr);
-        else
-            srd::k_frag_gather_agg<false><<<f->final_grid, srd::GATHER_BLOCK, 0, ctx->stream>>>(fdev, (const srd::AggDev*)a->dev.p, pass, vt,
-                                                                                        f->sel[cur].as<srd::SelEntry>(), cnt + k, fail_list, fail_count);
-        SR_LAUNCH_CHECK(ctx);
+        unsigned long long* fail_count = cnt + PASS_CNT_FAIL;
+        unsigned long long* spare_count = fail_count + 1;
+        SR_TRY(frag_launch_final(f, vt, f->sel[cur].as<srd::SelEntry>(), sel_count + k, hash ? f->sel[cur ^ 1].as<srd::SelEntry>() : nullptr, fail_count));
         SR_CUDA(ctx, cudaEventRecord(f->ev[3], ctx->stream));
         f->timed_push = true;
         if (hash) {
-            int fc = 8; // index of the live fail counter in `cnt`
             while (true) {
                 uint64_t ng;
                 int32_t ovf, bad;
-                SR_CUDA(ctx, cudaMemcpyAsync(ctx->pinned + 16, cnt + fc, 8, cudaMemcpyDeviceToHost, ctx->stream));
+                SR_CUDA(ctx, cudaMemcpyAsync(ctx->pinned + 16, fail_count, 8, cudaMemcpyDeviceToHost, ctx->stream));
                 SR_TRY(agg_read_counters(a, &ng, &ovf, &bad)); // synchronises
                 a->ngroups_host = (int64_t)ng;
                 const uint64_t failed = ctx->pinned[16];
@@ -693,30 +751,23 @@ static int32_t frag_push(sr_fragment* f, const sr_chunk_view* fact) {
                 while ((uint64_t)a->ngroups_host + failed > cap / 2) cap *= 2;
                 if (cap > (1ull << 33)) return sr_fail(ctx, SR_ERR_OUT_OF_MEMORY, "aggregate table would exceed 2^33 slots; push smaller batches");
                 SR_TRY(agg_grow(a, cap));
-                cur ^= 1; // the fail list becomes the input, the old input buffer the new fail list
-                const int nfc = fc == 8 ? 9 : 8;
-                SR_CUDA(ctx, cudaMemsetAsync(cnt + nfc, 0, 8, ctx->stream));
-                if (f->expand)
-                    srd::k_frag_gather_agg_expand<<<f->final_grid, srd::GATHER_BLOCK, 0, ctx->stream>>>(fdev, (const srd::AggDev*)a->dev.p, pass, vt,
-                                                                                               f->sel[cur].as<srd::SelEntry>(), cnt + fc,
-                                                                                               f->sel[cur ^ 1].as<srd::SelEntry>(), cnt + nfc);
-                else
-                    srd::k_frag_gather_agg<false><<<f->final_grid, srd::GATHER_BLOCK, 0, ctx->stream>>>(fdev, (const srd::AggDev*)a->dev.p, pass, vt,
-                                                                                                f->sel[cur].as<srd::SelEntry>(), cnt + fc,
-                                                                                                f->sel[cur ^ 1].as<srd::SelEntry>(), cnt + nfc);
-                SR_LAUNCH_CHECK(ctx);
-                fc = nfc;
+                // the fail list and its counter become the input, the old input buffer and the spare counter the new
+                // fail list; the launch runs the kernel of the first one (a hash aggregate's, see frag_launch_final)
+                cur ^= 1;
+                std::swap(fail_count, spare_count);
+                SR_CUDA(ctx, cudaMemsetAsync(fail_count, 0, 8, ctx->stream));
+                SR_TRY(frag_launch_final(f, vt, f->sel[cur].as<srd::SelEntry>(), spare_count, f->sel[cur ^ 1].as<srd::SelEntry>(), fail_count));
             }
         }
         return SR_OK;
     }
-    const int grid = (int)std::min<int64_t>(f->grid, (n + srd::FRAG_TILE - 1) / srd::FRAG_TILE);
+    const int grid = (int)std::min<int64_t>(f->cascade_grid, (n + srd::FRAG_TILE - 1) / srd::FRAG_TILE);
     if (f->smem_agg)
-        srd::k_fragment<true><<<grid, srd::FRAG_BLOCK, f->smem_bytes, ctx->stream>>>((const srd::FragDev*)f->dev.p, (const srd::AggDev*)a->dev.p, vt, n,
-                                                                                    f->queue_word_off);
+        srd::k_fragment<true><<<grid, srd::FRAG_BLOCK, f->cascade_smem, ctx->stream>>>((const srd::FragDev*)f->dev.p, (const srd::AggDev*)a->dev.p, vt, n,
+                                                                                      f->queue_word_off);
     else
-        srd::k_fragment<false><<<grid, srd::FRAG_BLOCK, f->smem_bytes, ctx->stream>>>((const srd::FragDev*)f->dev.p, (const srd::AggDev*)a->dev.p, vt, n,
-                                                                                     f->queue_word_off);
+        srd::k_fragment<false><<<grid, srd::FRAG_BLOCK, f->cascade_smem, ctx->stream>>>((const srd::FragDev*)f->dev.p, (const srd::AggDev*)a->dev.p, vt, n,
+                                                                                       f->queue_word_off);
     SR_LAUNCH_CHECK(ctx);
     if (hash) {
         uint64_t ng;

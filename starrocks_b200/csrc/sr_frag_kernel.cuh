@@ -28,6 +28,33 @@ struct FragDev {
     unsigned long long* rows_passed;
 };
 
+// k_frag_sample's counters: [j] rows passing join j, [SAMPLE_ALL_PREDS] rows passing every scan conjunct,
+// [SAMPLE_PREDS_UPTO + p] rows passing conjuncts 0..p
+constexpr int SAMPLE_ALL_PREDS = SR_MAX_FRAG_JOINS;
+constexpr int SAMPLE_PREDS_UPTO = 16;
+constexpr int SAMPLE_COUNTERS = SAMPLE_PREDS_UPTO + 8;
+static_assert(SAMPLE_ALL_PREDS < SAMPLE_PREDS_UPTO, "sample counter layout");
+
+// kernel prologues: copy `count` descriptors into shared memory, block-cooperatively (the caller synchronises)
+template <typename T>
+__device__ __forceinline__ void smem_copy(T* dst, const T* src, int count) {
+    for (int i = threadIdx.x; i < (int)(sizeof(T) / 4) * count; i += blockDim.x) ((uint32_t*)dst)[i] = ((const uint32_t*)src)[i];
+}
+
+// copy the bitmaps of joins [0, nj) that the plan put in shared memory (smem_off >= 0); GUARD: plus one zero word behind
+// each copy (stream_test_reg clamps an out-of-range key onto it)
+template <bool GUARD>
+__device__ __forceinline__ void smem_stage_bitmaps(uint32_t* smem, const FragJoinDev* joins, int nj) {
+    for (int j = 0; j < nj; j++) {
+        const FragJoinDev& fj = joins[j];
+        if (fj.smem_off < 0) continue;
+        if (GUARD)
+            for (int w = threadIdx.x; w <= fj.bitmap_words; w += blockDim.x) smem[fj.smem_off + w] = w < fj.bitmap_words ? fj.j.bitmap[w] : 0u;
+        else
+            for (int w = threadIdx.x; w < fj.bitmap_words; w += blockDim.x) smem[fj.smem_off + w] = fj.j.bitmap[w];
+    }
+}
+
 constexpr int FRAG_BLOCK = 512;
 constexpr int FRAG_WARPS = FRAG_BLOCK / 32;
 constexpr int FRAG_ROWS = 4;   // consecutive rows per thread and group (one 128-bit load of an int32 column)
@@ -233,13 +260,9 @@ __global__ void __launch_bounds__(FRAG_BLOCK, 2) k_fragment(const FragDev* __res
     const AggDev& ad = *adp;
     const int S = fd.num_joins;
     // descriptors + bitmaps of the leading joins into shared memory
-    for (int i = threadIdx.x; i < (int)(sizeof(FragJoinDev) / 4) * S; i += blockDim.x) ((uint32_t*)s_joins)[i] = ((const uint32_t*)fd.joins)[i];
-    for (int i = threadIdx.x; i < (int)(sizeof(CPred) / 4) * fd.num_preds; i += blockDim.x) ((uint32_t*)s_preds)[i] = ((const uint32_t*)fd.preds)[i];
-    for (int j = 0; j < S; j++) {
-        const FragJoinDev& fj = fd.joins[j];
-        if (fj.smem_off >= 0)
-            for (int w = threadIdx.x; w < fj.bitmap_words; w += blockDim.x) smem[fj.smem_off + w] = fj.j.bitmap[w];
-    }
+    smem_copy(s_joins, fd.joins, S);
+    smem_copy(s_preds, fd.preds, fd.num_preds);
+    smem_stage_bitmaps<false>(smem, fd.joins, S);
     AccPtrs acc;
     if (SMEM_AGG) {
         acc_ptrs_smem(ad, (long long*)smem, acc);
@@ -408,7 +431,7 @@ __global__ void __launch_bounds__(256) k_frag_sample(const FragDev* __restrict__
     for (int64_t row = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; row < n; row += (int64_t)gridDim.x * blockDim.x) {
         ChunkLoader ld{vt, row};
         {
-            // rows passing every scan conjunct -> counts[SR_MAX_FRAG_JOINS]
+            // rows passing every scan conjunct -> counts[SAMPLE_ALL_PREDS]
             bool pass = true;
             for (int p = 0; p < fd.num_preds; p++) {
                 if (pass) {
@@ -416,9 +439,9 @@ __global__ void __launch_bounds__(256) k_frag_sample(const FragDev* __restrict__
                     const bool nul = ld.load(fd.preds[p].value_id, bits);
                     pass = eval_pred(fd.preds[p], bits, nul);
                 }
-                // rows passing conjuncts 0..p -> counts[16 + p] (how many rows reach the next streamed column)
+                // rows passing conjuncts 0..p -> counts[SAMPLE_PREDS_UPTO + p] (how many rows reach the next streamed column)
                 const uint32_t mp = __ballot_sync(__activemask(), pass);
-                if (pass && (mp & lanemask_lt()) == 0) atomicAdd(&counts[16 + p], (unsigned long long)__popc(mp));
+                if (pass && (mp & lanemask_lt()) == 0) atomicAdd(&counts[SAMPLE_PREDS_UPTO + p], (unsigned long long)__popc(mp));
             }
             for (int e = 0; e < fd.num_exprs && pass; e++) {
                 int64_t bits;
@@ -426,7 +449,7 @@ __global__ void __launch_bounds__(256) k_frag_sample(const FragDev* __restrict__
                 pass = !nul && bits != 0;
             }
             const uint32_t m = __ballot_sync(__activemask(), pass);
-            if (pass && (m & lanemask_lt()) == 0) atomicAdd(&counts[SR_MAX_FRAG_JOINS], (unsigned long long)__popc(m));
+            if (pass && (m & lanemask_lt()) == 0) atomicAdd(&counts[SAMPLE_ALL_PREDS], (unsigned long long)__popc(m));
         }
         for (int j = 0; j < fd.num_joins; j++) {
             const FragJoinDev& fj = fd.joins[j];

@@ -30,7 +30,7 @@ struct StreamTest {
 };
 #define SR_MAX_STREAM_TESTS 6
 
-// How k_frag_stream_tests runs one of its two vector-column tests, planned on the host (frag_plan) and read from the kernel
+// How k_frag_stream_tests runs one of its two vector-column tests, planned on the host (frag_plan_stream_tests) and read from the kernel
 // parameter: nothing of it occupies a register of the issue-bound, register-capped kernel, and nothing is re-read from
 // shared memory per tile.  kind: 0 = range conjunct, 1 = bitmap in shared memory at word smem_off (int32 index arithmetic,
 // zero GUARD bit at index span + 1: an out-of-range key is clamped onto it, so the test needs neither a predicate nor a
@@ -244,13 +244,9 @@ __global__ void __launch_bounds__(STREAM_BLOCK, 2) k_frag_stream(const FragDev* 
     __shared__ CPred s_preds[8];
     const FragDev& fd = *fdp;
     const int SJ = pd.num_stream_joins;
-    for (int i = threadIdx.x; i < (int)(sizeof(FragJoinDev) / 4) * SJ; i += blockDim.x) ((uint32_t*)s_joins)[i] = ((const uint32_t*)fd.joins)[i];
-    for (int i = threadIdx.x; i < (int)(sizeof(CPred) / 4) * fd.num_preds; i += blockDim.x) ((uint32_t*)s_preds)[i] = ((const uint32_t*)fd.preds)[i];
-    for (int j = 0; j < SJ; j++) {
-        const FragJoinDev& fj = fd.joins[j];
-        if (fj.smem_off >= 0)
-            for (int w = threadIdx.x; w < fj.bitmap_words; w += blockDim.x) smem[fj.smem_off + w] = fj.j.bitmap[w];
-    }
+    smem_copy(s_joins, fd.joins, SJ);
+    smem_copy(s_preds, fd.preds, fd.num_preds);
+    smem_stage_bitmaps<false>(smem, fd.joins, SJ);
     __syncthreads();
 
     // (the common shapes -- range conjuncts and joins on plain int32 columns -- run in k_frag_stream_tests below;
@@ -419,13 +415,9 @@ __global__ void __launch_bounds__(STREAM_BLOCK, 2) k_frag_stream_tests(const Fra
     const int SJ = pd.num_stream_joins;
     const int NT = pd.num_tests;
     const int NV = pd.num_vec;
-    for (int i = threadIdx.x; i < (int)(sizeof(FragJoinDev) / 4) * SJ; i += blockDim.x) ((uint32_t*)s_joins)[i] = ((const uint32_t*)fd.joins)[i];
-    for (int i = threadIdx.x; i < (int)(sizeof(StreamTest) / 4) * NT; i += blockDim.x) ((uint32_t*)s_tests)[i] = ((const uint32_t*)pd.tests)[i];
-    for (int j = 0; j < SJ; j++) {
-        const FragJoinDev& fj = fd.joins[j];
-        if (fj.smem_off >= 0) // + the zero guard word behind the copy (frag_plan reserves it)
-            for (int w = threadIdx.x; w <= fj.bitmap_words; w += blockDim.x) smem[fj.smem_off + w] = w < fj.bitmap_words ? fj.j.bitmap[w] : 0u;
-    }
+    smem_copy(s_joins, fd.joins, SJ);
+    smem_copy(s_tests, pd.tests, NT);
+    smem_stage_bitmaps<true>(smem, fd.joins, SJ); // + the zero guard words (frag_plan_stream_smem reserves them)
     __syncthreads();
     const VecTest& t0 = pd.vec[0];
     const VecTest& t1 = pd.vec[1];
@@ -524,7 +516,7 @@ __global__ void __launch_bounds__(GATHER_BLOCK) k_frag_gather_join(const FragDev
                                                                     SelEntry* __restrict__ sel_out, unsigned long long* __restrict__ counter_out) {
     extern __shared__ __align__(16) uint32_t smem[];
     __shared__ FragJoinDev s_join;
-    for (int i = threadIdx.x; i < (int)(sizeof(FragJoinDev) / 4); i += blockDim.x) ((uint32_t*)&s_join)[i] = ((const uint32_t*)&fdp->joins[j])[i];
+    smem_copy(&s_join, &fdp->joins[j], 1);
     __syncthreads();
     const unsigned long long n_in = *n_in_ptr;
     const FragJoinDev& fj = s_join;
@@ -578,7 +570,7 @@ __global__ void __launch_bounds__(GATHER_BLOCK, GATHER_AGG_MIN_BLOCKS) k_frag_ga
     const int S = fd.num_joins;
     const bool hash_table = !SINGLE && !ad.dense && ad.num_keys > 0;
     unsigned long long known_groups = hash_table && fail_list ? *(volatile unsigned long long*)ad.ngroups : 0ull;
-    for (int i = threadIdx.x; i < (int)(sizeof(FragJoinDev) / 4) * S; i += blockDim.x) ((uint32_t*)s_joins)[i] = ((const uint32_t*)fd.joins)[i];
+    smem_copy(s_joins, fd.joins, S);
     AccPtrs acc;
     if (SMEM_AGG) {
         acc_ptrs_smem(ad, (long long*)smem, acc);
@@ -915,7 +907,7 @@ __global__ void __launch_bounds__(GATHER_BLOCK) k_frag_gather_agg_expand(const F
     const bool single = ad.num_keys == 0;
     const bool hash_table = !ad.dense && ad.num_keys > 0;
     unsigned long long known_groups = hash_table && fail_list ? *(volatile unsigned long long*)ad.ngroups : 0ull;
-    for (int i = threadIdx.x; i < (int)(sizeof(FragJoinDev) / 4) * S; i += blockDim.x) ((uint32_t*)s_joins)[i] = ((const uint32_t*)fd.joins)[i];
+    smem_copy(s_joins, fd.joins, S);
     AccPtrs acc;
     acc_ptrs_global(ad, acc);
     __syncthreads();

@@ -1355,19 +1355,21 @@ int32_t sr_fragment_get_plan(sr_fragment* frag, sr_fragment_plan* plan) {
         plan->bitmap_in_smem[q] = frag->host.joins[q].smem_off >= 0 ? 1 : 0;
         plan->pass_rate[q] = frag->pass_rate[q];
     }
-    plan->smem_bytes = (int32_t)frag->smem_bytes;
-    plan->grid = frag->grid;
-    plan->block = srd::FRAG_BLOCK;
     plan->agg_in_smem = frag->smem_agg ? 1 : 0;
     plan->mode = frag->selective ? 2 : 1;
     plan->num_stream_joins = frag->selective ? frag->pass.num_stream_joins : 0;
     plan->num_gather_passes = frag->selective ? (int32_t)frag->gather_joins.size() : 0;
     plan->pred_rate = frag->pred_rate;
     plan->final_pass = frag->final_pass;
+    // launch shape of the mode's first kernel: the streaming pass, or the cascade
     if (frag->selective) {
         plan->smem_bytes = (int32_t)frag->stream_smem;
         plan->grid = frag->stream_grid;
         plan->block = srd::STREAM_BLOCK;
+    } else {
+        plan->smem_bytes = (int32_t)frag->cascade_smem;
+        plan->grid = frag->cascade_grid;
+        plan->block = srd::FRAG_BLOCK;
     }
     return SR_OK;
 }
