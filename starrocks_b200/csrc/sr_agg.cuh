@@ -109,6 +109,59 @@ struct AccPtrs {
     long long* accn[SR_MAX_AGG_FNS];
 };
 
+// ---- state layout: which 8-byte arrays a table keeps, and in what order.  COUNT(*)'s counter first, then for every function
+// other than COUNT(*): acc0, acc1 (128-bit sums only), accn (when it counts its non-NULL inputs).  acc_ptrs_at is the one
+// statement of it; allocation, reset, the shared-memory images of the push kernels, the dense-state export and the
+// fragment's final pass all follow it.
+enum AccWord : int32_t { W_CNT, W_ACC0, W_ACC1, W_ACCN };
+__host__ __device__ __forceinline__ long long*& acc_ptr(AccPtrs& p, int f, AccWord w) {
+    return w == W_CNT ? p.cnt : w == W_ACC0 ? p.acc0[f] : w == W_ACC1 ? p.acc1[f] : p.accn[f];
+}
+// wire p to the arrays laid out from `base`, `stride` words apart (the table's slab, or a shared-memory image of it); the
+// arrays a table does not have are null
+__host__ __device__ __forceinline__ void acc_ptrs_at(const AggDev& a, long long* base, long long stride, AccPtrs& p) {
+    long long* q = base;
+    p.cnt = q;
+    q += stride;
+    for (int f = 0; f < SR_MAX_AGG_FNS; f++) {
+        p.acc0[f] = p.acc1[f] = p.accn[f] = nullptr;
+        if (f < a.num_fns && a.fns[f].mode != M_COUNT_STAR) {
+            p.acc0[f] = q;
+            q += stride;
+            if (a.fns[f].mode == M_SUM_I128) {
+                p.acc1[f] = q;
+                q += stride;
+            }
+            if (a.fns[f].track_n) {
+                p.accn[f] = q;
+                q += stride;
+            }
+        }
+    }
+}
+// the same layout as a walk, for host code: visit(f, word) once per array, in order (f = -1 for the counter)
+template <typename Visit>
+inline void agg_state_arrays(const AggDev& a, Visit&& visit) {
+    long long present;
+    AccPtrs p;
+    acc_ptrs_at(a, &present, 0, p); // stride 0: every array the table has points at `present`, the others are null
+    visit(-1, W_CNT);
+    for (int f = 0; f < SR_MAX_AGG_FNS; f++)
+        for (AccWord w : {W_ACC0, W_ACC1, W_ACCN})
+            if (acc_ptr(p, f, w)) visit(f, w);
+}
+inline int agg_state_words(const AggDev& a) {
+    int n = 0;
+    agg_state_arrays(a, [&](int, AccWord) { n++; });
+    return n;
+}
+// slots of every state array: a hash table has one more, the special slot of the all-ones key
+__host__ __device__ inline unsigned long long agg_slots(const AggDev& a) { return (!a.dense && a.num_keys > 0) ? a.cap + 1 : a.cap; }
+// words from one array of a table's slab to the next.  Dense arrays lie back to back: the all-reduce of the dense-state export
+// joins neighbouring arrays into one collective.  Each hash-table array starts on a 256-byte boundary, like an allocation of
+// its own, so the partitioned push's slice loads and write-backs touch whole sectors.
+inline unsigned long long agg_state_stride(const AggDev& a) { return (!a.dense && a.num_keys > 0) ? (agg_slots(a) + 31) & ~31ull : agg_slots(a); }
+
 // apply one (non-null) input value to the accumulators of slot
 __device__ __forceinline__ void acc_apply(int32_t mode, long long* a0, long long* a1, long long slot, long long bits) {
     switch (mode) {
@@ -349,9 +402,6 @@ __device__ __forceinline__ void smem_add_u64(long long* p, unsigned long long v)
     }
     if (hi) asm volatile("red.shared.add.u32 [%0], %1;" ::"r"(s + 4), "r"(hi) : "memory");
 }
-__device__ __forceinline__ void red_shared_add_u64(long long* p, unsigned long long v) {
-    smem_add_u64(p, v);
-}
 __device__ __forceinline__ void acc_apply_shared(int32_t mode, long long* a0, long long* a1, long long slot, long long bits) {
     const uint32_t s0 = (uint32_t)__cvta_generic_to_shared(a0 + slot);
     switch (mode) {
@@ -386,7 +436,7 @@ __device__ __forceinline__ void acc_apply_shared(int32_t mode, long long* a0, lo
 template <bool SHARED = false, typename Loader>
 __device__ __forceinline__ void agg_apply_row(const AggDev& a, const AccPtrs& p, long long slot, Loader& ld) {
     if (SHARED)
-        red_shared_add_u64(p.cnt + slot, 1ull);
+        smem_add_u64(p.cnt + slot, 1ull);
     else
         atomicAdd((unsigned long long*)p.cnt + slot, 1ull);
 #pragma unroll 1
@@ -404,7 +454,7 @@ __device__ __forceinline__ void agg_apply_row(const AggDev& a, const AccPtrs& p,
         }
         if (SHARED) {
             acc_apply_shared(fn.mode, p.acc0[f], p.acc1[f], slot, bits);
-            if (fn.track_n) red_shared_add_u64(p.accn[f] + slot, nadd);
+            if (fn.track_n) smem_add_u64(p.accn[f] + slot, nadd);
         } else {
             acc_apply(fn.mode, p.acc0[f], p.acc1[f], slot, bits);
             if (fn.track_n) atomicAdd((unsigned long long*)p.accn[f] + slot, nadd);
@@ -412,7 +462,7 @@ __device__ __forceinline__ void agg_apply_row(const AggDev& a, const AccPtrs& p,
     }
 }
 
-__device__ __forceinline__ void acc_ptrs_global(const AggDev& a, AccPtrs& p) {
+__host__ __device__ __forceinline__ void acc_ptrs_global(const AggDev& a, AccPtrs& p) {
     p.cnt = a.cnt_star;
     for (int f = 0; f < SR_MAX_AGG_FNS; f++) {
         p.acc0[f] = a.fns[f].acc0;
@@ -421,38 +471,19 @@ __device__ __forceinline__ void acc_ptrs_global(const AggDev& a, AccPtrs& p) {
     }
 }
 
-// shared-memory accumulators for a dense table: layout [cnt | per fn: acc0, acc1?, accn?]
-__device__ __forceinline__ void acc_ptrs_smem(const AggDev& a, long long* smem, AccPtrs& p) {
-    const long long cap = (long long)a.cap;
-    long long* q = smem;
-    p.cnt = q;
-    q += cap;
-    for (int f = 0; f < SR_MAX_AGG_FNS; f++) {
-        p.acc0[f] = p.acc1[f] = p.accn[f] = nullptr;
-        if (f < a.num_fns && a.fns[f].mode != M_COUNT_STAR) {
-            p.acc0[f] = q;
-            q += cap;
-            if (a.fns[f].mode == M_SUM_I128) {
-                p.acc1[f] = q;
-                q += cap;
-            }
-            if (a.fns[f].track_n) {
-                p.accn[f] = q;
-                q += cap;
-            }
-        }
+// every state word of slot i at its initial value
+__device__ __forceinline__ void acc_init_slot(const AggDev& a, const AccPtrs& p, long long i) {
+    p.cnt[i] = 0;
+    for (int f = 0; f < a.num_fns; f++) {
+        if (p.acc0[f]) p.acc0[f][i] = acc_init_value(a.fns[f].mode);
+        if (p.acc1[f]) p.acc1[f][i] = 0;
+        if (p.accn[f]) p.accn[f][i] = 0;
     }
 }
+// shared-memory accumulators for a dense table (wired by acc_ptrs_at with stride cap)
 __device__ __forceinline__ void acc_smem_init(const AggDev& a, const AccPtrs& p) {
     const long long cap = (long long)a.cap;
-    for (long long i = threadIdx.x; i < cap; i += blockDim.x) {
-        p.cnt[i] = 0;
-        for (int f = 0; f < a.num_fns; f++) {
-            if (p.acc0[f]) p.acc0[f][i] = acc_init_value(a.fns[f].mode);
-            if (p.acc1[f]) p.acc1[f][i] = 0;
-            if (p.accn[f]) p.accn[f][i] = 0;
-        }
-    }
+    for (long long i = threadIdx.x; i < cap; i += blockDim.x) acc_init_slot(a, p, i);
 }
 __device__ __forceinline__ void acc_smem_flush(const AggDev& a, const AccPtrs& p) {
     const long long cap = (long long)a.cap;
@@ -485,7 +516,7 @@ __global__ void __launch_bounds__(AGG_BLOCK, AGG_MIN_BLOCKS) k_agg_push(const Ag
     const AggDev& a = *ad;
     AccPtrs p;
     if (SMEM) {
-        acc_ptrs_smem(a, s_acc, p);
+        acc_ptrs_at(a, s_acc, a.cap, p);
         acc_smem_init(a, p);
         __syncthreads();
     } else {
@@ -670,9 +701,6 @@ __global__ void __launch_bounds__(AGG_BLOCK, AGG_MIN_BLOCKS) k_agg_push_single(c
     single_acc_flush(a, s);
 }
 
-__global__ void __launch_bounds__(256) k_fill_i64(long long* p, int64_t n, long long v) {
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) p[i] = v;
-}
 __global__ void __launch_bounds__(256) k_copy_i64(long long* dst, const long long* src, int64_t n) {
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) dst[i] = src[i];
 }
@@ -997,8 +1025,8 @@ struct sr_agg {
     VReg reg;
     srd::AggDev host; // host mirror of the device descriptor
     DevBuf dev;       // AggDev on device
-    DevBuf hkeys, cnt_star, counters /* ngroups + flags */;
-    DevBuf acc0[SR_MAX_AGG_FNS], acc1[SR_MAX_AGG_FNS], accn[SR_MAX_AGG_FNS];
+    DevBuf hkeys, slab /* every state array, laid out by agg_state_arrays */, counters /* ngroups + flags */;
+    DevBuf late_accn[SR_MAX_AGG_FNS]; // accn of a function whose input turned nullable after the slab was laid out
     DevBuf slots_tmp;
     // radix-partitioned push (sr_agg_part.cuh): bucket histogram / bases / cursors, tile list, staged records, retry lists
     DevBuf part_cursor, part_tiles, part_rec[2], part_ovf, part_fail, part_fail64, part_fail64b;
@@ -1082,12 +1110,39 @@ static int32_t agg_upload(sr_agg* a) {
     return SR_OK;
 }
 
-// allocate + initialise state arrays for `cap` slots into the given buffers, wiring `h`
-static int32_t agg_alloc_tables(sr_agg* a, srd::AggDev* h, uint64_t cap, DevBuf* hkeys, DevBuf* cnt, DevBuf* a0, DevBuf* a1, DevBuf* an) {
-    sr_ctx* ctx = a->ctx;
+// every key slot empty, every state array at its initial value: one memset per run of neighbouring arrays that start from
+// zero (all the arrays of a dense table of sums and counts: the per-step reset of the fused fragment is one memset), one
+// fill per MIN / MAX array.  Each array is written once, an accn started after the slab was laid out included.
+static int32_t agg_init_tables(sr_ctx* ctx, const srd::AggDev& h) {
+    const uint64_t slots = srd::agg_slots(h), stride = srd::agg_state_stride(h);
+    const int grid = std::min(grid_for((int64_t)slots, 256), ctx->num_sms * 8);
+    if (h.hkeys) {
+        srd::k_fill_u64<<<grid, 256, 0, ctx->stream>>>(h.hkeys, (int64_t)(slots * (h.wide ? 2 : 1)), SR_AGG_EMPTY);
+        SR_LAUNCH_CHECK(ctx);
+    }
+    srd::AccPtrs p;
+    srd::acc_ptrs_global(h, p);
+    std::vector<std::pair<long long*, long long>> arrays; // (array, initial value) in layout order
+    srd::agg_state_arrays(h, [&](int f, srd::AccWord w) {
+        arrays.push_back({srd::acc_ptr(p, f, w), w == srd::W_ACC0 ? srd::acc_init_value(h.fns[f].mode) : 0});
+    });
+    for (size_t i = 0, j; i < arrays.size(); i = j) {
+        j = i + 1;
+        if (arrays[i].second != 0) {
+            srd::k_fill_u64<<<grid, 256, 0, ctx->stream>>>((unsigned long long*)arrays[i].first, (int64_t)slots, (unsigned long long)arrays[i].second);
+            SR_LAUNCH_CHECK(ctx);
+            continue;
+        }
+        while (j < arrays.size() && arrays[j].second == 0 && arrays[j].first == arrays[j - 1].first + stride) j++;
+        SR_CUDA(ctx, cudaMemsetAsync(arrays[i].first, 0, sizeof(int64_t) * (size_t)(arrays[j - 1].first + slots - arrays[i].first), ctx->stream));
+    }
+    return SR_OK;
+}
+
+// allocate + initialise the tables of `cap` slots into the given buffers, wiring `h`.  hkeys is an allocation of its own: the
+// 128-bit claim needs 16-byte aligned pairs.
+static int32_t agg_alloc_tables(sr_ctx* ctx, srd::AggDev* h, uint64_t cap, DevBuf* hkeys, DevBuf* slab) {
     const bool hash = !h->dense && h->num_keys > 0;
-    const uint64_t total = hash ? cap + 1 : cap;
-    const int grid = std::min(grid_for((int64_t)total, 256), ctx->num_sms * 8);
     h->cap = cap;
     h->mask = cap - 1;
     h->limit = hash ? cap / 2 : ~0ull;
@@ -1100,75 +1155,45 @@ static int32_t agg_alloc_tables(sr_agg* a, srd::AggDev* h, uint64_t cap, DevBuf*
         h->slice_log2 = 0;
         h->slice_mask = 0;
     }
+    h->hkeys = nullptr;
     if (hash) {
-        const uint64_t kwords = total * (h->wide ? 2 : 1);
-        SR_TRY(hkeys->reserve(ctx, sizeof(uint64_t) * kwords));
-        srd::k_fill_u64<<<grid, 256, 0, ctx->stream>>>(hkeys->as<unsigned long long>(), (int64_t)kwords, SR_AGG_EMPTY);
-        SR_LAUNCH_CHECK(ctx);
+        SR_TRY(hkeys->reserve(ctx, sizeof(uint64_t) * srd::agg_slots(*h) * (h->wide ? 2 : 1)));
         h->hkeys = hkeys->as<unsigned long long>();
-    } else {
-        h->hkeys = nullptr;
     }
-    if (!hash) {
-        // dense tables: ONE slab holds every state array back to back (cnt | per fn: acc0, acc1?, accn?), so that the
-        // element-wise merge of the partial tables of several GPUs (sr_agg_dense_state + all-reduce) is one in-place
-        // collective over one contiguous range per (operator, element type) instead of a cat / copy per array
-        size_t words = 1;
-        for (int f = 0; f < h->num_fns; f++)
-            if (h->fns[f].mode != srd::M_COUNT_STAR) words += 1 + (h->fns[f].mode == srd::M_SUM_I128 ? 1 : 0) + (h->fns[f].track_n ? 1 : 0);
-        SR_TRY(cnt->reserve(ctx, sizeof(int64_t) * total * words));
-        SR_CUDA(ctx, cudaMemsetAsync(cnt->p, 0, sizeof(int64_t) * total * words, ctx->stream));
-        long long* q = cnt->as<long long>();
-        h->cnt_star = q;
-        q += total;
-        for (int f = 0; f < h->num_fns; f++) {
-            srd::AggFnDev& fn = h->fns[f];
-            fn.acc0 = fn.acc1 = fn.accn = nullptr;
-            if (fn.mode == srd::M_COUNT_STAR) continue;
-            fn.acc0 = q;
-            q += total;
-            if (srd::acc_init_value(fn.mode) != 0) {
-                srd::k_fill_i64<<<grid, 256, 0, ctx->stream>>>(fn.acc0, (int64_t)total, srd::acc_init_value(fn.mode));
-                SR_LAUNCH_CHECK(ctx);
-            }
-            if (fn.mode == srd::M_SUM_I128) {
-                fn.acc1 = q;
-                q += total;
-            }
-            if (fn.track_n) {
-                fn.accn = q;
-                q += total;
-            }
-        }
-        return SR_OK;
+    // ONE slab holds every state array: for a dense table the element-wise merge of the partial tables of several GPUs
+    // (sr_agg_dense_state + all-reduce) is then one in-place collective over one contiguous range per (operator, element
+    // type), and every reset is one memset
+    const uint64_t stride = srd::agg_state_stride(*h);
+    SR_TRY(slab->reserve(ctx, sizeof(int64_t) * stride * srd::agg_state_words(*h)));
+    srd::AccPtrs p;
+    srd::acc_ptrs_at(*h, slab->as<long long>(), stride, p);
+    h->cnt_star = p.cnt;
+    for (int f = 0; f < SR_MAX_AGG_FNS; f++) {
+        h->fns[f].acc0 = p.acc0[f];
+        h->fns[f].acc1 = p.acc1[f];
+        h->fns[f].accn = p.accn[f];
     }
-    SR_TRY(cnt->reserve(ctx, sizeof(int64_t) * total));
-    SR_CUDA(ctx, cudaMemsetAsync(cnt->p, 0, sizeof(int64_t) * total, ctx->stream));
-    h->cnt_star = cnt->as<long long>();
-    for (int f = 0; f < h->num_fns; f++) {
-        srd::AggFnDev& fn = h->fns[f];
-        fn.acc0 = fn.acc1 = fn.accn = nullptr;
-        if (fn.mode == srd::M_COUNT_STAR) continue;
-        SR_TRY(a0[f].reserve(ctx, sizeof(int64_t) * total));
-        srd::k_fill_i64<<<grid, 256, 0, ctx->stream>>>(a0[f].as<long long>(), (int64_t)total, srd::acc_init_value(fn.mode));
-        SR_LAUNCH_CHECK(ctx);
-        fn.acc0 = a0[f].as<long long>();
-        if (fn.mode == srd::M_SUM_I128) {
-            SR_TRY(a1[f].reserve(ctx, sizeof(int64_t) * total));
-            SR_CUDA(ctx, cudaMemsetAsync(a1[f].p, 0, sizeof(int64_t) * total, ctx->stream));
-            fn.acc1 = a1[f].as<long long>();
-        }
-        if (fn.track_n) {
-            SR_TRY(an[f].reserve(ctx, sizeof(int64_t) * total));
-            SR_CUDA(ctx, cudaMemsetAsync(an[f].p, 0, sizeof(int64_t) * total, ctx->stream));
-            fn.accn = an[f].as<long long>();
-        }
-    }
-    return SR_OK;
+    return agg_init_tables(ctx, *h);
 }
 
-// bytes of table state one group slot owns (keys + COUNT(*) + every accumulator array)
-static uint64_t agg_slot_bytes(const srd::AggDev& h) { return (uint64_t)srd::agg_slot_bytes_of(h); }
+// counters and tables of `cap` slots for the compiled layout in a->host, and whether pushes accumulate in shared memory
+static int32_t agg_setup_tables(sr_agg* a, uint64_t cap) {
+    sr_ctx* ctx = a->ctx;
+    srd::AggDev& h = a->host;
+    SR_TRY(a->counters.reserve(ctx, 64));
+    SR_CUDA(ctx, cudaMemsetAsync(a->counters.p, 0, 64, ctx->stream));
+    h.ngroups = a->counters.as<unsigned long long>();
+    h.flags = (int32_t*)(a->counters.as<unsigned long long>() + 1);
+    SR_TRY(agg_alloc_tables(ctx, &h, cap, &a->hkeys, &a->slab));
+    // shared-memory accumulation for small dense tables -- including the single state of a query without GROUP BY
+    // inside a fused fragment (every surviving row would otherwise hit the same global address with an atomic; the
+    // standalone push reduces per warp instead, k_agg_push_single)
+    const size_t bytes = sizeof(int64_t) * cap * srd::agg_state_words(h);
+    a->smem_bytes = h.dense && bytes <= 40 * 1024 ? bytes : 0;
+    SR_TRY(agg_upload(a));
+    a->compiled = true;
+    return SR_OK;
+}
 
 typedef int32_t (*agg_type_fn)(void* user, int32_t slot);
 typedef bool (*agg_nullable_fn)(void* user, int32_t slot);
@@ -1307,26 +1332,7 @@ static int32_t agg_compile(sr_agg* a, slot_type_fn tf, agg_nullable_fn nf, void*
         const uint64_t want = d.expected_groups > 0 ? (uint64_t)d.expected_groups * 2 : 0; // load <= 1/2: a probe sequence stays in its 256-slot slice
         while (cap < want) cap <<= 1;
     }
-    SR_TRY(a->counters.reserve(ctx, 64));
-    SR_CUDA(ctx, cudaMemsetAsync(a->counters.p, 0, 64, ctx->stream));
-    h.ngroups = a->counters.as<unsigned long long>();
-    h.flags = (int32_t*)(a->counters.as<unsigned long long>() + 1);
-    SR_TRY(agg_alloc_tables(a, &h, cap, &a->hkeys, &a->cnt_star, a->acc0, a->acc1, a->accn));
-    // shared-memory accumulation for small dense tables -- including the single state of a query without GROUP BY
-    // inside a fused fragment (every surviving row would otherwise hit the same global address with an atomic; the
-    // standalone push reduces per warp instead, k_agg_push_single)
-    a->smem_bytes = 0;
-    if (h.dense) {
-        size_t words = 1;
-        for (int f = 0; f < h.num_fns; f++) {
-            if (h.fns[f].mode == srd::M_COUNT_STAR) continue;
-            words += 1 + (h.fns[f].mode == srd::M_SUM_I128 ? 1 : 0) + (h.fns[f].track_n ? 1 : 0);
-        }
-        const size_t bytes = words * cap * sizeof(int64_t);
-        if (bytes <= 40 * 1024) a->smem_bytes = bytes;
-    }
-    SR_TRY(agg_upload(a));
-    a->compiled = true;
+    SR_TRY(agg_setup_tables(a, cap));
     // COUNT(DISTINCT value): the (group keys, value) set, an aggregate without functions over the same input
     for (int f = 0; f < d.num_fns; f++) {
         if (d.fns[f].kind != SR_AGG_COUNT_DISTINCT) continue;
@@ -1353,8 +1359,8 @@ static int32_t agg_compile(sr_agg* a, slot_type_fn tf, agg_nullable_fn nf, void*
 static int32_t agg_grow(sr_agg* a, uint64_t new_cap) {
     sr_ctx* ctx = a->ctx;
     srd::AggDev nh = a->host;
-    DevBuf nk, nc, n0[SR_MAX_AGG_FNS], n1[SR_MAX_AGG_FNS], nn[SR_MAX_AGG_FNS], ndev;
-    SR_TRY(agg_alloc_tables(a, &nh, new_cap, &nk, &nc, n0, n1, nn));
+    DevBuf nk, nslab, ndev;
+    SR_TRY(agg_alloc_tables(ctx, &nh, new_cap, &nk, &nslab));
     SR_TRY(ndev.reserve(ctx, sizeof(srd::AggDev)));
     SR_CUDA(ctx, cudaMemcpyAsync(ndev.p, &nh, sizeof(srd::AggDev), cudaMemcpyHostToDevice, ctx->stream));
     const int grid = std::min(grid_for((int64_t)a->host.cap + 1, 256), ctx->num_sms * 16);
@@ -1362,12 +1368,8 @@ static int32_t agg_grow(sr_agg* a, uint64_t new_cap) {
     SR_LAUNCH_CHECK(ctx);
     SR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     std::swap(a->hkeys, nk);
-    std::swap(a->cnt_star, nc);
-    for (int f = 0; f < SR_MAX_AGG_FNS; f++) {
-        std::swap(a->acc0[f], n0[f]);
-        std::swap(a->acc1[f], n1[f]);
-        std::swap(a->accn[f], nn[f]);
-    }
+    std::swap(a->slab, nslab);
+    for (DevBuf& b : a->late_accn) b.release(); // the new slab has every accn
     a->host = nh;
     return agg_upload(a);
 }
@@ -1390,6 +1392,22 @@ static bool staged_slot_nullable(void* user, int32_t slot) {
     return k >= 0 && st->cols[k].nulls != nullptr;
 }
 
+// start counting the non-NULL inputs of function f, whose inputs were all non-NULL so far: accn := cnt_star.  The array
+// lies outside the slab, so shared-memory accumulation (sized for the slab's layout) stops.
+static int32_t agg_start_track_n(sr_agg* a, int f) {
+    sr_ctx* ctx = a->ctx;
+    srd::AggFnDev& fn = a->host.fns[f];
+    const uint64_t slots = srd::agg_slots(a->host);
+    SR_TRY(a->late_accn[f].reserve(ctx, sizeof(int64_t) * slots));
+    srd::k_copy_i64<<<std::min(grid_for((int64_t)slots, 256), ctx->num_sms * 8), 256, 0, ctx->stream>>>(a->late_accn[f].as<long long>(), a->host.cnt_star,
+                                                                                                      (int64_t)slots);
+    SR_LAUNCH_CHECK(ctx);
+    fn.accn = a->late_accn[f].as<long long>();
+    fn.track_n = 1;
+    a->smem_bytes = 0;
+    return agg_upload(a);
+}
+
 static int32_t agg_check_nullability(sr_agg* a, const VTab& vt) {
     // a column that was non-nullable at compile time must stay so (its null-tracking state was elided)
     const srd::AggDev& h = a->host;
@@ -1401,17 +1419,7 @@ static int32_t agg_check_nullability(sr_agg* a, const VTab& vt) {
         if (fn.mode == srd::M_COUNT_STAR || fn.mode == srd::M_COUNT || fn.track_n) continue;
         for (int k = 0; k < fn.input.num_nodes; k++)
             if ((fn.input.nodes[k].op == srd::C_LOAD_I || fn.input.nodes[k].op == srd::C_LOAD_D) && vt.v[fn.input.nodes[k].arg].nulls) {
-                // start tracking the non-null count: accn := cnt_star so far
-                srd::AggFnDev& hf = a->host.fns[f];
-                const uint64_t total = (!h.dense && h.num_keys > 0) ? h.cap + 1 : h.cap;
-                SR_TRY(a->accn[f].reserve(a->ctx, sizeof(int64_t) * total));
-                srd::k_copy_i64<<<std::min(grid_for((int64_t)total, 256), a->ctx->num_sms * 8), 256, 0, a->ctx->stream>>>(
-                        a->accn[f].as<long long>(), a->host.cnt_star, (int64_t)total);
-                SR_LAUNCH_CHECK(a->ctx);
-                hf.accn = a->accn[f].as<long long>();
-                hf.track_n = 1;
-                a->smem_bytes = 0; // layout changed; fall back to global accumulation
-                SR_TRY(agg_upload(a));
+                SR_TRY(agg_start_track_n(a, f));
                 break;
             }
     }
@@ -1507,7 +1515,7 @@ static int32_t agg_finish_output(sr_agg* a) {
         SR_TRY(agg_compile(a, Tf::f, Tf::n, (void*)&a->desc));
     }
     const srd::AggDev& h = a->host;
-    const uint64_t total = (!h.dense && h.num_keys > 0) ? h.cap + 1 : h.cap;
+    const uint64_t total = srd::agg_slots(h);
     if (a->has_distinct && !a->distinct_folded) {
         for (int f = 0; f < d.num_fns; f++) {
             sr_agg* c = a->distinct[f];

@@ -363,36 +363,12 @@ __global__ void __launch_bounds__(1024) k_aggp_tiles(const uint32_t* __restrict_
 
 // ---- apply ----------------------------------------------------------------------------------------------------------
 // bytes of table state one group slot owns (keys + COUNT(*) + every accumulator array)
-__host__ __device__ inline size_t agg_slot_bytes_of(const AggDev& h) {
-    size_t b = 8 * (h.wide ? 2 : 1) + 8;
-    for (int f = 0; f < h.num_fns; f++) {
-        if (h.fns[f].mode == M_COUNT_STAR) continue;
-        b += 8 + (h.fns[f].mode == M_SUM_I128 ? 8 : 0) + (h.fns[f].track_n ? 8 : 0);
-    }
-    return b;
-}
+inline size_t agg_slot_bytes_of(const AggDev& h) { return 8 * ((h.wide ? 2 : 1) + agg_state_words(h)); }
 
-// shared-memory image of a bucket's slices: [keys | cnt | per fn: acc0, acc1?, accn?], S slots each
+// shared-memory image of a bucket's slices: the keys, then the state arrays (acc_ptrs_at), S slots each
 __device__ __forceinline__ void aggp_slice_ptrs(const AggDev& a, unsigned char* smem, int S, unsigned long long*& keys, AccPtrs& p) {
     keys = (unsigned long long*)smem;
-    long long* q = (long long*)(keys + (size_t)S * (a.wide ? 2 : 1));
-    p.cnt = q;
-    q += S;
-    for (int f = 0; f < SR_MAX_AGG_FNS; f++) {
-        p.acc0[f] = p.acc1[f] = p.accn[f] = nullptr;
-        if (f < a.num_fns && a.fns[f].mode != M_COUNT_STAR) {
-            p.acc0[f] = q;
-            q += S;
-            if (a.fns[f].mode == M_SUM_I128) {
-                p.acc1[f] = q;
-                q += S;
-            }
-            if (a.fns[f].track_n) {
-                p.accn[f] = q;
-                q += S;
-            }
-        }
-    }
+    acc_ptrs_at(a, (long long*)(keys + (size_t)S * (a.wide ? 2 : 1)), S, p);
 }
 
 struct ApplyArgs {
@@ -478,14 +454,7 @@ __global__ void __launch_bounds__(AGGP_APPLY_BLOCK, 4) k_aggp_apply(const AggDev
         if (tid == 0) s_fail = 0;
         if (aa.fresh) {
             for (int i = tid; i < S * kw; i += AGGP_APPLY_BLOCK) s_keys[i] = SR_AGG_EMPTY;
-            for (int i = tid; i < S; i += AGGP_APPLY_BLOCK) {
-                sp.cnt[i] = 0;
-                for (int f = 0; f < a.num_fns; f++) {
-                    if (sp.acc0[f]) sp.acc0[f][i] = acc_init_value(a.fns[f].mode);
-                    if (sp.acc1[f]) sp.acc1[f][i] = 0;
-                    if (sp.accn[f]) sp.accn[f][i] = 0;
-                }
-            }
+            for (int i = tid; i < S; i += AGGP_APPLY_BLOCK) acc_init_slot(a, sp, i);
         } else {
             for (int i = tid; i < S * kw; i += AGGP_APPLY_BLOCK) s_keys[i] = a.hkeys[g0 * kw + i];
             for (int i = tid; i < S; i += AGGP_APPLY_BLOCK) sp.cnt[i] = a.cnt_star[g0 + i];

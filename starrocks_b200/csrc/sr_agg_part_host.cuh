@@ -140,7 +140,7 @@ static int32_t agg_push_partitioned(sr_agg* a, const VTab& vt, int64_t n, bool f
             }
         }
         // bucket = the slices one apply CTA loads: as many (power of two, <= 8) as fit 48 KB (four CTAs per SM)
-        const size_t slot_bytes = agg_slot_bytes(h);
+        const size_t slot_bytes = srd::agg_slot_bytes_of(h);
         int nw = srd::AGGP_MAX_APPLY_SLICES;
         while (nw > 1 && ((size_t)nw << srd::AGGP_SLICE_LOG2) * slot_bytes > 48 * 1024) nw >>= 1;
         int log2nw = 0;

@@ -272,7 +272,12 @@ static int32_t frag_plan_final_dense(sr_fragment* f) {
         if (!is_key) return SR_OK;
     }
     // aggregate functions
-    int32_t off = (int32_t)ah.cap; // shared-memory layout of acc_ptrs_smem: [cnt | acc0 per function]
+    int32_t acc0_off[SR_MAX_AGG_FNS] = {}; // shared-memory image of the push kernels: the state arrays, cap slots each
+    int32_t off = 0;
+    srd::agg_state_arrays(ah, [&](int q, srd::AccWord w) {
+        if (w == srd::W_ACC0) acc0_off[q] = off;
+        off += (int32_t)ah.cap;
+    });
     for (int q = 0; q < ah.num_fns; q++) {
         const srd::AggFnDev& fn = ah.fns[q];
         if (fn.mode == srd::M_COUNT_STAR) continue;
@@ -284,8 +289,7 @@ static int32_t frag_plan_final_dense(sr_fragment* f) {
         srd::FinalDense::Fn& d = fp.fn[fp.num_fns++];
         d.mode = fn.mode;
         d.val = fn.mode == srd::M_COUNT ? -1 : val_of(id);
-        d.smem_off = off;
-        off += (int32_t)ah.cap;
+        d.smem_off = acc0_off[q];
     }
     // joins the final pass handles
     int look_join[srd::FINAL_MAX_LOOK] = {};

@@ -265,7 +265,7 @@ __global__ void __launch_bounds__(FRAG_BLOCK, 2) k_fragment(const FragDev* __res
     smem_stage_bitmaps<false>(smem, fd.joins, S);
     AccPtrs acc;
     if (SMEM_AGG) {
-        acc_ptrs_smem(ad, (long long*)smem, acc);
+        acc_ptrs_at(ad, (long long*)smem, ad.cap, acc);
         acc_smem_init(ad, acc);
     } else {
         acc_ptrs_global(ad, acc);

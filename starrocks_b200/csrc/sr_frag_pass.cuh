@@ -573,7 +573,7 @@ __global__ void __launch_bounds__(GATHER_BLOCK, GATHER_AGG_MIN_BLOCKS) k_frag_ga
     smem_copy(s_joins, fd.joins, S);
     AccPtrs acc;
     if (SMEM_AGG) {
-        acc_ptrs_smem(ad, (long long*)smem, acc);
+        acc_ptrs_at(ad, (long long*)smem, ad.cap, acc);
         acc_smem_init(ad, acc);
     } else {
         acc_ptrs_global(ad, acc);

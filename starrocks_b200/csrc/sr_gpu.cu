@@ -893,49 +893,8 @@ static int32_t agg_reset_impl(sr_agg* a) {
     for (sr_agg* c : a->distinct)
         if (c) SR_TRY(agg_reset_impl(c));
     if (!a->compiled) return SR_OK;
-    srd::AggDev& h = a->host;
-    const bool hash = !h.dense && h.num_keys > 0;
-    const uint64_t total = hash ? h.cap + 1 : h.cap;
-    const int grid = std::min(grid_for((int64_t)total, 256), ctx->num_sms * 8);
-    if (hash) {
-        srd::k_fill_u64<<<grid, 256, 0, ctx->stream>>>(a->hkeys.as<unsigned long long>(), (int64_t)(total * (h.wide ? 2 : 1)), SR_AGG_EMPTY);
-        SR_LAUNCH_CHECK(ctx);
-    }
     SR_CUDA(ctx, cudaMemsetAsync(a->counters.p, 0, 64, ctx->stream));
-    if (!hash) {
-        // dense tables live in one slab (agg_alloc_tables): when every array follows the previous one and starts from
-        // zero, the whole reset is ONE memset (the per-step reset of the fused fragment's 175-slot table was 4 launches)
-        long long* end = h.cnt_star + total;
-        bool one = true;
-        for (int f = 0; f < h.num_fns && one; f++) {
-            const srd::AggFnDev& fn = h.fns[f];
-            for (long long* p : {fn.acc0, fn.acc1, fn.accn}) {
-                if (!p) continue;
-                if (p != end || (p == fn.acc0 && srd::acc_init_value(fn.mode) != 0)) one = false;
-                end = p + total;
-            }
-        }
-        if (one) {
-            SR_CUDA(ctx, cudaMemsetAsync(h.cnt_star, 0, sizeof(int64_t) * (size_t)(end - h.cnt_star), ctx->stream));
-            return SR_OK;
-        }
-    }
-    SR_CUDA(ctx, cudaMemsetAsync(h.cnt_star, 0, sizeof(int64_t) * total, ctx->stream));
-    for (int f = 0; f < h.num_fns; f++) {
-        const srd::AggFnDev& fn = h.fns[f];
-        if (fn.acc0) {
-            const long long init = srd::acc_init_value(fn.mode);
-            if (init == 0) {
-                SR_CUDA(ctx, cudaMemsetAsync(fn.acc0, 0, sizeof(int64_t) * total, ctx->stream));
-            } else {
-                srd::k_fill_i64<<<grid, 256, 0, ctx->stream>>>(fn.acc0, (int64_t)total, init);
-                SR_LAUNCH_CHECK(ctx);
-            }
-        }
-        if (fn.acc1) SR_CUDA(ctx, cudaMemsetAsync(fn.acc1, 0, sizeof(int64_t) * total, ctx->stream));
-        if (fn.accn) SR_CUDA(ctx, cudaMemsetAsync(fn.accn, 0, sizeof(int64_t) * total, ctx->stream));
-    }
-    return SR_OK;
+    return agg_init_tables(ctx, a->host);
 }
 
 int32_t sr_agg_reset(sr_agg* a) {
@@ -954,38 +913,36 @@ int32_t sr_agg_dense_state(sr_agg* a, sr_agg_state_array* arrays, int32_t max_ar
     if (!a->compiled) return sr_fail(ctx, SR_ERR_STATE, "dense state requested before any input was pushed");
     const srd::AggDev& h = a->host;
     if (!h.dense && h.num_keys > 0) return sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "hash aggregate tables have no element-wise mergeable layout");
-    int n = 0;
-    auto add = [&](void* p, int32_t type, int32_t reduce) {
-        if (n < max_arrays) arrays[n] = sr_agg_state_array{p, (int64_t)h.cap, type, reduce};
-        n++;
-    };
-    add(h.cnt_star, SR_TYPE_BIGINT, SR_STATE_SUM);
-    for (int f = 0; f < h.num_fns; f++) {
-        const srd::AggFnDev& fn = h.fns[f];
-        switch (fn.mode) {
-        case srd::M_COUNT_STAR:
-            break; // cnt_star itself
-        case srd::M_COUNT:
-        case srd::M_SUM_I64:
-            add(fn.acc0, SR_TYPE_BIGINT, SR_STATE_SUM);
-            break;
-        case srd::M_SUM_F64:
-        case srd::M_AVG:
-            add(fn.acc0, SR_TYPE_DOUBLE, SR_STATE_SUM);
-            break;
-        case srd::M_MIN_I64:
-        case srd::M_MIN_F64: // doubles are kept as their order-preserving int64 image
-            add(fn.acc0, SR_TYPE_BIGINT, SR_STATE_MIN);
-            break;
-        case srd::M_MAX_I64:
-        case srd::M_MAX_F64:
-            add(fn.acc0, SR_TYPE_BIGINT, SR_STATE_MAX);
-            break;
-        default:
-            return sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "aggregate function %d keeps a state that is not element-wise mergeable", f);
+    srd::AccPtrs p;
+    srd::acc_ptrs_global(h, p);
+    int n = 0, unmergeable = -1;
+    srd::agg_state_arrays(h, [&](int f, srd::AccWord w) {
+        int32_t type = SR_TYPE_BIGINT, reduce = SR_STATE_SUM; // the counters and accn
+        if (w == srd::W_ACC0) {
+            switch (h.fns[f].mode) {
+            case srd::M_SUM_F64:
+            case srd::M_AVG:
+                type = SR_TYPE_DOUBLE;
+                break;
+            case srd::M_MIN_I64:
+            case srd::M_MIN_F64: // doubles are kept as their order-preserving int64 image
+                reduce = SR_STATE_MIN;
+                break;
+            case srd::M_MAX_I64:
+            case srd::M_MAX_F64:
+                reduce = SR_STATE_MAX;
+                break;
+            case srd::M_SUM_I128:
+                if (unmergeable < 0) unmergeable = f;
+                break;
+            default: // M_COUNT, M_SUM_I64
+                break;
+            }
         }
-        if (fn.accn) add(fn.accn, SR_TYPE_BIGINT, SR_STATE_SUM);
-    }
+        if (n < max_arrays) arrays[n] = sr_agg_state_array{srd::acc_ptr(p, f, w), (int64_t)h.cap, type, reduce};
+        n++;
+    });
+    if (unmergeable >= 0) return sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "aggregate function %d keeps a state that is not element-wise mergeable", unmergeable);
     if (n > max_arrays) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "%d state arrays, room for %d", n, max_arrays);
     *num_arrays = n;
     return SR_OK;
@@ -1212,42 +1169,23 @@ int32_t sr_agg_merge(sr_agg* a, sr_agg* o) {
     if (desc_has_distinct(&a->desc)) return sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "COUNT(DISTINCT) states do not merge; shuffle on the group keys instead");
     if (!o->compiled) return SR_OK; // nothing was pushed into `other`
     if (memcmp(&a->desc, &o->desc, sizeof(sr_agg_desc)) != 0) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "merge needs identical descriptors");
-    if (!a->compiled) {
-        // adopt other's compiled layout with fresh tables
+    if (!a->compiled) { // adopt other's compiled layout with fresh tables
         a->reg = o->reg;
         a->host = o->host;
-        for (int f = 0; f < a->host.num_fns; f++) a->host.fns[f].track_n = o->host.fns[f].track_n;
-        SR_TRY(a->counters.reserve(ctx, 64));
-        SR_CUDA(ctx, cudaMemsetAsync(a->counters.p, 0, 64, ctx->stream));
-        a->host.ngroups = a->counters.as<unsigned long long>();
-        a->host.flags = (int32_t*)(a->counters.as<unsigned long long>() + 1);
-        SR_TRY(agg_alloc_tables(a, &a->host, o->host.cap, &a->hkeys, &a->cnt_star, a->acc0, a->acc1, a->accn));
-        a->smem_bytes = o->smem_bytes;
-        SR_TRY(agg_upload(a));
-        a->compiled = true;
+        SR_TRY(agg_setup_tables(a, o->host.cap));
     }
     const srd::AggDev& oh = o->host;
     const bool hash = !a->host.dense && a->host.num_keys > 0;
-    for (int f = 0; f < oh.num_fns; f++) {
-        if (oh.fns[f].track_n && !a->host.fns[f].track_n && a->host.fns[f].mode != srd::M_COUNT_STAR && a->host.fns[f].mode != srd::M_COUNT) {
-            const uint64_t total = hash ? a->host.cap + 1 : a->host.cap;
-            SR_TRY(a->accn[f].reserve(ctx, sizeof(int64_t) * total));
-            srd::k_copy_i64<<<std::min(grid_for((int64_t)total, 256), ctx->num_sms * 8), 256, 0, ctx->stream>>>(a->accn[f].as<long long>(),
-                                                                                                               a->host.cnt_star, (int64_t)total);
-            SR_LAUNCH_CHECK(ctx);
-            a->host.fns[f].accn = a->accn[f].as<long long>();
-            a->host.fns[f].track_n = 1;
-            a->smem_bytes = 0;
-            SR_TRY(agg_upload(a));
-        }
-    }
+    for (int f = 0; f < oh.num_fns; f++)
+        if (oh.fns[f].track_n && !a->host.fns[f].track_n && a->host.fns[f].mode != srd::M_COUNT_STAR && a->host.fns[f].mode != srd::M_COUNT)
+            SR_TRY(agg_start_track_n(a, f));
     if (hash) {
         uint64_t ng_o;
         int32_t ovf, bad;
         SR_TRY(agg_read_counters(o, &ng_o, &ovf, &bad));
         while ((uint64_t)a->ngroups_host + ng_o > a->host.limit) SR_TRY(agg_grow(a, a->host.cap * 4));
     }
-    const uint64_t total_o = (!oh.dense && oh.num_keys > 0) ? oh.cap + 1 : oh.cap;
+    const uint64_t total_o = srd::agg_slots(oh);
     a->table_touched = true;
     srd::k_agg_merge<<<std::min(grid_for((int64_t)total_o, 256), ctx->num_sms * 16), 256, 0, ctx->stream>>>((const srd::AggDev*)o->dev.p,
                                                                                                             (const srd::AggDev*)a->dev.p);
