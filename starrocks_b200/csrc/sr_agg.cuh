@@ -1040,13 +1040,12 @@ struct sr_agg {
     int64_t cursor = 0;
     DevBuf block_counts, block_offsets;
     ScanScratch scan_scratch;
-    std::vector<DevBuf> out_bufs;      // device result columns (data, nulls) x (keys + fns)
+    ColBufs out_cols;                 // device result columns: keys, then fns
     std::vector<PinnedBuf> host_bufs; // host-memory pull: page-locked, the D2H copies are plain DMA
     int32_t out_types[SR_MAX_GROUP_KEYS + SR_MAX_AGG_FNS];
-    bool out_has_nulls[SR_MAX_GROUP_KEYS + SR_MAX_AGG_FNS];
-    std::vector<DevBuf> conv_bufs; // sr_agg_convert_to_states: (data, nulls) per function
+    ColBufs conv_cols; // sr_agg_convert_to_states: one column per function
     DevBuf sel_flags, sel_pos, sel_index, sel_tmp; // sr_agg_push_selective: streaming selection, its prefix sums, the streamed rows
-    std::vector<DevBuf> sel_bufs;                  //   compacted (data, nulls) per output column
+    ColBufs sel_cols;                              //   the compacted output columns
     // COUNT(DISTINCT) functions: one (group keys, value) set each -- an aggregate of its own with no functions, fed the
     // same chunks; agg_finish_output folds it into acc0 of the function (which until then holds COUNT(value))
     sr_agg* distinct[SR_MAX_AGG_FNS] = {};
@@ -1534,24 +1533,17 @@ static int32_t agg_finish_output(sr_agg* a) {
     SR_TRY(a->block_offsets.reserve(ctx, sizeof(uint64_t) * (size_t)blocks));
     srd::k_agg_count<<<blocks, srd::EMIT_BLOCK, 0, ctx->stream>>>((const srd::AggDev*)a->dev.p, total, a->block_counts.as<uint32_t>());
     SR_LAUNCH_CHECK(ctx);
-    SR_TRY(scan_counts(ctx, &a->scan_scratch, a->block_counts.as<uint32_t>(), blocks, a->block_offsets.as<uint64_t>()));
-    // one read-back, one synchronisation: the row count and the table's status counters together
-    SR_CUDA(ctx, cudaMemcpyAsync(ctx->pinned, ctx->dscratch, sizeof(uint64_t), cudaMemcpyDeviceToHost, ctx->stream));
+    // one synchronisation: the table's status counters are read back with the row count
     SR_CUDA(ctx, cudaMemcpyAsync(ctx->pinned + 8, a->counters.p, 16, cudaMemcpyDeviceToHost, ctx->stream));
-    SR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    int64_t rows = 0;
+    SR_TRY(scan_counts(ctx, &a->scan_scratch, a->block_counts.as<uint32_t>(), blocks, a->block_offsets.as<uint64_t>(), &rows));
     {
         const int32_t* fl = (const int32_t*)(ctx->pinned + 9);
         if (fl[1]) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "a group-by value fell outside the declared group_min/group_max range");
         if (fl[0]) return sr_fail(ctx, SR_ERR_STATE, "aggregate hash table overflow (internal)");
     }
-    const int64_t rows = (int64_t)ctx->pinned[0];
     const int nc = d.num_group_keys + d.num_fns;
-    // output buffers are kept across finish/reset cycles (they only grow): a repeated query pays no cudaMalloc/cudaFree
-    if (a->out_bufs.size() < 2 * (size_t)nc) {
-        std::vector<DevBuf> nb(2 * (size_t)nc);
-        for (size_t i = 0; i < a->out_bufs.size(); i++) std::swap(nb[i], a->out_bufs[i]);
-        a->out_bufs.swap(nb);
-    }
+    a->out_cols.resize(nc); // kept across finish/reset cycles: a repeated query pays no cudaMalloc/cudaFree
     srd::EmitArgs ea;
     memset(&ea, 0, sizeof(ea));
     for (int k = 0; k < nc; k++) {
@@ -1565,20 +1557,15 @@ static int32_t agg_finish_output(sr_agg* a) {
             type = fn.result_type;
             nullable = !(fn.mode == srd::M_COUNT || fn.mode == srd::M_COUNT_STAR);
         }
-        const int w = srd::type_width(type);
-        SR_TRY(a->out_bufs[2 * k].reserve(ctx, (size_t)std::max<int64_t>(rows, 1) * w));
-        if (nullable) SR_TRY(a->out_bufs[2 * k + 1].reserve(ctx, (size_t)std::max<int64_t>(rows, 1)));
         srd::EmitCol ec;
-        ec.data = a->out_bufs[2 * k].p;
-        ec.nulls = nullable ? (uint8_t*)a->out_bufs[2 * k + 1].p : nullptr;
         ec.type = type;
-        ec.width = w;
+        ec.width = srd::type_width(type);
+        SR_TRY(a->out_cols.reserve(ctx, k, rows, ec.width, nullable, &ec.data, &ec.nulls));
         if (k < d.num_group_keys)
             ea.keys[k] = ec;
         else
             ea.res[k - d.num_group_keys] = ec;
         a->out_types[k] = type;
-        a->out_has_nulls[k] = nullable;
     }
     if (rows > 0) {
         srd::k_agg_emit<<<blocks, srd::EMIT_BLOCK, 0, ctx->stream>>>((const srd::AggDev*)a->dev.p, total, a->block_offsets.as<uint64_t>(), ea);

@@ -23,6 +23,17 @@ struct DCol {
     int32_t width;
 };
 
+// one column of k_gather (sr_scan.cuh)
+struct GatherCol {
+    const void* src;
+    const uint8_t* src_nulls;
+    void* dst;
+    uint8_t* dst_nulls;
+    int32_t width;
+    int32_t zero_is_null; // build side of an outer join
+    int32_t vec16;        // width 16 with src and dst 16-byte aligned: one int4 per value (set by launch_gather)
+};
+
 __host__ __device__ inline int type_width(int32_t t) {
     switch (t) {
     case SR_TYPE_BOOLEAN:

@@ -156,7 +156,7 @@ struct sr_xchg {
     Staged staged;
     DevBuf hash_values, channel_ids, counts, offsets, row_index;
     ScanScratch scan_scratch;
-    std::vector<DevBuf> out_bufs;
+    ColBufs out_cols;
 };
 
 // ---------------------------------------------------------------------------------------
@@ -376,32 +376,21 @@ int32_t sr_scan_filter(sr_scan* s, const sr_chunk_view* in, sr_chunk_out* out) {
     int64_t total = 0;
     SR_TRY(scan_select(s, in, true, &total));
     const int nout = (int)s->out_slots.size();
-    if ((int)s->out_bufs.size() < 2 * nout) {
-        std::vector<DevBuf> nb(2 * nout);
-        for (size_t i = 0; i < s->out_bufs.size(); i++) std::swap(nb[i], s->out_bufs[i]);
-        s->out_bufs.swap(nb);
-    }
+    s->out_cols.resize(nout);
     srd::CompactArgs ca;
     ca.n = 0;
-    out->num_cols = nout;
-    out->mem = SR_MEM_DEVICE;
-    out->num_rows = total;
+    ColBufs::header(out, nout, total);
     for (int k = 0; k < nout; k++) {
         const int c = s->staged.find(s->out_slots[k]);
         if (c < 0) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "chunk misses output slot %d", s->out_slots[k]);
         const srd::DCol& dc = s->staged.cols[c];
-        SR_TRY(s->out_bufs[2 * k].reserve(ctx, (size_t)std::max<int64_t>(total, 1) * dc.width));
-        const int32_t vec16 = dc.width == 16 && (((uintptr_t)dc.data | (uintptr_t)s->out_bufs[2 * k].p) & 15) == 0 ? 1 : 0;
-        ca.c[ca.n++] = srd::CompactCol{dc.data, s->out_bufs[2 * k].p, dc.width, vec16};
-        out->cols[k].data = s->out_bufs[2 * k].p;
-        out->cols[k].nulls = nullptr;
-        out->cols[k].type = dc.type;
-        out->cols[k].slot_id = s->out_slots[k];
-        if (dc.nulls) {
-            SR_TRY(s->out_bufs[2 * k + 1].reserve(ctx, (size_t)std::max<int64_t>(total, 1)));
-            ca.c[ca.n++] = srd::CompactCol{dc.nulls, s->out_bufs[2 * k + 1].p, 1, 0};
-            out->cols[k].nulls = (uint8_t*)s->out_bufs[2 * k + 1].p;
-        }
+        void* data;
+        uint8_t* nulls;
+        SR_TRY(s->out_cols.reserve(ctx, k, total, dc.width, dc.nulls != nullptr, &data, &nulls));
+        const int32_t vec16 = dc.width == 16 && (((uintptr_t)dc.data | (uintptr_t)data) & 15) == 0 ? 1 : 0;
+        ca.c[ca.n++] = srd::CompactCol{dc.data, data, dc.width, vec16};
+        if (nulls) ca.c[ca.n++] = srd::CompactCol{dc.nulls, nulls, 1, 0};
+        s->out_cols.fill(out, k, dc.type, s->out_slots[k]);
     }
     if (total > 0 && ca.n > 0) {
         const int64_t tiles = (in->num_rows + srd::SCANW_TILE - 1) / srd::SCANW_TILE;
@@ -861,8 +850,9 @@ int32_t sr_agg_pull(sr_agg* a, int64_t max_rows, int32_t out_mem, sr_chunk_out* 
         out->cols[k].data = nullptr;
         out->cols[k].nulls = nullptr;
         if (n <= 0) continue;
-        const uint8_t* ddata = (const uint8_t*)a->out_bufs[2 * k].p + (size_t)a->cursor * w;
-        const uint8_t* dnull = a->out_has_nulls[k] ? (const uint8_t*)a->out_bufs[2 * k + 1].p + a->cursor : nullptr;
+        const ColBufs::Col& oc = a->out_cols.cols[k];
+        const uint8_t* ddata = (const uint8_t*)oc.data.p + (size_t)a->cursor * w;
+        const uint8_t* dnull = oc.nullable ? (const uint8_t*)oc.nulls.p + a->cursor : nullptr;
         if (out_mem == SR_MEM_DEVICE) {
             out->cols[k].data = (void*)ddata;
             out->cols[k].nulls = (uint8_t*)dnull;
@@ -1046,14 +1036,8 @@ static int32_t agg_convert_impl(sr_agg* a, const sr_chunk_view* chunk, sr_chunk_
     if (vt_out) *vt_out = vt;
     const int64_t n = chunk->num_rows;
     const srd::AggDev& h = a->host;
-    if (a->conv_bufs.size() < 2 * (size_t)SR_MAX_AGG_FNS) {
-        std::vector<DevBuf> nb(2 * (size_t)SR_MAX_AGG_FNS);
-        for (size_t i = 0; i < a->conv_bufs.size(); i++) std::swap(nb[i], a->conv_bufs[i]);
-        a->conv_bufs.swap(nb);
-    }
-    out->num_cols = d.num_group_keys + d.num_fns;
-    out->mem = SR_MEM_DEVICE;
-    out->num_rows = n;
+    a->conv_cols.resize(d.num_fns);
+    ColBufs::header(out, d.num_group_keys + d.num_fns, n);
     for (int k = 0; k < d.num_group_keys; k++) { // group-by columns travel as they are (device copies of the staged input)
         const int c = a->staged.find(d.group_slots[k]);
         if (c < 0) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "chunk misses group slot %d", d.group_slots[k]);
@@ -1070,14 +1054,11 @@ static int32_t agg_convert_impl(sr_agg* a, const sr_chunk_view* chunk, sr_chunk_
         const int w = srd::type_width(type);
         if (w > 8) return sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "fn %d: 128-bit states in the intermediate format", f);
         const bool nullable = !(fn.mode == srd::M_COUNT || fn.mode == srd::M_COUNT_STAR);
-        SR_TRY(a->conv_bufs[2 * f].reserve(ctx, (size_t)std::max<int64_t>(n, 1) * w));
-        if (nullable) SR_TRY(a->conv_bufs[2 * f + 1].reserve(ctx, (size_t)std::max<int64_t>(n, 1)));
-        ca.c[f] = srd::ConvertCol{a->conv_bufs[2 * f].p, nullable ? (uint8_t*)a->conv_bufs[2 * f + 1].p : nullptr, w, type};
-        sr_col_out& oc = out->cols[d.num_group_keys + f];
-        oc.data = ca.c[f].data;
-        oc.nulls = ca.c[f].nulls;
-        oc.type = type;
-        oc.slot_id = d.fns[f].out_slot;
+        void* data;
+        uint8_t* nulls;
+        SR_TRY(a->conv_cols.reserve(ctx, f, n, w, nullable, &data, &nulls));
+        ca.c[f] = srd::ConvertCol{data, nulls, w, type};
+        out->cols[d.num_group_keys + f] = sr_col_out{data, nulls, type, d.fns[f].out_slot};
     }
     if (n > 0 && d.num_fns > 0) {
         srd::k_agg_convert_states<<<std::min(grid_for(n, 256), ctx->num_sms * 8), 256, 0, ctx->stream>>>((const srd::AggDev*)a->dev.p, vt, n, ca);
@@ -1134,26 +1115,13 @@ int32_t sr_agg_push_selective(sr_agg* a, const sr_chunk_view* chunk, sr_chunk_ou
     srd::k_selection_index<<<std::min(grid_for(n, 256), ctx->num_sms * 8), 256, 0, ctx->stream>>>(a->sel_flags.as<uint8_t>(), a->sel_pos.as<uint32_t>(), n,
                                                                                                  a->sel_index.as<uint32_t>());
     SR_LAUNCH_CHECK(ctx);
-    if (a->sel_bufs.size() < 2 * (size_t)out->num_cols) {
-        std::vector<DevBuf> nb(2 * (size_t)out->num_cols);
-        for (size_t i = 0; i < a->sel_bufs.size(); i++) std::swap(nb[i], a->sel_bufs[i]);
-        a->sel_bufs.swap(nb);
-    }
+    a->sel_cols.resize(out->num_cols);
     srd::GatherArgs ga;
-    ga.n = 0;
+    ga.n = out->num_cols;
     for (int k = 0; k < out->num_cols; k++) {
-        srd::GatherCol g;
-        g.src = out->cols[k].data;
-        g.src_nulls = out->cols[k].nulls;
-        g.width = srd::type_width(out->cols[k].type);
-        g.zero_is_null = 0;
-        SR_TRY(a->sel_bufs[2 * k].reserve(ctx, (size_t)m * g.width));
-        if (g.src_nulls) SR_TRY(a->sel_bufs[2 * k + 1].reserve(ctx, (size_t)m));
-        g.dst = a->sel_bufs[2 * k].p;
-        g.dst_nulls = g.src_nulls ? (uint8_t*)a->sel_bufs[2 * k + 1].p : nullptr;
-        out->cols[k].data = g.dst;
-        out->cols[k].nulls = g.dst_nulls;
-        ga.c[ga.n++] = g;
+        sr_col_out& oc = out->cols[k];
+        SR_TRY(a->sel_cols.gather(ctx, k, m, oc.data, oc.nulls, srd::type_width(oc.type), false, &ga.c[k]));
+        a->sel_cols.fill(out, k, oc.type, oc.slot_id);
     }
     SR_TRY(launch_gather(ctx, a->sel_index.as<uint32_t>(), m, ga));
     if (chunk->mem != SR_MEM_DEVICE) SR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
@@ -1407,21 +1375,16 @@ int32_t sr_xchg_partition(sr_xchg* x, const sr_chunk_view* in, sr_chunk_out* out
     SR_TRY(xchg_part_cols(x, &pc));
     const int64_t n = in->num_rows;
     const int nch = x->desc.num_channels;
-    out->num_cols = in->num_cols;
-    out->mem = SR_MEM_DEVICE;
-    out->num_rows = n;
-    if ((int)x->out_bufs.size() < 2 * in->num_cols) {
-        std::vector<DevBuf> nb(2 * in->num_cols);
-        for (size_t i = 0; i < x->out_bufs.size(); i++) std::swap(nb[i], x->out_bufs[i]);
-        x->out_bufs.swap(nb);
-    }
-    if (n <= 0) { // zero rows of every column; a nullable column keeps a (zero-row) null column
+    ColBufs::header(out, in->num_cols, n);
+    x->out_cols.resize(in->num_cols);
+    if (n <= 0) { // zero rows of every column, with no data buffer; a nullable column keeps a (zero-row) null column
         for (int c = 0; c <= nch; c++) channel_offsets_host[c] = 0;
         for (int k = 0; k < in->num_cols; k++) {
             uint8_t* nulls = nullptr;
             if (in->cols[k].nulls) {
-                SR_TRY(x->out_bufs[2 * k + 1].reserve(ctx, 16));
-                nulls = (uint8_t*)x->out_bufs[2 * k + 1].p;
+                DevBuf& nb = x->out_cols.cols[k].nulls;
+                SR_TRY(nb.reserve(ctx, 1));
+                nulls = (uint8_t*)nb.p;
             }
             out->cols[k] = sr_col_out{nullptr, nulls, in->cols[k].type, in->cols[k].slot_id};
         }
@@ -1444,23 +1407,11 @@ int32_t sr_xchg_partition(sr_xchg* x, const sr_chunk_view* in, sr_chunk_out* out
     SR_CUDA(ctx, cudaMemcpy2DAsync(starts.data(), sizeof(uint64_t), x->offsets.p, sizeof(uint64_t) * (size_t)tiles, sizeof(uint64_t), nch,
                                    cudaMemcpyDeviceToHost, ctx->stream));
     srd::GatherArgs ga;
-    ga.n = 0;
+    ga.n = in->num_cols;
     for (int k = 0; k < in->num_cols; k++) {
         const srd::DCol& dc = x->staged.cols[k];
-        SR_TRY(x->out_bufs[2 * k].reserve(ctx, (size_t)n * dc.width));
-        srd::GatherCol g;
-        g.src = dc.data;
-        g.src_nulls = dc.nulls;
-        g.dst = x->out_bufs[2 * k].p;
-        g.dst_nulls = nullptr;
-        g.width = dc.width;
-        g.zero_is_null = 0;
-        if (dc.nulls) {
-            SR_TRY(x->out_bufs[2 * k + 1].reserve(ctx, (size_t)n));
-            g.dst_nulls = (uint8_t*)x->out_bufs[2 * k + 1].p;
-        }
-        ga.c[ga.n++] = g;
-        out->cols[k] = sr_col_out{g.dst, g.dst_nulls, dc.type, x->staged.slots[k]};
+        SR_TRY(x->out_cols.gather(ctx, k, n, dc.data, dc.nulls, dc.width, false, &ga.c[k]));
+        x->out_cols.fill(out, k, dc.type, x->staged.slots[k]);
     }
     SR_TRY(launch_gather(ctx, x->row_index.as<uint32_t>(), n, ga));
     SR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));

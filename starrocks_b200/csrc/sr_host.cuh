@@ -192,6 +192,51 @@ struct DevBuf {
     }
 };
 
+// The device columns one handle stages or hands back in an sr_chunk_out: a (data, nulls) pair of grow-only buffers per
+// column, kept across calls so that a repeated call pays no cudaMalloc.  What a call hands back stays valid until the
+// next call on the handle (include/sr_gpu_ops.h).
+struct ColBufs {
+    struct Col {
+        DevBuf data, nulls;
+        bool nullable = false; // the last reserve gave the column a null column
+    };
+    std::vector<Col> cols;
+    void resize(int num_cols) {
+        if (cols.size() < (size_t)num_cols) cols.resize(num_cols);
+    }
+    // column k for `rows` values of `width` bytes, plus one null byte per row when `nullable` (*nulls is NULL
+    // otherwise); a column of zero rows still gets the buffers of one row
+    int32_t reserve(sr_ctx* ctx, int k, int64_t rows, int width, bool nullable, void** data, uint8_t** nulls) {
+        Col& c = cols[k];
+        const size_t r = (size_t)std::max<int64_t>(rows, 1);
+        SR_TRY(c.data.reserve(ctx, r * width));
+        if (nullable) SR_TRY(c.nulls.reserve(ctx, r));
+        c.nullable = nullable;
+        *data = c.data.p;
+        *nulls = nullable ? (uint8_t*)c.nulls.p : nullptr;
+        return SR_OK;
+    }
+    static void header(sr_chunk_out* out, int num_cols, int64_t rows) {
+        out->num_cols = num_cols;
+        out->mem = SR_MEM_DEVICE;
+        out->num_rows = rows;
+    }
+    // out->cols[k] <- column k as the last reserve left it
+    void fill(sr_chunk_out* out, int k, int32_t type, int32_t slot) const {
+        const Col& c = cols[k];
+        out->cols[k] = sr_col_out{c.data.p, c.nullable ? (uint8_t*)c.nulls.p : nullptr, type, slot};
+    }
+    // column k reserved for `rows` gathered values of a source column; it has a null column when the source has one or
+    // index 0 means NULL (`zero_is_null`: the build side of an outer join)
+    int32_t gather(sr_ctx* ctx, int k, int64_t rows, const void* src, const uint8_t* src_nulls, int width, bool zero_is_null, srd::GatherCol* g) {
+        void* dst;
+        uint8_t* dst_nulls;
+        SR_TRY(reserve(ctx, k, rows, width, src_nulls != nullptr || zero_is_null, &dst, &dst_nulls));
+        *g = srd::GatherCol{src, src_nulls, dst, dst_nulls, width, zero_is_null ? 1 : 0, 0};
+        return SR_OK;
+    }
+};
+
 static inline const sr_col_view* find_col(const sr_chunk_view* c, int32_t slot) {
     for (int k = 0; k < c->num_cols; k++)
         if (c->cols[k].slot_id == slot) return &c->cols[k];
@@ -207,7 +252,7 @@ static inline bool col_aligned(const void* p, int width) {
 // buffers owned by `Staged`; device chunks (and pinned ones read in place) are referenced in place and must be
 // naturally aligned.
 struct Staged {
-    std::vector<DevBuf> bufs; // 2 per column (data, nulls)
+    ColBufs bufs;
     std::vector<srd::DCol> cols;
     std::vector<int32_t> slots;
     int64_t num_rows = 0;
@@ -228,11 +273,7 @@ struct Staged {
         num_rows = in->num_rows;
         if (in->mem != SR_MEM_HOST && in->mem != SR_MEM_DEVICE && in->mem != SR_MEM_HOST_PINNED)
             return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "unknown memory kind %d", in->mem);
-        if ((int)bufs.size() < 2 * in->num_cols) {
-            std::vector<DevBuf> nb(2 * in->num_cols);
-            for (size_t i = 0; i < bufs.size(); i++) std::swap(nb[i], bufs[i]);
-            bufs.swap(nb);
-        }
+        bufs.resize(in->num_cols);
         for (int k = 0; k < in->num_cols; k++) {
             const sr_col_view& c = in->cols[k];
             if (only_slots && std::find(only_slots->begin(), only_slots->end(), c.slot_id) == only_slots->end()) continue;
@@ -260,14 +301,16 @@ struct Staged {
                     d.nulls = (const uint8_t*)p;
                 }
             } else {
-                SR_TRY(bufs[2 * k].reserve(ctx, (size_t)in->num_rows * w + 16));
-                SR_CUDA(ctx, cudaMemcpyAsync(bufs[2 * k].p, c.data, (size_t)in->num_rows * w, cudaMemcpyHostToDevice, ctx->stream));
-                d.data = bufs[2 * k].p;
+                DevBuf& data = bufs.cols[k].data;
+                DevBuf& nulls = bufs.cols[k].nulls;
+                SR_TRY(data.reserve(ctx, (size_t)in->num_rows * w + 16));
+                SR_CUDA(ctx, cudaMemcpyAsync(data.p, c.data, (size_t)in->num_rows * w, cudaMemcpyHostToDevice, ctx->stream));
+                d.data = data.p;
                 d.nulls = nullptr;
                 if (c.nulls) {
-                    SR_TRY(bufs[2 * k + 1].reserve(ctx, (size_t)in->num_rows + 16));
-                    SR_CUDA(ctx, cudaMemcpyAsync(bufs[2 * k + 1].p, c.nulls, (size_t)in->num_rows, cudaMemcpyHostToDevice, ctx->stream));
-                    d.nulls = (const uint8_t*)bufs[2 * k + 1].p;
+                    SR_TRY(nulls.reserve(ctx, (size_t)in->num_rows + 16));
+                    SR_CUDA(ctx, cudaMemcpyAsync(nulls.p, c.nulls, (size_t)in->num_rows, cudaMemcpyHostToDevice, ctx->stream));
+                    d.nulls = (const uint8_t*)nulls.p;
                 }
             }
             cols.push_back(d);

@@ -619,7 +619,7 @@ struct ProberState {
     DevBuf heads, block_counts, block_offsets, probe_index, build_index;
     DevBuf conj_keep, conj_any, conj_k, conj_u, conj_tmp, conj_pi, conj_bi; // other-join conjunct: flags, their prefix sums, final pairs
     ScanScratch scan_scratch;
-    std::vector<DevBuf> out_bufs;
+    ColBufs out_cols;
     int64_t last_count = 0;
 };
 
@@ -644,7 +644,7 @@ struct sr_join {
     bool match_ready = false;
     int32_t probe_types_seen[SR_MAX_JOIN_OUT] = {}; // types of the probe_out columns, from the first probed chunk
     ScanScratch remain_scan;
-    std::vector<DevBuf> remain_bufs;
+    ColBufs remain_cols;
     Staged staged_build;
     std::vector<ProberState*> probers;
     ~sr_join() {
@@ -947,10 +947,7 @@ static int32_t join_probe_remain(sr_join* j, sr_chunk_out* out) {
         SR_TRY(j->remain_offsets.reserve(ctx, sizeof(uint64_t) * (size_t)blocks));
         srd::k_remain_count<<<blocks, srd::REMAIN_BLOCK, 0, ctx->stream>>>((const uint8_t*)j->match.p, rows, want, j->remain_counts.as<uint32_t>());
         SR_LAUNCH_CHECK(ctx);
-        SR_TRY(scan_counts(ctx, &j->remain_scan, j->remain_counts.as<uint32_t>(), blocks, j->remain_offsets.as<uint64_t>()));
-        SR_CUDA(ctx, cudaMemcpyAsync(ctx->pinned, ctx->dscratch, sizeof(uint64_t), cudaMemcpyDeviceToHost, ctx->stream));
-        SR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        total = (int64_t)ctx->pinned[0];
+        SR_TRY(scan_counts(ctx, &j->remain_scan, j->remain_counts.as<uint32_t>(), blocks, j->remain_offsets.as<uint64_t>(), &total));
     }
     SR_TRY(j->remain_index.reserve(ctx, sizeof(uint32_t) * (size_t)std::max<int64_t>(total, 1)));
     if (total > 0) {
@@ -960,59 +957,36 @@ static int32_t join_probe_remain(sr_join* j, sr_chunk_out* out) {
     }
     const int np = with_probe_cols ? j->desc.num_probe_out : 0, nb = j->desc.num_build_out;
     if (np + nb > SR_MAX_OUT_COLS) return sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "too many join output columns");
-    if ((int)j->remain_bufs.size() < 2 * (np + nb)) {
-        std::vector<DevBuf> nbv(2 * (np + nb));
-        for (size_t i = 0; i < j->remain_bufs.size(); i++) std::swap(nbv[i], j->remain_bufs[i]);
-        j->remain_bufs.swap(nbv);
-    }
-    out->num_cols = np + nb;
-    out->mem = SR_MEM_DEVICE;
-    out->num_rows = total;
+    j->remain_cols.resize(np + nb);
+    ColBufs::header(out, np + nb, total);
     srd::GatherArgs ga;
     ga.n = 0;
-    const size_t cap = (size_t)std::max<int64_t>(total, 1);
     for (int k = 0; k < np + nb; k++) {
         if (k < np) { // probe side: NULL (_probe_null_output, join_hash_map.hpp:206-232)
             const int32_t type = j->desc.probe_out_types[k] ? j->desc.probe_out_types[k] : j->probe_types_seen[k];
             const int w = srd::type_width(type);
             if (w == 0)
                 return sr_fail(ctx, SR_ERR_STATE, "type of probe output slot %d is unknown (never probed): declare it in sr_join_desc.probe_out_types", j->desc.probe_out_slots[k]);
-            SR_TRY(j->remain_bufs[2 * k].reserve(ctx, cap * w));
-            SR_TRY(j->remain_bufs[2 * k + 1].reserve(ctx, cap));
+            void* data;
+            uint8_t* nulls;
+            SR_TRY(j->remain_cols.reserve(ctx, k, total, w, true, &data, &nulls));
             if (total > 0) {
-                SR_CUDA(ctx, cudaMemsetAsync(j->remain_bufs[2 * k].p, 0, (size_t)total * w, ctx->stream));
-                SR_CUDA(ctx, cudaMemsetAsync(j->remain_bufs[2 * k + 1].p, 1, (size_t)total, ctx->stream));
+                SR_CUDA(ctx, cudaMemsetAsync(data, 0, (size_t)total * w, ctx->stream));
+                SR_CUDA(ctx, cudaMemsetAsync(nulls, 1, (size_t)total, ctx->stream));
             }
-            out->cols[k].data = j->remain_bufs[2 * k].p;
-            out->cols[k].nulls = (uint8_t*)j->remain_bufs[2 * k + 1].p;
-            out->cols[k].type = type;
-            out->cols[k].slot_id = j->desc.probe_out_slots[k];
+            j->remain_cols.fill(out, k, type, j->desc.probe_out_slots[k]);
             continue;
         }
         const int32_t slot = j->desc.build_out_slots[k - np];
         const BuildCol* bc = j->find_col(slot);
         if (!bc) {
             if (total > 0 || j->desc.build_out_types[k - np] == 0) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "build chunk misses output slot %d", slot);
-            out->cols[k].data = nullptr; // empty build side: zero rows of the declared type
-            out->cols[k].nulls = nullptr;
-            out->cols[k].type = j->desc.build_out_types[k - np];
-            out->cols[k].slot_id = slot;
+            out->cols[k] = sr_col_out{nullptr, nullptr, j->desc.build_out_types[k - np], slot}; // empty build side: zero rows of the declared type
             continue;
         }
-        srd::GatherCol g;
-        g.src = bc->data.p;
-        g.src_nulls = bc->nullable ? (const uint8_t*)bc->nulls.p : nullptr;
-        g.width = bc->width;
-        g.zero_is_null = 0;
-        SR_TRY(j->remain_bufs[2 * k].reserve(ctx, cap * g.width));
-        if (g.src_nulls) SR_TRY(j->remain_bufs[2 * k + 1].reserve(ctx, cap));
-        g.dst = j->remain_bufs[2 * k].p;
-        g.dst_nulls = g.src_nulls ? (uint8_t*)j->remain_bufs[2 * k + 1].p : nullptr;
-        out->cols[k].data = g.dst;
-        out->cols[k].nulls = g.dst_nulls;
-        out->cols[k].type = bc->type;
-        out->cols[k].slot_id = slot;
-        ga.c[ga.n++] = g;
+        const uint8_t* src_nulls = bc->nullable ? (const uint8_t*)bc->nulls.p : nullptr;
+        SR_TRY(j->remain_cols.gather(ctx, k, total, bc->data.p, src_nulls, bc->width, false, &ga.c[ga.n++]));
+        j->remain_cols.fill(out, k, bc->type, slot);
     }
     if (total > 0 && ga.n > 0) SR_TRY(launch_gather(ctx, j->remain_index.as<uint32_t>(), total, ga));
     return SR_OK;
@@ -1146,10 +1120,7 @@ static int32_t join_probe(sr_join* j, int32_t prober_id, const sr_chunk_view* pr
             srd::k_probe_count<<<blocks, srd::PROBE_BLOCK, 0, ctx->stream>>>(jd, kc, jt_run, n, vec_keys, match_run, ps.heads.as<uint32_t>(),
                                                                             ps.block_counts.as<uint32_t>());
         SR_LAUNCH_CHECK(ctx);
-        SR_TRY(scan_counts(ctx, &ps.scan_scratch, ps.block_counts.as<uint32_t>(), blocks, ps.block_offsets.as<uint64_t>()));
-        SR_CUDA(ctx, cudaMemcpyAsync(ctx->pinned, ctx->dscratch, sizeof(uint64_t), cudaMemcpyDeviceToHost, ctx->stream));
-        SR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        total = (int64_t)ctx->pinned[0];
+        SR_TRY(scan_counts(ctx, &ps.scan_scratch, ps.block_counts.as<uint32_t>(), blocks, ps.block_offsets.as<uint64_t>(), &total));
     }
     if (total >= 0xFFFFFFF0ll) return sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "join output of more than 2^32 rows in one batch; probe in smaller batches");
     SR_TRY(ps.probe_index.reserve(ctx, sizeof(uint32_t) * (size_t)std::max<int64_t>(total, 1)));
@@ -1174,67 +1145,48 @@ static int32_t join_probe(sr_join* j, int32_t prober_id, const sr_chunk_view* pr
     const bool right_only = jt == SR_JOIN_RIGHT_SEMI || jt == SR_JOIN_RIGHT_ANTI; // no probe column in the output, no probe-phase rows
     const int np = right_only ? 0 : j->desc.num_probe_out, nb = semi ? 0 : j->desc.num_build_out;
     if (np + nb > SR_MAX_OUT_COLS) return sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "too many join output columns");
-    if ((int)ps.out_bufs.size() < 2 * (np + nb)) {
-        std::vector<DevBuf> nbv(2 * (np + nb));
-        for (size_t i = 0; i < ps.out_bufs.size(); i++) std::swap(nbv[i], ps.out_bufs[i]);
-        ps.out_bufs.swap(nbv);
-    }
+    ps.out_cols.resize(np + nb);
     srd::GatherArgs ga_p, ga_b;
     ga_p.n = 0;
     ga_b.n = 0;
-    out->num_cols = np + nb;
-    out->mem = SR_MEM_DEVICE;
-    out->num_rows = total;
+    ColBufs::header(out, np + nb, total);
     for (int k = 0; k < np + nb; k++) {
-        srd::GatherCol g;
         int32_t slot, type;
         if (k < np) {
             slot = j->desc.probe_out_slots[k];
             const int c = ps.staged.find(slot);
             if (c < 0) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "probe chunk misses output slot %d", slot);
-            g.src = ps.staged.cols[c].data;
-            g.src_nulls = ps.staged.cols[c].nulls;
-            g.width = ps.staged.cols[c].width;
-            g.zero_is_null = 0;
-            type = ps.staged.cols[c].type;
+            const srd::DCol& dc = ps.staged.cols[c];
+            type = dc.type;
+            SR_TRY(ps.out_cols.gather(ctx, k, total, dc.data, dc.nulls, dc.width, false, &ga_p.c[ga_p.n++]));
         } else {
             slot = j->desc.build_out_slots[k - np];
             const BuildCol* bc = j->find_col(slot);
+            const void* src;
+            const uint8_t* src_nulls = nullptr;
+            int width;
             if (bc) {
-                g.src = bc->data.p;
-                g.src_nulls = bc->nullable ? (const uint8_t*)bc->nulls.p : nullptr;
-                g.width = bc->width;
+                src = bc->data.p;
+                src_nulls = bc->nullable ? (const uint8_t*)bc->nulls.p : nullptr;
+                width = bc->width;
                 type = bc->type;
             } else if (j->cols.empty() && j->desc.build_out_types[k - np] != 0) {
                 // no build chunk ever arrived (a dimension scan that filtered everything out): the schema comes from the
                 // desc; INNER probes to zero rows, LEFT OUTER to one all-NULL build row per probe row (index 0 = "no row")
                 type = j->desc.build_out_types[k - np];
-                g.width = srd::type_width(type);
-                if (g.width == 0) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "build_out_types[%d] = %d is not a type", k - np, type);
+                width = srd::type_width(type);
+                if (width == 0) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "build_out_types[%d] = %d is not a type", k - np, type);
                 SR_TRY(j->zero_row.reserve(ctx, 16));
                 SR_CUDA(ctx, cudaMemsetAsync(j->zero_row.p, 0, 16, ctx->stream));
-                g.src = j->zero_row.p;
-                g.src_nulls = nullptr;
+                src = j->zero_row.p;
             } else {
                 if (j->cols.empty())
                     return sr_fail(ctx, SR_ERR_STATE, "build side is empty and the type of slot %d is unknown: declare it in sr_join_desc.build_out_types", slot);
                 return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "build chunk misses output slot %d", slot);
             }
-            g.zero_is_null = outer ? 1 : 0;
+            SR_TRY(ps.out_cols.gather(ctx, k, total, src, src_nulls, width, outer, &ga_b.c[ga_b.n++]));
         }
-        const bool need_nulls = g.src_nulls != nullptr || g.zero_is_null;
-        SR_TRY(ps.out_bufs[2 * k].reserve(ctx, (size_t)std::max<int64_t>(total, 1) * g.width));
-        if (need_nulls) SR_TRY(ps.out_bufs[2 * k + 1].reserve(ctx, (size_t)std::max<int64_t>(total, 1)));
-        g.dst = ps.out_bufs[2 * k].p;
-        g.dst_nulls = need_nulls ? (uint8_t*)ps.out_bufs[2 * k + 1].p : nullptr;
-        out->cols[k].data = g.dst;
-        out->cols[k].nulls = g.dst_nulls;
-        out->cols[k].type = type;
-        out->cols[k].slot_id = slot;
-        if (k < np)
-            ga_p.c[ga_p.n++] = g;
-        else
-            ga_b.c[ga_b.n++] = g;
+        ps.out_cols.fill(out, k, type, slot);
     }
     if (total > 0) {
         if (ga_p.n > 0) SR_TRY(launch_gather(ctx, ps.probe_index.as<uint32_t>(), total, ga_p));

@@ -357,15 +357,6 @@ __device__ __forceinline__ void copy_elem(const void* src, void* dst, int64_t s,
 
 // K11: dst[j] = src[index[j]] (Column::append_selective); index 0 of a build column is the
 // sentinel row.  null_out (optional): 1 when index == 0 (outer join miss) or src null.
-struct GatherCol {
-    const void* src;
-    const uint8_t* src_nulls;
-    void* dst;
-    uint8_t* dst_nulls;
-    int32_t width;
-    int32_t zero_is_null; // build side of an outer join
-    int32_t vec16;        // width 16 with src and dst 16-byte aligned: one int4 per value (set by launch_gather)
-};
 struct GatherArgs {
     GatherCol c[SR_MAX_OUT_COLS];
     int32_t n;
@@ -413,25 +404,32 @@ __global__ void __launch_bounds__(256) k_gather(const uint32_t* __restrict__ ind
 // Exclusive scan of n uint32 counts into uint64 offsets, total -> ctx->dscratch[0].  Small inputs: one block walks
 // the array (k_scan_counts); large inputs: 1024-entry blocks in parallel, a scan of the block sums, a fix-up pass
 // (a single block walks 1024 entries at a time, far too slow for the ~780 K tiles of a 200 M-row probe).
+// With `total`, the total is also read back to the host: one synchronisation, which also covers whatever the caller
+// enqueued before.
 struct ScanScratch {
     DevBuf local, sums, bases;
 };
-static int32_t scan_counts(sr_ctx* ctx, ScanScratch* sc, const uint32_t* counts, int64_t n, uint64_t* offsets) {
+static int32_t scan_counts(sr_ctx* ctx, ScanScratch* sc, const uint32_t* counts, int64_t n, uint64_t* offsets, int64_t* total = nullptr) {
     if (n <= 16 * 1024) {
         srd::k_scan_counts<<<1, 1024, 0, ctx->stream>>>(counts, n, offsets, ctx->dscratch);
         SR_LAUNCH_CHECK(ctx);
-        return SR_OK;
+    } else {
+        const int64_t nblk = (n + 1023) / 1024;
+        SR_TRY(sc->local.reserve(ctx, sizeof(uint32_t) * (size_t)n));
+        SR_TRY(sc->sums.reserve(ctx, sizeof(uint32_t) * (size_t)nblk));
+        SR_TRY(sc->bases.reserve(ctx, sizeof(uint64_t) * (size_t)nblk));
+        srd::k_scan_lvl1<true><<<(int)nblk, 1024, 0, ctx->stream>>>(counts, n, sc->local.as<uint32_t>(), sc->sums.as<uint32_t>());
+        SR_LAUNCH_CHECK(ctx);
+        srd::k_scan_counts<<<1, 1024, 0, ctx->stream>>>(sc->sums.as<uint32_t>(), nblk, sc->bases.as<uint64_t>(), ctx->dscratch);
+        SR_LAUNCH_CHECK(ctx);
+        srd::k_scan_add_base<<<(int)nblk, 1024, 0, ctx->stream>>>(sc->local.as<uint32_t>(), sc->bases.as<uint64_t>(), n, offsets);
+        SR_LAUNCH_CHECK(ctx);
     }
-    const int64_t nblk = (n + 1023) / 1024;
-    SR_TRY(sc->local.reserve(ctx, sizeof(uint32_t) * (size_t)n));
-    SR_TRY(sc->sums.reserve(ctx, sizeof(uint32_t) * (size_t)nblk));
-    SR_TRY(sc->bases.reserve(ctx, sizeof(uint64_t) * (size_t)nblk));
-    srd::k_scan_lvl1<true><<<(int)nblk, 1024, 0, ctx->stream>>>(counts, n, sc->local.as<uint32_t>(), sc->sums.as<uint32_t>());
-    SR_LAUNCH_CHECK(ctx);
-    srd::k_scan_counts<<<1, 1024, 0, ctx->stream>>>(sc->sums.as<uint32_t>(), nblk, sc->bases.as<uint64_t>(), ctx->dscratch);
-    SR_LAUNCH_CHECK(ctx);
-    srd::k_scan_add_base<<<(int)nblk, 1024, 0, ctx->stream>>>(sc->local.as<uint32_t>(), sc->bases.as<uint64_t>(), n, offsets);
-    SR_LAUNCH_CHECK(ctx);
+    if (total) {
+        SR_CUDA(ctx, cudaMemcpyAsync(ctx->pinned, ctx->dscratch, sizeof(uint64_t), cudaMemcpyDeviceToHost, ctx->stream));
+        SR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        *total = (int64_t)ctx->pinned[0];
+    }
     return SR_OK;
 }
 
@@ -474,7 +472,7 @@ struct sr_scan {
     std::vector<RfUse> rf_use;
     DevBuf rf_stats; // 2 counters per filter, cleared per batch
     bool rf_adaptive = true;
-    std::vector<DevBuf> out_bufs; // 2 per out slot
+    ColBufs out_cols; // one per out slot
 };
 
 static int32_t staged_slot_type(void* user, int32_t slot) {

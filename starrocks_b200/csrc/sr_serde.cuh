@@ -8,8 +8,8 @@
 
 struct sr_serde {
     sr_ctx* ctx = nullptr;
-    std::vector<DevBuf> bufs; // 2 per column: data, nulls
-    DevBuf staging;           // host payloads are copied to the device once, then split
+    ColBufs cols;   // the deserialized columns
+    DevBuf staging; // host payloads are copied to the device once, then split
 };
 
 namespace srd {
@@ -167,27 +167,16 @@ static int32_t serde_deserialize(sr_serde* h, const void* src, int64_t bytes, in
         off += sz;
     }
     if (off != bytes) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "%lld bytes after the last column", (long long)(bytes - off));
-    if (h->bufs.size() < 2 * (size_t)meta->num_cols) {
-        std::vector<DevBuf> nb(2 * (size_t)meta->num_cols);
-        for (size_t i = 0; i < h->bufs.size(); i++) std::swap(nb[i], h->bufs[i]);
-        h->bufs.swap(nb);
-    }
     const cudaMemcpyKind kind = src_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
-    out->num_cols = meta->num_cols;
-    out->mem = SR_MEM_DEVICE;
-    out->num_rows = rows;
+    h->cols.resize(meta->num_cols);
+    ColBufs::header(out, meta->num_cols, rows);
     for (int k = 0; k < meta->num_cols; k++) {
-        out->cols[k].type = meta->types[k];
-        out->cols[k].slot_id = meta->slot_ids[k];
-        out->cols[k].nulls = nullptr;
-        if (null_off[k] >= 0) {
-            SR_TRY(h->bufs[2 * k + 1].reserve(ctx, (size_t)std::max<uint32_t>(rows, 1)));
-            if (rows) SR_CUDA(ctx, cudaMemcpyAsync(h->bufs[2 * k + 1].p, in + null_off[k], rows, kind, ctx->stream));
-            out->cols[k].nulls = (uint8_t*)h->bufs[2 * k + 1].p;
-        }
-        SR_TRY(h->bufs[2 * k].reserve(ctx, (size_t)std::max<int64_t>(data_size[k], 1)));
-        if (data_size[k]) SR_CUDA(ctx, cudaMemcpyAsync(h->bufs[2 * k].p, in + data_off[k], (size_t)data_size[k], kind, ctx->stream));
-        out->cols[k].data = h->bufs[2 * k].p;
+        void* data;
+        uint8_t* nulls;
+        SR_TRY(h->cols.reserve(ctx, k, rows, srd::type_width(meta->types[k]), null_off[k] >= 0, &data, &nulls));
+        if (nulls && rows) SR_CUDA(ctx, cudaMemcpyAsync(nulls, in + null_off[k], rows, kind, ctx->stream));
+        if (data_size[k]) SR_CUDA(ctx, cudaMemcpyAsync(data, in + data_off[k], (size_t)data_size[k], kind, ctx->stream));
+        h->cols.fill(out, k, meta->types[k], meta->slot_ids[k]);
     }
     if (!src_dev) SR_CUDA(ctx, cudaStreamSynchronize(ctx->stream)); // the caller's host buffer may go away
     return SR_OK;
