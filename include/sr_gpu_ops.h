@@ -76,15 +76,26 @@ typedef enum sr_type {
 /* byte width of one value of the type (0 for an unknown type). */
 int32_t sr_type_width(int32_t type);
 
-/* SR_MEM_HOST: pageable or pinned host memory, staged with H2D copies on the context's stream.
- * SR_MEM_DEVICE: device pointers, read in place.
+/* Where a caller's buffer lives: every `mem`, `sel_mem`, `out_mem`, `dst_mem`, `src_mem` argument and sr_chunk_view.mem.
+ * SR_MEM_HOST: pageable or pinned host memory, copied with H2D / D2H copies on the context's stream.
+ * SR_MEM_DEVICE: device pointers, read and written in place.
  * SR_MEM_HOST_PINNED: page-locked host memory mapped into the device address space (cudaHostAlloc /
- *   cudaHostRegister, e.g. a registered ColumnAllocator pool).  sr_fragment_push reads such columns IN PLACE over
- *   PCIe (late materialisation: a column is only fetched for the 32-byte sectors holding rows that survived the
- *   earlier joins, so far fewer bytes cross the bus than a full H2D copy); every other entry point treats it like
- *   SR_MEM_HOST.  Passing unpinned memory with this tag is rejected with SR_ERR_INVALID_ARGUMENT.  The buffers
- *   must stay valid and unmodified until the next synchronising call on the context (sr_ctx_sync,
- *   sr_agg_sink_finish, sr_fragment_rows_passed). */
+ *   cudaHostRegister, e.g. a registered ColumnAllocator pool).
+ * One rule for all entry points:
+ *  1. An unknown kind is refused with SR_ERR_INVALID_ARGUMENT before any copy, allocation or launch.
+ *  2. Only sr_fragment_push (the fact columns) and sr_pages_decode (the pages) read SR_MEM_HOST_PINNED buffers IN PLACE
+ *     over PCIe: the fragment fetches a column only for the 32-byte sectors holding rows that survived the earlier
+ *     joins, so far fewer bytes cross the bus than a full H2D copy.  Where a buffer is read in place, memory that is not
+ *     page-locked and mapped is refused with SR_ERR_INVALID_ARGUMENT.  Every other entry point treats SR_MEM_HOST_PINNED
+ *     exactly like SR_MEM_HOST, for inputs and for outputs.
+ *  3. A call that writes its result into host memory (either host kind) synchronises before it returns; a result
+ *     handed back in host memory (sr_chunk_out.mem) is reported as SR_MEM_HOST.
+ *  4. Host inputs: a call waits for the copies of its host inputs before it returns, so that the caller may free or
+ *     reuse them, except sr_fragment_push, sr_agg_push and sr_agg_push_selective on a dense or single-state table,
+ *     sr_scan_evaluate with a device selection, sr_xchg_hash with device outputs and sr_chunk_serialize into device
+ *     memory.  After one of these a page-locked input (pageable memory may be reused at once), and after any call a
+ *     buffer read in place, must stay valid and unmodified until the next synchronising call on the context
+ *     (sr_ctx_sync, sr_agg_sink_finish, sr_fragment_rows_passed, or any call that waits). */
 typedef enum sr_mem { SR_MEM_HOST = 0, SR_MEM_DEVICE = 1, SR_MEM_HOST_PINNED = 2 } sr_mem;
 
 /* mirrors FixedLengthColumn / NullableColumn raw buffers (be/src/column/nullable_column.h:32:
@@ -259,8 +270,8 @@ void sr_scan_destroy(sr_scan* scan);
  * next push) holding the surviving rows in input order; out->num_rows is filled after an
  * internal sync on the tiny row counter. */
 int32_t sr_scan_filter(sr_scan* scan, const sr_chunk_view* in, sr_chunk_out* out);
-/* evaluate only: write the uint8 selection vector (1 = row passes) to `selection`
- * (host or device pointer according to sel_mem) -- the ColumnPredicate::evaluate contract. */
+/* evaluate only: write the uint8 selection vector (1 = row passes) to `selection` in sel_mem (sr_mem rules: a host
+ * selection is complete on return) -- the ColumnPredicate::evaluate contract. */
 int32_t sr_scan_evaluate(sr_scan* scan, const sr_chunk_view* in, uint8_t* selection, int32_t sel_mem);
 
 /* ---------------------------------------------------------------------------------------
@@ -382,7 +393,8 @@ int32_t sr_join_probe_indexes(sr_join* join, int32_t prober_id, const uint32_t**
 
 /* K5: JoinKeyHash / calc_bucket_num (be/src/exec/join/join_hash_map_helper.h:35-54,79-84)
  * on the device, exposed so the multiplicative hash can be pinned against the reference's
- * golden vectors.  keys: `n` values of key_type in `mem`; buckets: n uint32 in `mem`. */
+ * golden vectors.  keys: `n` values of key_type in `mem`; buckets: n uint32 in `mem` (sr_mem rules: host buckets are
+ * complete on return; device keys and buckets must be naturally aligned). */
 int32_t sr_join_key_hash(sr_ctx* ctx, const void* keys, int32_t key_type, int64_t n, uint32_t log_bucket_size,
                          uint32_t* buckets, int32_t mem);
 
@@ -526,8 +538,9 @@ int64_t sr_agg_num_groups(sr_agg* agg);
 /* AggregateBlockingSourceOperator::pull_chunk (aggregate_blocking_source_operator.cpp:47-72) ->
  * Aggregator::convert_hash_map_to_chunk / convert_to_chunk_no_groupby (aggregator.cpp:1696-1791, 997-1042).
  * Emit up to max_rows groups starting at the handle's cursor: key columns (group_slots order)
- * then one result column per function.  out_mem selects host (copied back, synchronised) or
- * device buffers.  Returns SR_OK with out->num_rows == 0 at end of stream. */
+ * then one result column per function.  out_mem selects host buffers (page-locked, owned by the handle, complete on
+ * return; out->mem = SR_MEM_HOST for either host kind) or device buffers.  Returns SR_OK with out->num_rows == 0 at
+ * end of stream. */
 int32_t sr_agg_pull(sr_agg* agg, int64_t max_rows, int32_t out_mem, sr_chunk_out* out);
 /* Operator::reset_state (be/src/exec/pipeline/operator.h:143): clear every group and state so
  * the handle can aggregate a new stream; keeps the compiled plan and the table capacity. */
@@ -702,7 +715,7 @@ void sr_xchg_destroy(sr_xchg* x);
  * zero-row columns whose `data` may be NULL; a nullable input column still gets a non-NULL (empty) `nulls`, so every
  * batch's output, and every channel's ChunkPB, has the same null columns. */
 int32_t sr_xchg_partition(sr_xchg* x, const sr_chunk_view* in, sr_chunk_out* out, int64_t* channel_offsets_host);
-/* hash values + channel ids only (device or host arrays of num_rows uint32, per `mem`). */
+/* hash values + channel ids only (arrays of num_rows uint32 in `mem`; sr_mem rules: host arrays are complete on return). */
 int32_t sr_xchg_hash(sr_xchg* x, const sr_chunk_view* in, uint32_t* hash_values, uint32_t* channel_ids, int32_t mem);
 
 /* ---------------------------------------------------------------------------------------
@@ -780,7 +793,7 @@ typedef struct sr_chunk_pb_meta {
 } sr_chunk_pb_meta;
 /* bytes rows [row_begin, row_end) of `chunk` serialize to */
 int64_t sr_chunk_serialized_size(const sr_chunk_view* chunk, int64_t row_begin, int64_t row_end);
-/* Serialize rows [row_begin, row_end) of `chunk` (host or device columns) into dst (dst_mem: SR_MEM_HOST -- a page-locked
+/* Serialize rows [row_begin, row_end) of `chunk` (host or device columns) into dst (dst_mem: host memory -- a page-locked
  * buffer makes it one DMA per column -- or SR_MEM_DEVICE); dst_capacity >= sr_chunk_serialized_size.  Queued on the context's
  * stream; synchronises when dst is host memory. */
 int32_t sr_chunk_serialize(sr_ctx* ctx, const sr_chunk_view* chunk, int64_t row_begin, int64_t row_end, void* dst, int64_t dst_capacity,

@@ -159,15 +159,6 @@ struct sr_xchg {
     ColBufs out_cols;
 };
 
-// ---------------------------------------------------------------------------------------
-// helpers
-// ---------------------------------------------------------------------------------------
-static int32_t copy_out(sr_ctx* ctx, void* dst, const void* src_dev, size_t bytes, int32_t mem) {
-    if (bytes == 0) return SR_OK;
-    SR_CUDA(ctx, cudaMemcpyAsync(dst, src_dev, bytes, mem == SR_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, ctx->stream));
-    return SR_OK;
-}
-
 extern "C" {
 
 int32_t sr_abi_version(void) {
@@ -362,11 +353,11 @@ int32_t sr_scan_evaluate(sr_scan* s, const sr_chunk_view* in, uint8_t* selection
     if (!s || !in || !selection) return SR_ERR_INVALID_ARGUMENT;
     sr_ctx* ctx = s->ctx;
     SR_BIND(ctx);
+    SR_TRY(mem_check(ctx, sel_mem, "sel_mem"));
     int64_t total;
     SR_TRY(scan_select(s, in, false, &total));
-    SR_TRY(copy_out(ctx, selection, s->sel.p, (size_t)in->num_rows, sel_mem));
-    if (sel_mem == SR_MEM_HOST) SR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    return SR_OK;
+    SR_TRY(mem_out(ctx, selection, s->sel.p, (size_t)in->num_rows, sel_mem));
+    return mem_sync(ctx, sel_mem);
 }
 
 int32_t sr_scan_filter(sr_scan* s, const sr_chunk_view* in, sr_chunk_out* out) {
@@ -559,8 +550,7 @@ int32_t sr_rf_insert(sr_rf* rf, const sr_chunk_view* in, int32_t slot_id, int32_
     const int c = rf->staged.find(slot_id);
     if (c < 0) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "chunk misses slot %d", slot_id);
     SR_TRY(rf_insert_dcol(rf, rf->staged.cols[c], in->num_rows, insert_nulls));
-    if (in->mem != SR_MEM_DEVICE) SR_CUDA(ctx, cudaStreamSynchronize(ctx->stream)); // caller may free host buffers
-    return SR_OK;
+    return mem_sync(ctx, in->mem);
 }
 
 sr_rf* sr_join_build_runtime_filter(sr_join* join, int32_t key_index, int32_t with_bloom, int32_t insert_nulls) {
@@ -615,8 +605,9 @@ int32_t sr_rf_copy_directory(sr_rf* rf, void* dst, int64_t bytes, int32_t mem) {
     if (!rf || (!dst && bytes > 0)) return SR_ERR_INVALID_ARGUMENT;
     sr_ctx* ctx = rf->ctx;
     SR_BIND(ctx);
+    SR_TRY(mem_check(ctx, mem, "sr_rf_copy_directory"));
     if (bytes != (int64_t)rf->dir_bytes()) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "directory is %zu bytes, caller passed %lld", rf->dir_bytes(), (long long)bytes);
-    SR_TRY(copy_out(ctx, dst, rf->dir.p, (size_t)bytes, mem));
+    SR_TRY(mem_out(ctx, dst, rf->dir.p, (size_t)bytes, mem));
     SR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     return SR_OK;
 }
@@ -655,23 +646,20 @@ int32_t sr_rf_merge_directory(sr_rf* rf, const void* directory, int64_t bytes, i
     if (!rf || !other) return SR_ERR_INVALID_ARGUMENT;
     sr_ctx* ctx = rf->ctx;
     SR_BIND(ctx);
+    SR_TRY(mem_check(ctx, mem, "sr_rf_merge_directory"));
     if (other->log_num_buckets != rf->log_num_buckets) // SimdBlockFilter::merge DCHECKs equal sizes
         return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "bloom directories of different size (2^%d vs 2^%d buckets)", rf->log_num_buckets, other->log_num_buckets);
     if (bytes != (int64_t)rf->dir_bytes() || (bytes > 0 && !directory)) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "directory is %zu bytes, caller passed %lld", rf->dir_bytes(), (long long)bytes);
-    if (mem == SR_MEM_DEVICE && !col_aligned(directory, 4)) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "device directory at %p is not 4-byte aligned", directory);
+    if (!mem_is_host(mem) && !col_aligned(directory, 4)) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "device directory at %p is not 4-byte aligned", directory);
     rf->stats_valid = false;
     if (bytes > 0) {
         DevBuf tmp;
-        const uint32_t* src = (const uint32_t*)directory;
-        if (mem != SR_MEM_DEVICE) {
-            SR_TRY(tmp.reserve(ctx, (size_t)bytes));
-            SR_CUDA(ctx, cudaMemcpyAsync(tmp.p, directory, (size_t)bytes, cudaMemcpyHostToDevice, ctx->stream));
-            src = tmp.as<uint32_t>();
-        }
+        const void* src;
+        SR_TRY(mem_in(ctx, directory, (size_t)bytes, mem, &tmp, &src));
         const int64_t words = bytes / 4;
-        srd::k_or_u32<<<std::min(grid_for(words, 256), ctx->num_sms * 8), 256, 0, ctx->stream>>>(rf->dir.as<uint32_t>(), src, words);
+        srd::k_or_u32<<<std::min(grid_for(words, 256), ctx->num_sms * 8), 256, 0, ctx->stream>>>(rf->dir.as<uint32_t>(), (const uint32_t*)src, words);
         SR_LAUNCH_CHECK(ctx);
-        if (mem != SR_MEM_DEVICE) SR_CUDA(ctx, cudaStreamSynchronize(ctx->stream)); // tmp is freed on return
+        SR_TRY(mem_sync(ctx, mem));
     }
     srd::k_rf_merge_stats<<<1, 1, 0, ctx->stream>>>(rf->stats.as<long long>(), other->min_value, other->max_value, other->num_inserted, other->has_null ? 1 : 0);
     SR_LAUNCH_CHECK(ctx);
@@ -682,6 +670,8 @@ int32_t sr_rf_evaluate(sr_rf* rf, const sr_chunk_view* in, int32_t slot_id, uint
     if (!rf || !in || (!selection && in->num_rows > 0)) return SR_ERR_INVALID_ARGUMENT;
     sr_ctx* ctx = rf->ctx;
     SR_BIND(ctx);
+    SR_TRY(mem_check(ctx, in->mem, "chunk"));
+    SR_TRY(mem_check(ctx, sel_mem, "sel_mem"));
     const int64_t n = in->num_rows;
     if (n <= 0) return SR_OK;
     const std::vector<int32_t> only{slot_id};
@@ -693,20 +683,12 @@ int32_t sr_rf_evaluate(sr_rf* rf, const sr_chunk_view* in, int32_t slot_id, uint
     srd::RfDev d;
     SR_TRY(rf_device_desc(rf, &d));
     DevBuf tmp;
-    uint8_t* dsel = selection;
-    if (sel_mem != SR_MEM_DEVICE) {
-        SR_TRY(tmp.reserve(ctx, (size_t)n));
-        if (merge_and) SR_CUDA(ctx, cudaMemcpyAsync(tmp.p, selection, (size_t)n, cudaMemcpyHostToDevice, ctx->stream));
-        dsel = tmp.as<uint8_t>();
-    }
-    srd::k_rf_evaluate<<<std::min(grid_for(n, 256), ctx->num_sms * 8), 256, 0, ctx->stream>>>(d, col, n, dsel, merge_and ? 1 : 0);
+    const void* dsel;
+    SR_TRY(mem_in(ctx, selection, (size_t)n, sel_mem, &tmp, &dsel, merge_and != 0));
+    srd::k_rf_evaluate<<<std::min(grid_for(n, 256), ctx->num_sms * 8), 256, 0, ctx->stream>>>(d, col, n, (uint8_t*)dsel, merge_and ? 1 : 0);
     SR_LAUNCH_CHECK(ctx);
-    if (sel_mem != SR_MEM_DEVICE) {
-        SR_CUDA(ctx, cudaMemcpyAsync(selection, dsel, (size_t)n, cudaMemcpyDeviceToHost, ctx->stream));
-        SR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    } else if (in->mem != SR_MEM_DEVICE) {
-        SR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    }
+    SR_TRY(mem_out(ctx, selection, dsel, (size_t)n, sel_mem));
+    if (mem_is_host(sel_mem) || mem_is_host(in->mem)) SR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     return SR_OK;
 }
 
@@ -745,29 +727,21 @@ int32_t sr_scan_set_rf_adaptive(sr_scan* scan, int32_t adaptive) {
 
 int32_t sr_join_key_hash(sr_ctx* ctx, const void* keys, int32_t key_type, int64_t n, uint32_t log_bucket_size, uint32_t* buckets, int32_t mem) {
     SR_BIND(ctx);
+    SR_TRY(mem_check(ctx, mem, "sr_join_key_hash"));
     const int w = srd::type_width(key_type);
     if ((w != 4 && w != 8) || srd::is_float_class(key_type)) return sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "sr_join_key_hash: 4- or 8-byte integer keys only");
     if (log_bucket_size < 1 || log_bucket_size > 31) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "log_bucket_size %u", log_bucket_size);
     if (n <= 0) return SR_OK;
-    if (mem != SR_MEM_HOST && (!col_aligned(keys, w) || !col_aligned(buckets, 4)))
+    if (!mem_is_host(mem) && (!col_aligned(keys, w) || !col_aligned(buckets, 4)))
         return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "sr_join_key_hash: device keys or buckets are not naturally aligned");
     DevBuf kin, kout;
-    const void* dk = keys;
-    uint32_t* dout = buckets;
-    if (mem == SR_MEM_HOST) {
-        SR_TRY(kin.reserve(ctx, (size_t)n * w));
-        SR_TRY(kout.reserve(ctx, (size_t)n * 4));
-        SR_CUDA(ctx, cudaMemcpyAsync(kin.p, keys, (size_t)n * w, cudaMemcpyHostToDevice, ctx->stream));
-        dk = kin.p;
-        dout = kout.as<uint32_t>();
-    }
-    srd::k_join_key_hash<<<std::min(grid_for(n, 256), ctx->num_sms * 8), 256, 0, ctx->stream>>>(dk, key_type, n, log_bucket_size, dout);
+    const void *dk, *dout;
+    SR_TRY(mem_in(ctx, keys, (size_t)n * w, mem, &kin, &dk));
+    SR_TRY(mem_in(ctx, buckets, (size_t)n * 4, mem, &kout, &dout, false));
+    srd::k_join_key_hash<<<std::min(grid_for(n, 256), ctx->num_sms * 8), 256, 0, ctx->stream>>>(dk, key_type, n, log_bucket_size, (uint32_t*)dout);
     SR_LAUNCH_CHECK(ctx);
-    if (mem == SR_MEM_HOST) {
-        SR_CUDA(ctx, cudaMemcpyAsync(buckets, dout, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream));
-        SR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    }
-    return SR_OK;
+    SR_TRY(mem_out(ctx, buckets, dout, (size_t)n * 4, mem));
+    return mem_sync(ctx, mem);
 }
 
 // ------------------------------------------------------------------ aggregate
@@ -834,14 +808,15 @@ int32_t sr_agg_pull(sr_agg* a, int64_t max_rows, int32_t out_mem, sr_chunk_out* 
     sr_ctx* ctx = a->ctx;
     SR_BIND(ctx);
     if (!a->finished) return sr_fail(ctx, SR_ERR_STATE, "pull before sink_finish");
+    SR_TRY(mem_check(ctx, out_mem, "out_mem"));
     SR_TRY(agg_finish_output(a));
     const sr_agg_desc& d = a->desc;
     const int nc = d.num_group_keys + d.num_fns;
     const int64_t n = std::min<int64_t>(max_rows, a->out_rows - a->cursor);
     out->num_cols = nc;
-    out->mem = out_mem;
+    out->mem = mem_is_host(out_mem) ? SR_MEM_HOST : SR_MEM_DEVICE;
     out->num_rows = std::max<int64_t>(n, 0);
-    if (out_mem == SR_MEM_HOST && a->host_bufs.size() < 2 * (size_t)nc) a->host_bufs.resize(2 * (size_t)nc);
+    if (mem_is_host(out_mem) && a->host_bufs.size() < 2 * (size_t)nc) a->host_bufs.resize(2 * (size_t)nc);
     for (int k = 0; k < nc; k++) {
         const int32_t type = a->out_rows > 0 || a->compiled ? a->out_types[k] : (k < d.num_group_keys ? d.group_types[k] : agg_result_type(d.fns[k - d.num_group_keys]));
         const int w = srd::type_width(type);
@@ -853,7 +828,7 @@ int32_t sr_agg_pull(sr_agg* a, int64_t max_rows, int32_t out_mem, sr_chunk_out* 
         const ColBufs::Col& oc = a->out_cols.cols[k];
         const uint8_t* ddata = (const uint8_t*)oc.data.p + (size_t)a->cursor * w;
         const uint8_t* dnull = oc.nullable ? (const uint8_t*)oc.nulls.p + a->cursor : nullptr;
-        if (out_mem == SR_MEM_DEVICE) {
+        if (!mem_is_host(out_mem)) {
             out->cols[k].data = (void*)ddata;
             out->cols[k].nulls = (uint8_t*)dnull;
         } else {
@@ -867,7 +842,7 @@ int32_t sr_agg_pull(sr_agg* a, int64_t max_rows, int32_t out_mem, sr_chunk_out* 
             }
         }
     }
-    if (out_mem == SR_MEM_HOST) SR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    SR_TRY(mem_sync(ctx, out_mem));
     if (n > 0) a->cursor += n;
     return SR_OK;
 }
@@ -1072,8 +1047,7 @@ int32_t sr_agg_convert_to_states(sr_agg* a, const sr_chunk_view* chunk, sr_chunk
     sr_ctx* ctx = a->ctx;
     SR_BIND(ctx);
     SR_TRY(agg_convert_impl(a, chunk, out, nullptr));
-    if (chunk->mem != SR_MEM_DEVICE) SR_CUDA(ctx, cudaStreamSynchronize(ctx->stream)); // caller may free host buffers
-    return SR_OK;
+    return mem_sync(ctx, chunk->mem);
 }
 
 // SELECTIVE_PREAGG leg of the streaming aggregate (aggregate_streaming_sink_operator.cpp:173-210)
@@ -1124,8 +1098,7 @@ int32_t sr_agg_push_selective(sr_agg* a, const sr_chunk_view* chunk, sr_chunk_ou
         a->sel_cols.fill(out, k, oc.type, oc.slot_id);
     }
     SR_TRY(launch_gather(ctx, a->sel_index.as<uint32_t>(), m, ga));
-    if (chunk->mem != SR_MEM_DEVICE) SR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    return SR_OK;
+    return mem_sync(ctx, chunk->mem);
 }
 
 int32_t sr_agg_merge(sr_agg* a, sr_agg* o) {
@@ -1348,6 +1321,7 @@ int32_t sr_xchg_hash(sr_xchg* x, const sr_chunk_view* in, uint32_t* hash_values,
     if (!x || !in) return SR_ERR_INVALID_ARGUMENT;
     sr_ctx* ctx = x->ctx;
     SR_BIND(ctx);
+    SR_TRY(mem_check(ctx, mem, "sr_xchg_hash"));
     SR_TRY(x->staged.stage(ctx, in));
     srd::PartCols pc;
     SR_TRY(xchg_part_cols(x, &pc));
@@ -1358,10 +1332,9 @@ int32_t sr_xchg_hash(sr_xchg* x, const sr_chunk_view* in, uint32_t* hash_values,
     const int tiles = grid_for(n, srd::PART_TILE);
     srd::k_part_hash<<<tiles, srd::PART_BLOCK, 0, ctx->stream>>>(pc, n, x->hash_values.as<uint32_t>(), x->channel_ids.as<uint32_t>(), nullptr, tiles);
     SR_LAUNCH_CHECK(ctx);
-    if (hash_values) SR_TRY(copy_out(ctx, hash_values, x->hash_values.p, sizeof(uint32_t) * (size_t)n, mem));
-    if (channel_ids) SR_TRY(copy_out(ctx, channel_ids, x->channel_ids.p, sizeof(uint32_t) * (size_t)n, mem));
-    if (mem == SR_MEM_HOST) SR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    return SR_OK;
+    if (hash_values) SR_TRY(mem_out(ctx, hash_values, x->hash_values.p, sizeof(uint32_t) * (size_t)n, mem));
+    if (channel_ids) SR_TRY(mem_out(ctx, channel_ids, x->channel_ids.p, sizeof(uint32_t) * (size_t)n, mem));
+    return mem_sync(ctx, mem);
 }
 
 int32_t sr_xchg_partition(sr_xchg* x, const sr_chunk_view* in, sr_chunk_out* out, int64_t* channel_offsets_host) {
@@ -1425,7 +1398,8 @@ int32_t sr_gather(sr_ctx* ctx, const void* src, int32_t type, const uint32_t* in
     SR_BIND(ctx);
     const int w = srd::type_width(type);
     if (w == 0) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "unknown type %d", type);
-    if (mem != SR_MEM_DEVICE) return sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "sr_gather takes device pointers");
+    SR_TRY(mem_check(ctx, mem, "sr_gather"));
+    if (mem_is_host(mem)) return sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "sr_gather takes device pointers");
     if (n <= 0) return SR_OK;
     if (!col_aligned(src, w) || !col_aligned(dst, w) || !col_aligned(index, 4))
         return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "sr_gather: a device pointer is not naturally aligned for width %d", w);
@@ -1566,10 +1540,10 @@ int32_t sr_page_decoder_set_dict(sr_page_decoder* d, const int32_t* values, int6
     SR_BIND(d->ctx);
     sr_ctx* ctx = d->ctx;
     if (num_words < 0 || num_words > INT32_MAX || (num_words > 0 && !values)) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "sr_page_decoder_set_dict: %lld words", (long long)num_words);
-    if (mem != SR_MEM_HOST && mem != SR_MEM_DEVICE && mem != SR_MEM_HOST_PINNED) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "unknown memory kind %d", mem);
+    SR_TRY(mem_check(ctx, mem, "sr_page_decoder_set_dict"));
     d->dict_words = -1; // a failed call leaves no table
     SR_TRY(d->dict.reserve(ctx, 4 * (size_t)num_words + 4));
-    if (num_words > 0) SR_CUDA(ctx, cudaMemcpyAsync(d->dict.p, values, 4 * (size_t)num_words, cudaMemcpyDefault, ctx->stream));
+    if (num_words > 0) SR_CUDA(ctx, cudaMemcpyAsync(d->dict.p, values, 4 * (size_t)num_words, mem_is_host(mem) ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, ctx->stream));
     SR_CUDA(ctx, cudaStreamSynchronize(ctx->stream)); // the caller may free `values` on return
     d->dict_words = num_words;
     return SR_OK;

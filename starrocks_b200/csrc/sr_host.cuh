@@ -248,6 +248,42 @@ static inline bool col_aligned(const void* p, int width) {
     return ((uintptr_t)p & (uintptr_t)(std::min(width, 8) - 1)) == 0;
 }
 
+// memory kinds: the sr_mem rule of include/sr_gpu_ops.h.  Outside the two in-place readers (Staged::stage for
+// sr_fragment_push, pages_decode), SR_MEM_HOST_PINNED is host memory like SR_MEM_HOST.
+static inline bool mem_is_host(int32_t mem) {
+    return mem == SR_MEM_HOST || mem == SR_MEM_HOST_PINNED;
+}
+
+// refuses an unknown kind: every entry point checks its kinds before any copy, allocation or launch
+static int32_t mem_check(sr_ctx* ctx, int32_t mem, const char* what) {
+    if (mem == SR_MEM_DEVICE || mem_is_host(mem)) return SR_OK;
+    return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "%s: unknown memory kind %d", what, mem);
+}
+
+// the caller's buffer as a device pointer: the buffer itself for device memory, else `tmp` holding an H2D copy of it
+// (copy = false: an output buffer, `tmp` is only its space); `tmp` must outlive the queued work (mem_sync)
+static int32_t mem_in(sr_ctx* ctx, const void* buf, size_t bytes, int32_t mem, DevBuf* tmp, const void** dev, bool copy = true) {
+    *dev = buf;
+    if (!mem_is_host(mem)) return SR_OK;
+    SR_TRY(tmp->reserve(ctx, bytes));
+    if (copy) SR_CUDA(ctx, cudaMemcpyAsync(tmp->p, buf, bytes, cudaMemcpyHostToDevice, ctx->stream));
+    *dev = tmp->p;
+    return SR_OK;
+}
+
+// queues the copy of a device result into the caller's buffer (none when the result is already there)
+static int32_t mem_out(sr_ctx* ctx, void* dst, const void* src_dev, size_t bytes, int32_t mem) {
+    if (bytes == 0 || dst == src_dev) return SR_OK;
+    SR_CUDA(ctx, cudaMemcpyAsync(dst, src_dev, bytes, mem_is_host(mem) ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, ctx->stream));
+    return SR_OK;
+}
+
+// for host memory, waits for the stream: a host result is complete, a host input (and its staging) free, on return
+static int32_t mem_sync(sr_ctx* ctx, int32_t mem) {
+    if (mem_is_host(mem)) SR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    return SR_OK;
+}
+
 // A chunk made resident on the device: host chunks are staged (H2D on the ctx stream) into
 // buffers owned by `Staged`; device chunks (and pinned ones read in place) are referenced in place and must be
 // naturally aligned.
@@ -271,8 +307,7 @@ struct Staged {
         cols.clear();
         slots.clear();
         num_rows = in->num_rows;
-        if (in->mem != SR_MEM_HOST && in->mem != SR_MEM_DEVICE && in->mem != SR_MEM_HOST_PINNED)
-            return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "unknown memory kind %d", in->mem);
+        SR_TRY(mem_check(ctx, in->mem, "chunk"));
         bufs.resize(in->num_cols);
         for (int k = 0; k < in->num_cols; k++) {
             const sr_col_view& c = in->cols[k];

@@ -707,7 +707,8 @@ static int32_t join_grow(sr_join* j, int64_t need_rows_incl_sentinel) {
 static int32_t join_append(sr_join* j, const sr_chunk_view* chunk) {
     sr_ctx* ctx = j->ctx;
     if (j->built) return sr_fail(ctx, SR_ERR_STATE, "append_build after build_finish");
-    const cudaMemcpyKind kind = chunk->mem == SR_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+    SR_TRY(mem_check(ctx, chunk->mem, "chunk"));
+    const cudaMemcpyKind kind = mem_is_host(chunk->mem) ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice;
     if (j->cols.empty()) {
         for (int k = 0; k < chunk->num_cols; k++) {
             const sr_col_view& c = chunk->cols[k];
@@ -748,7 +749,7 @@ static int32_t join_append(sr_join* j, const sr_chunk_view* chunk) {
                 SR_CUDA(ctx, cudaMemsetAsync((uint8_t*)bc->nulls.p + (j->rows + 1), 0, (size_t)n, ctx->stream));
         }
     }
-    if (chunk->mem != SR_MEM_DEVICE) SR_CUDA(ctx, cudaStreamSynchronize(ctx->stream)); // caller may free host buffers
+    SR_TRY(mem_sync(ctx, chunk->mem));
     j->rows += n;
     return SR_OK;
 }

@@ -512,7 +512,7 @@ static int32_t pages_decode(sr_ctx* ctx, PageScratch* sc, int32_t encoding, int3
         if (encoding != SR_PAGE_PLAIN && encoding != SR_PAGE_FOR) return sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "page encoding %d", encoding);
     }
     if (num_pages < 0 || (num_pages > 0 && !pv)) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "pages");
-    if (mem != SR_MEM_HOST && mem != SR_MEM_DEVICE && mem != SR_MEM_HOST_PINNED) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "unknown memory kind %d", mem);
+    SR_TRY(mem_check(ctx, mem, "pages"));
     *out_rows = 0;
     if (num_pages == 0) return SR_OK;
     if (!sc->host_pages.reserve(sizeof(srd::PageDesc) * (size_t)num_pages) || !sc->host_counts.reserve(16 * (size_t)num_pages + 16))
@@ -528,7 +528,7 @@ static int32_t pages_decode(sr_ctx* ctx, PageScratch* sc, int32_t encoding, int3
         int first, last;
     };
     std::vector<Run> runs;
-    if (mem != SR_MEM_DEVICE) {
+    if (mem_is_host(mem)) {
         for (int p = 0; p < num_pages; p++) {
             const uint8_t* d = (const uint8_t*)pv[p].data;
             if (!runs.empty() && pv[p].size > 0 && d >= runs.back().begin + runs.back().bytes && d < runs.back().begin + runs.back().bytes + 64) {

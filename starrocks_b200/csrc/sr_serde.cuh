@@ -57,8 +57,9 @@ static int32_t serde_serialize(sr_ctx* ctx, const sr_chunk_view* c, int64_t r0, 
     }
     const int64_t total = serde_size(c, rows);
     if (total > cap) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "destination of %lld bytes, %lld needed", (long long)cap, (long long)total);
-    if (dst_mem != SR_MEM_HOST && dst_mem != SR_MEM_DEVICE && dst_mem != SR_MEM_HOST_PINNED) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "dst_mem %d", dst_mem);
-    const bool dst_dev = dst_mem == SR_MEM_DEVICE, src_dev = c->mem == SR_MEM_DEVICE;
+    SR_TRY(mem_check(ctx, c->mem, "chunk"));
+    SR_TRY(mem_check(ctx, dst_mem, "dst_mem"));
+    const bool dst_dev = !mem_is_host(dst_mem), src_dev = !mem_is_host(c->mem);
     const cudaMemcpyKind kind = src_dev ? (dst_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost) : (dst_dev ? cudaMemcpyHostToDevice : cudaMemcpyHostToHost);
     uint8_t* out = (uint8_t*)dst;
     srd::SerdeWords words;
@@ -116,6 +117,7 @@ static int32_t serde_serialize(sr_ctx* ctx, const sr_chunk_view* c, int64_t r0, 
 // last column.  The whole layout is checked before the first column is copied, so a refused payload queues no copy.
 static int32_t serde_deserialize(sr_serde* h, const void* src, int64_t bytes, int32_t src_mem, const sr_chunk_pb_meta* meta, sr_chunk_out* out) {
     sr_ctx* ctx = h->ctx;
+    SR_TRY(mem_check(ctx, src_mem, "src_mem"));
     if (meta->num_cols < 0 || meta->num_cols > SR_MAX_OUT_COLS) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "%d columns", meta->num_cols);
     for (int k = 0; k < meta->num_cols; k++)
         if (meta->is_consts[k]) return sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "column %d is a const column: ConstColumnSerde payloads are not parsed", k);
@@ -124,7 +126,7 @@ static int32_t serde_deserialize(sr_serde* h, const void* src, int64_t bytes, in
         return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "payload of %lld bytes, meta.serialized_size %lld", (long long)bytes, (long long)meta->serialized_size);
     // the header words and the per-column sizes steer the parse: read them on the host (device payload: the first pass
     // copies the whole payload's size words one by one -- at most 2 per column)
-    const bool src_dev = src_mem == SR_MEM_DEVICE;
+    const bool src_dev = !mem_is_host(src_mem);
     const uint8_t* in = (const uint8_t*)src;
     auto read32 = [&](int64_t off, uint32_t* v) -> int32_t {
         if (off + 4 > bytes) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "payload truncated at byte %lld", (long long)off);
@@ -178,6 +180,5 @@ static int32_t serde_deserialize(sr_serde* h, const void* src, int64_t bytes, in
         if (data_size[k]) SR_CUDA(ctx, cudaMemcpyAsync(data, in + data_off[k], (size_t)data_size[k], kind, ctx->stream));
         h->cols.fill(out, k, meta->types[k], meta->slot_ids[k]);
     }
-    if (!src_dev) SR_CUDA(ctx, cudaStreamSynchronize(ctx->stream)); // the caller's host buffer may go away
-    return SR_OK;
+    return mem_sync(ctx, src_mem); // the caller's host buffer may go away
 }
