@@ -246,13 +246,16 @@ __device__ __forceinline__ void hkey_or(HKey& k, unsigned long long bits, int sh
 __device__ __forceinline__ unsigned long long hkey_bits(const HKey& k, int shift) { return shift < 64 ? k.lo >> shift : k.hi >> (shift - 64); }
 __device__ __forceinline__ bool hkey_is_empty(const AggDev& a, const HKey& k) { return k.lo == SR_AGG_EMPTY && (!a.wide || k.hi == SR_AGG_EMPTY); }
 __device__ __forceinline__ bool hkey_eq(const AggDev& a, const HKey& x, const HKey& y) { return x.lo == y.lo && (!a.wide || x.hi == y.hi); }
-// xorshift - multiply - xorshift: half the instructions of the murmur finaliser (mix64), and the radix-partitioned push
-// hashes every row three times.  The leading fold keeps keys that differ only in their high bits (ids shifted left, packed
-// second columns) apart in the LOW bits, which pick the slot inside a 256-slot probing slice.
+// the murmur3 finaliser (fmix64).  A probe never leaves its 256-slot slice, so the hash must spread keys over the slices as
+// a uniform one would: the single multiply of xorshift - multiply - xorshift put up to 317 of the keys 1000 i, 2^32 i or
+// 1.6e12 + 10000 i in one slice of a half-full table (a uniform hash: about 175), which refused them.  fmix64 keeps every
+// such family at the uniform bound (tests/test_gpu_agg_table_load.py).
 __device__ __forceinline__ unsigned long long agg_hash64(unsigned long long x) {
-    x ^= x >> 32;
-    x *= 0x9E3779B97F4A7C15ull;
-    return x ^ (x >> 29);
+    x ^= x >> 33;
+    x *= 0xFF51AFD7ED558CCDull;
+    x ^= x >> 33;
+    x *= 0xC4CEB9FE1A85EC53ull;
+    return x ^ (x >> 33);
 }
 __device__ __forceinline__ unsigned long long hkey_hash(const AggDev& a, const HKey& k) {
     return a.wide ? agg_hash64(k.lo ^ (agg_hash64(k.hi) + 0x632BE59BD9B4E019ull)) : agg_hash64(k.lo);
@@ -508,10 +511,12 @@ constexpr int AGG_MIN_BLOCKS = 8;
 
 // standalone aggregate sink: one pass over a chunk.
 //  SMEM: dense table accumulated in shared memory.  slots_out (optional): pass-1-only mode
-//  (find slots, no update); slots_in (optional): pass-2 mode (slots precomputed).
+//  (find slots, no update); slots_in (optional): pass-2 mode (slots precomputed).  fail_rows (optional, hash tables): the
+//  rows the table refused, none of whose state was applied, are appended there (counted at fail_count).
 template <bool SMEM>
 __global__ void __launch_bounds__(AGG_BLOCK, AGG_MIN_BLOCKS) k_agg_push(const AggDev* __restrict__ ad, const __grid_constant__ VTab vt, int64_t n, long long* __restrict__ slots_out,
-                                                         const long long* __restrict__ slots_in) {
+                                                         const long long* __restrict__ slots_in, uint32_t* __restrict__ fail_rows,
+                                                         unsigned long long* __restrict__ fail_count) {
     extern __shared__ long long s_acc[];
     const AggDev& a = *ad;
     AccPtrs p;
@@ -541,7 +546,10 @@ __global__ void __launch_bounds__(AGG_BLOCK, AGG_MIN_BLOCKS) k_agg_push(const Ag
             slots_out[row] = slot;
             continue;
         }
-        if (slot >= 0) agg_apply_row<SMEM>(a, p, slot, ld);
+        if (slot >= 0)
+            agg_apply_row<SMEM>(a, p, slot, ld);
+        else if (fail_rows)
+            fail_rows[atomicAdd(fail_count, 1ull)] = (uint32_t)row;
     }
     if (SMEM) {
         __syncthreads();
@@ -742,12 +750,14 @@ __global__ void __launch_bounds__(256) k_agg_rehash(const AggDev* __restrict__ o
     }
 }
 
-// merge every occupied slot of `o` (finished) into `a` (AggregateFunction::merge)
-__global__ void __launch_bounds__(256) k_agg_merge(const AggDev* __restrict__ od, const AggDev* __restrict__ nd) {
+// merge every occupied slot of `o` (finished) into `a` (AggregateFunction::merge), or only the slots listed in
+// slots_in[0, total).  A slot `a` refuses applies nothing and is appended to fail_slots (counted at fail_count).
+__global__ void __launch_bounds__(256) k_agg_merge(const AggDev* __restrict__ od, const AggDev* __restrict__ nd, const unsigned long long* __restrict__ slots_in,
+                                                   unsigned long long total, unsigned long long* __restrict__ fail_slots, unsigned long long* __restrict__ fail_count) {
     const AggDev& o = *od;
     const AggDev& a = *nd;
-    const unsigned long long total = o.dense ? o.cap : o.cap + 1;
-    for (unsigned long long s = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; s < total; s += (unsigned long long)gridDim.x * blockDim.x) {
+    for (unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (unsigned long long)gridDim.x * blockDim.x) {
+        const unsigned long long s = slots_in ? slots_in[i] : i;
         const long long c = o.cnt_star[s];
         if (c == 0) continue;
         long long t;
@@ -777,6 +787,7 @@ __global__ void __launch_bounds__(256) k_agg_merge(const AggDev* __restrict__ od
             }
             if (t < 0) {
                 a.flags[0] = 1;
+                fail_slots[atomicAdd(fail_count, 1ull)] = s;
                 continue;
             }
         }
@@ -1025,7 +1036,11 @@ struct sr_agg {
     VReg reg;
     srd::AggDev host; // host mirror of the device descriptor
     DevBuf dev;       // AggDev on device
-    DevBuf hkeys, slab /* every state array, laid out by agg_state_arrays */, counters /* ngroups + flags */;
+    // counters: [0] ngroups, [1] flags, [4] / [5] the partitioned push's fail / overflow counts, [6] the fail count of
+    // agg_retry_rows and the merge
+    DevBuf hkeys, slab /* every state array, laid out by agg_state_arrays */, counters;
+    DevBuf fail_list;       // rows (or merged slots) the table refused, for agg_retry_rows and the merge
+    ColBufs retry_cols[2];  // agg_retry_rows: the refused rows gathered, alternately
     DevBuf late_accn[SR_MAX_AGG_FNS]; // accn of a function whose input turned nullable after the slab was laid out
     DevBuf slots_tmp;
     // radix-partitioned push (sr_agg_part.cuh): bucket histogram / bases / cursors, tile list, staged records, retry lists
@@ -1427,6 +1442,59 @@ static int32_t agg_check_nullability(sr_agg* a, const VTab& vt) {
 
 #include "sr_agg_part_host.cuh"
 
+static unsigned long long* agg_fail_count(sr_agg* a) { return a->counters.as<unsigned long long>() + 6; }
+
+// the rows index[0, m) of the columns `vt` reads at the kernel's own row, gathered into `bufs`: `out` reads the same
+// values at rows [0, m) (values read at a join's build row stay where they are)
+static int32_t vtab_gather(sr_ctx* ctx, const VTab& vt, const uint32_t* index, int64_t m, ColBufs* bufs, VTab* out) {
+    *out = vt;
+    srd::GatherArgs ga;
+    ga.n = 0;
+    bufs->resize(vt.n);
+    for (int k = 0; k < vt.n; k++) {
+        const VDesc& d = vt.v[k];
+        if (d.src >= 0) continue;
+        srd::GatherCol& g = ga.c[ga.n++];
+        SR_TRY(bufs->gather(ctx, k, m, d.data, d.nulls, srd::type_width(d.type), false, &g));
+        out->v[k].data = g.dst;
+        out->v[k].nulls = g.dst_nulls;
+    }
+    if (ga.n > 0) SR_TRY(launch_gather(ctx, index, m, ga));
+    vt_mark_plain32(out);
+    return SR_OK;
+}
+
+// A one-pass kernel has run over the rows of `vt`, appending the rows a full 256-slot slice refused (they applied nothing)
+// to a->fail_list, counted at agg_fail_count(a).  While there are any: grow the table so that they fit even if each is a
+// new group (a full slice refuses rows below the admission limit, so at least double: its keys then split between two
+// slices), gather them into a chunk of their own and run launch(sub_vt, rows, fail_list, fail_count) over it, which
+// refuses into the same list -- the gather has read it by then.  Leaves ngroups_host current and the flags clear.
+template <typename Launch>
+static int32_t agg_retry_rows(sr_agg* a, const VTab& vt, Launch&& launch) {
+    sr_ctx* ctx = a->ctx;
+    VTab cur = vt;
+    for (int k = 0;; k ^= 1) {
+        SR_CUDA(ctx, cudaMemcpyAsync(ctx->pinned + 8, a->counters.p, 56, cudaMemcpyDeviceToHost, ctx->stream));
+        SR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        a->ngroups_host = (int64_t)ctx->pinned[8];
+        const uint64_t failed = ctx->pinned[8 + 6];
+        if (failed == 0) {
+            if (((const int32_t*)(ctx->pinned + 9))[0]) return sr_fail(ctx, SR_ERR_STATE, "aggregate hash table overflow (internal)");
+            return SR_OK;
+        }
+        uint64_t cap = a->host.cap * 2;
+        while ((uint64_t)a->ngroups_host + failed > cap / 2) cap *= 2;
+        if (cap > (1ull << 33)) return sr_fail(ctx, SR_ERR_OUT_OF_MEMORY, "aggregate table would exceed 2^33 slots; push smaller batches");
+        SR_CUDA(ctx, cudaMemsetAsync((uint8_t*)a->counters.p + 8, 0, 8, ctx->stream)); // overflow / range flags
+        SR_TRY(agg_grow(a, cap));
+        VTab sub;
+        SR_TRY(vtab_gather(ctx, cur, a->fail_list.as<uint32_t>(), (int64_t)failed, &a->retry_cols[k], &sub));
+        cur = sub;
+        SR_CUDA(ctx, cudaMemsetAsync(agg_fail_count(a), 0, 8, ctx->stream));
+        SR_TRY(launch(cur, (int64_t)failed, a->fail_list.as<uint32_t>(), agg_fail_count(a)));
+    }
+}
+
 static int32_t agg_push_vtab(sr_agg* a, const VTab& vt, int64_t n) {
     sr_ctx* ctx = a->ctx;
     if (n <= 0) return SR_OK;
@@ -1443,9 +1511,9 @@ static int32_t agg_push_vtab(sr_agg* a, const VTab& vt, int64_t n) {
     }
     if (h.dense) {
         if (a->smem_bytes > 0) {
-            srd::k_agg_push<true><<<grid, srd::AGG_BLOCK, a->smem_bytes, ctx->stream>>>(dev, vt, n, nullptr, nullptr);
+            srd::k_agg_push<true><<<grid, srd::AGG_BLOCK, a->smem_bytes, ctx->stream>>>(dev, vt, n, nullptr, nullptr, nullptr, nullptr);
         } else {
-            srd::k_agg_push<false><<<grid, srd::AGG_BLOCK, 0, ctx->stream>>>(dev, vt, n, nullptr, nullptr);
+            srd::k_agg_push<false><<<grid, srd::AGG_BLOCK, 0, ctx->stream>>>(dev, vt, n, nullptr, nullptr, nullptr, nullptr);
         }
         SR_LAUNCH_CHECK(ctx);
         return SR_OK;
@@ -1460,32 +1528,34 @@ static int32_t agg_push_vtab(sr_agg* a, const VTab& vt, int64_t n) {
         if (!merge_fns && n >= min_rows) return agg_push_partitioned(a, vt, n, fresh);
     }
     if ((uint64_t)a->ngroups_host + (uint64_t)n <= h.limit) {
-        // cannot overflow: single fused pass
-        srd::k_agg_push<false><<<grid, srd::AGG_BLOCK, 0, ctx->stream>>>(dev, vt, n, nullptr, nullptr);
-        SR_LAUNCH_CHECK(ctx);
-    } else {
-        // two passes: find/insert slots (growing the table until every row is placed), then update
-        SR_TRY(a->slots_tmp.reserve(ctx, sizeof(int64_t) * (size_t)n));
-        while (true) {
-            srd::k_agg_push<false><<<grid, srd::AGG_BLOCK, 0, ctx->stream>>>((const srd::AggDev*)a->dev.p, vt, n, a->slots_tmp.as<long long>(), nullptr);
+        // below the admission limit: one fused pass; the rows a full slice refuses are pushed again after a growth
+        SR_TRY(a->fail_list.reserve(ctx, sizeof(uint32_t) * (size_t)n));
+        SR_CUDA(ctx, cudaMemsetAsync(agg_fail_count(a), 0, 8, ctx->stream));
+        const auto launch = [&](const VTab& v, int64_t m, uint32_t* fail_rows, unsigned long long* fail_count) -> int32_t {
+            srd::k_agg_push<false><<<std::min(grid_for(m, srd::AGG_BLOCK), ctx->num_sms * 8), srd::AGG_BLOCK, 0, ctx->stream>>>(
+                    (const srd::AggDev*)a->dev.p, v, m, nullptr, nullptr, fail_rows, fail_count);
             SR_LAUNCH_CHECK(ctx);
-            uint64_t ng;
-            int32_t ovf, bad;
-            SR_TRY(agg_read_counters(a, &ng, &ovf, &bad));
-            a->ngroups_host = (int64_t)ng;
-            if (!ovf) break;
-            SR_CUDA(ctx, cudaMemsetAsync((uint8_t*)a->counters.p + 8, 0, 8, ctx->stream));
-            SR_TRY(agg_grow(a, a->host.cap * 4));
-        }
-        srd::k_agg_push<false><<<grid, srd::AGG_BLOCK, 0, ctx->stream>>>((const srd::AggDev*)a->dev.p, vt, n, nullptr, a->slots_tmp.as<long long>());
-        SR_LAUNCH_CHECK(ctx);
-        return SR_OK;
+            return SR_OK;
+        };
+        SR_TRY(launch(vt, n, a->fail_list.as<uint32_t>(), agg_fail_count(a)));
+        return agg_retry_rows(a, vt, launch);
     }
-    uint64_t ng;
-    int32_t ovf, bad;
-    SR_TRY(agg_read_counters(a, &ng, &ovf, &bad));
-    a->ngroups_host = (int64_t)ng;
-    if (ovf) return sr_fail(ctx, SR_ERR_STATE, "aggregate hash table overflow (internal)");
+    // two passes: find/insert slots (growing the table until every row is placed), then update
+    SR_TRY(a->slots_tmp.reserve(ctx, sizeof(int64_t) * (size_t)n));
+    while (true) {
+        srd::k_agg_push<false><<<grid, srd::AGG_BLOCK, 0, ctx->stream>>>((const srd::AggDev*)a->dev.p, vt, n, a->slots_tmp.as<long long>(), nullptr, nullptr, nullptr);
+        SR_LAUNCH_CHECK(ctx);
+        uint64_t ng;
+        int32_t ovf, bad;
+        SR_TRY(agg_read_counters(a, &ng, &ovf, &bad));
+        a->ngroups_host = (int64_t)ng;
+        if (!ovf) break;
+        if (a->host.cap >= (1ull << 33)) return sr_fail(ctx, SR_ERR_OUT_OF_MEMORY, "aggregate table would exceed 2^33 slots");
+        SR_CUDA(ctx, cudaMemsetAsync((uint8_t*)a->counters.p + 8, 0, 8, ctx->stream));
+        SR_TRY(agg_grow(a, a->host.cap * 4));
+    }
+    srd::k_agg_push<false><<<grid, srd::AGG_BLOCK, 0, ctx->stream>>>((const srd::AggDev*)a->dev.p, vt, n, nullptr, a->slots_tmp.as<long long>(), nullptr, nullptr);
+    SR_LAUNCH_CHECK(ctx);
     return SR_OK;
 }
 

@@ -677,8 +677,8 @@ static int32_t frag_push(sr_fragment* f, const sr_chunk_view* fact) {
     const srd::AggDev& ah = a->host;
     const bool hash = !ah.dense && ah.num_keys > 0;
     if (hash) {
-        // Survivors are unknown before the pass.  The single-kernel cascade has no way to retry a row, so its table is
-        // made large enough for the worst case (every row a new group).  The selection-vector passes size the table
+        // Survivors are unknown before the pass.  The single-kernel cascade retries only the rows a full slice refuses, so
+        // its table is made large enough for the worst case (every row a new group).  The selection-vector passes size the table
         // from the sampled survivor estimate (x2 + slack) and re-apply the rows the table refused after growing it.
         uint64_t want = (uint64_t)n;
         if (f->selective) want = std::min<uint64_t>((uint64_t)n, (uint64_t)((double)n * std::min(1.0, f->est_rate) * 2.0) + (1u << 16));
@@ -765,20 +765,24 @@ static int32_t frag_push(sr_fragment* f, const sr_chunk_view* fact) {
         }
         return SR_OK;
     }
-    const int grid = (int)std::min<int64_t>(f->cascade_grid, (n + srd::FRAG_TILE - 1) / srd::FRAG_TILE);
-    if (f->smem_agg)
-        srd::k_fragment<true><<<grid, srd::FRAG_BLOCK, f->cascade_smem, ctx->stream>>>((const srd::FragDev*)f->dev.p, (const srd::AggDev*)a->dev.p, vt, n,
-                                                                                      f->queue_word_off);
-    else
-        srd::k_fragment<false><<<grid, srd::FRAG_BLOCK, f->cascade_smem, ctx->stream>>>((const srd::FragDev*)f->dev.p, (const srd::AggDev*)a->dev.p, vt, n,
-                                                                                       f->queue_word_off);
-    SR_LAUNCH_CHECK(ctx);
-    if (hash) {
-        uint64_t ng;
-        int32_t ovf, bad;
-        SR_TRY(agg_read_counters(a, &ng, &ovf, &bad));
-        a->ngroups_host = (int64_t)ng;
-        if (ovf) return sr_fail(ctx, SR_ERR_STATE, "aggregate hash table overflow (internal)");
-    }
-    return SR_OK;
+    // a hash table refuses a row only when its 256-slot slice is full (the table was sized for every row being a new
+    // group): the refused fact rows are gathered and run through the cascade again after a growth.  That is exact because
+    // the cascade never expands a row (a one-to-many join forces the selection-vector passes), so a refused fact row is
+    // one aggregate input that applied nothing, and the same predicates and joins pass it again.
+    const auto launch = [&](const VTab& v, int64_t m, uint32_t* fail_rows, unsigned long long* fail_count) -> int32_t {
+        const int grid = (int)std::min<int64_t>(f->cascade_grid, (m + srd::FRAG_TILE - 1) / srd::FRAG_TILE);
+        if (f->smem_agg)
+            srd::k_fragment<true><<<grid, srd::FRAG_BLOCK, f->cascade_smem, ctx->stream>>>((const srd::FragDev*)f->dev.p, (const srd::AggDev*)a->dev.p, v, m,
+                                                                                          f->queue_word_off, fail_rows, fail_count);
+        else
+            srd::k_fragment<false><<<grid, srd::FRAG_BLOCK, f->cascade_smem, ctx->stream>>>((const srd::FragDev*)f->dev.p, (const srd::AggDev*)a->dev.p, v, m,
+                                                                                           f->queue_word_off, fail_rows, fail_count);
+        SR_LAUNCH_CHECK(ctx);
+        return SR_OK;
+    };
+    if (!hash) return launch(vt, n, nullptr, nullptr);
+    SR_TRY(a->fail_list.reserve(ctx, sizeof(uint32_t) * (size_t)n));
+    SR_CUDA(ctx, cudaMemsetAsync(agg_fail_count(a), 0, 8, ctx->stream));
+    SR_TRY(launch(vt, n, a->fail_list.as<uint32_t>(), agg_fail_count(a)));
+    return agg_retry_rows(a, vt, launch);
 }

@@ -153,6 +153,8 @@ struct Cascade {
     int shared_acc; // the accumulators live in shared memory
     uint32_t lane;
     unsigned long long passed;
+    uint32_t* fail_rows; // hash aggregate: the rows a full slice refuses (they applied nothing), counted at fail_count
+    unsigned long long* fail_count;
 
     __device__ __forceinline__ void set_count(int k, uint32_t v) {
         if (lane == 0) qc[k] = v;
@@ -198,6 +200,9 @@ struct Cascade {
                     agg_apply_row<true>(ad, acc, slot, ld);
                 else
                     agg_apply_row<false>(ad, acc, slot, ld);
+            } else if (!ad.dense) {
+                fail_rows[atomicAdd(fail_count, 1ull)] = row32;
+                return; // counted in rows_passed when it is run again
             }
             passed++;
         }
@@ -252,7 +257,7 @@ struct Cascade {
 
 template <bool SMEM_AGG>
 __global__ void __launch_bounds__(FRAG_BLOCK, 2) k_fragment(const FragDev* __restrict__ fdp, const AggDev* __restrict__ adp, const __grid_constant__ VTab vt, int64_t n,
-                                                             int32_t queue_word_off) {
+                                                             int32_t queue_word_off, uint32_t* __restrict__ fail_rows, unsigned long long* __restrict__ fail_count) {
     extern __shared__ __align__(16) uint32_t smem[];
     __shared__ FragJoinDev s_joins[SR_MAX_FRAG_JOINS];
     __shared__ CPred s_preds[8];
@@ -292,7 +297,7 @@ __global__ void __launch_bounds__(FRAG_BLOCK, 2) k_fragment(const FragDev* __res
     }
 
     // queue k feeds join k+1 (k+1 < S) or the aggregate (the last queue)
-    Cascade cs{vt, ad, acc, s_joins, smem, wq, wq + (SR_MAX_FRAG_JOINS + 1) * FRAG_QCAP, S, S > 1 ? S : 1, fast1 ? 1 : 0, SMEM_AGG ? 1 : 0, lane_id(), 0ull};
+    Cascade cs{vt, ad, acc, s_joins, smem, wq, wq + (SR_MAX_FRAG_JOINS + 1) * FRAG_QCAP, S, S > 1 ? S : 1, fast1 ? 1 : 0, SMEM_AGG ? 1 : 0, lane_id(), 0ull, fail_rows, fail_count};
 
     const int64_t num_tiles = (n + FRAG_TILE - 1) / FRAG_TILE;
     const int64_t full_tiles = n / FRAG_TILE; // tiles [0, full_tiles) have every row in range

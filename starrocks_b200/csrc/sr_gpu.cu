@@ -1126,19 +1126,39 @@ int32_t sr_agg_merge(sr_agg* a, sr_agg* o) {
         SR_TRY(agg_read_counters(o, &ng_o, &ovf, &bad));
         while ((uint64_t)a->ngroups_host + ng_o > a->host.limit) SR_TRY(agg_grow(a, a->host.cap * 4));
     }
-    const uint64_t total_o = srd::agg_slots(oh);
     a->table_touched = true;
-    srd::k_agg_merge<<<std::min(grid_for((int64_t)total_o, 256), ctx->num_sms * 16), 256, 0, ctx->stream>>>((const srd::AggDev*)o->dev.p,
-                                                                                                            (const srd::AggDev*)a->dev.p);
-    SR_LAUNCH_CHECK(ctx);
-    if (hash) {
-        uint64_t ng;
-        int32_t ovf, bad;
-        SR_TRY(agg_read_counters(a, &ng, &ovf, &bad));
-        a->ngroups_host = (int64_t)ng;
-        if (ovf) return sr_fail(ctx, SR_ERR_STATE, "aggregate hash table overflow during merge (internal)");
+    // a slot of `o` that a full 256-slot slice refuses merges nothing: it is listed and merged again after a growth
+    uint64_t total = srd::agg_slots(oh);
+    const unsigned long long* slots_in = nullptr;
+    unsigned long long* fail_count = agg_fail_count(a);
+    DevBuf retry;
+    if (hash) SR_TRY(a->fail_list.reserve(ctx, sizeof(uint64_t) * (size_t)total));
+    while (true) {
+        if (hash) SR_CUDA(ctx, cudaMemsetAsync(fail_count, 0, 8, ctx->stream));
+        srd::k_agg_merge<<<std::min(grid_for((int64_t)total, 256), ctx->num_sms * 16), 256, 0, ctx->stream>>>(
+                (const srd::AggDev*)o->dev.p, (const srd::AggDev*)a->dev.p, slots_in, total, a->fail_list.as<unsigned long long>(), fail_count);
+        SR_LAUNCH_CHECK(ctx);
+        if (!hash) return SR_OK;
+        SR_CUDA(ctx, cudaMemcpyAsync(ctx->pinned + 8, a->counters.p, 56, cudaMemcpyDeviceToHost, ctx->stream));
+        SR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        a->ngroups_host = (int64_t)ctx->pinned[8];
+        const uint64_t failed = ctx->pinned[8 + 6];
+        if (failed == 0) {
+            if (((const int32_t*)(ctx->pinned + 9))[0]) return sr_fail(ctx, SR_ERR_STATE, "aggregate hash table overflow during merge (internal)");
+            return SR_OK;
+        }
+        // at least doubled: the refused keys of a full slice then split between two slices
+        uint64_t cap = a->host.cap * 2;
+        while ((uint64_t)a->ngroups_host + failed > cap / 2) cap *= 2;
+        if (cap > (1ull << 33)) return sr_fail(ctx, SR_ERR_OUT_OF_MEMORY, "aggregate table would exceed 2^33 slots");
+        SR_CUDA(ctx, cudaMemsetAsync((uint8_t*)a->counters.p + 8, 0, 8, ctx->stream)); // overflow / range flags
+        SR_TRY(agg_grow(a, cap));
+        // the refused slots become the input, the old input list takes the next refusals
+        SR_TRY(retry.reserve(ctx, sizeof(uint64_t) * (size_t)failed));
+        std::swap(a->fail_list, retry);
+        slots_in = retry.as<unsigned long long>();
+        total = failed;
     }
-    return SR_OK;
 }
 
 // ------------------------------------------------------------------ fragment
