@@ -625,7 +625,8 @@ typedef struct sr_frag_join {
 } sr_frag_join;
 
 typedef struct sr_fragment_desc {
-    sr_scan_desc scan; /* preds / filter_exprs on fact columns; out_slots ignored */
+    sr_scan_desc scan; /* preds / filter_exprs on fact columns; out_slots ignored.  They name fact slots only: one that
+                        * names a join's payload slot makes the first sr_fragment_push fail with SR_ERR_NOT_SUPPORTED */
     int32_t num_joins;
     /* execution mode: 0 = decide from the pass rates sampled on the first batch, 1 = single fused kernel
      * (warp-queue cascade), 2 = selection-vector passes (stream -> gather -> aggregate).  Both modes give

@@ -1209,6 +1209,14 @@ static int32_t agg_setup_tables(sr_agg* a, uint64_t cap) {
     return SR_OK;
 }
 
+// SUM / MIN / MAX: the state follows the compiled expression's class, the result type follows input_type, so the two
+// must agree (a DOUBLE state read back as an integer result, or the reverse, would hand out its bit pattern)
+static int32_t agg_check_input_class(sr_ctx* ctx, int f, bool dbl, int32_t input_type) {
+    if (!dbl && srd::is_float_class(input_type)) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "fn %d: input_type is floating but the expression is integer", f);
+    if (dbl && !srd::is_float_class(input_type)) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "fn %d: input_type is integer but the expression is double", f);
+    return SR_OK;
+}
+
 typedef int32_t (*agg_type_fn)(void* user, int32_t slot);
 typedef bool (*agg_nullable_fn)(void* user, int32_t slot);
 
@@ -1262,10 +1270,12 @@ static int32_t agg_compile(sr_agg* a, slot_type_fn tf, agg_nullable_fn nf, void*
         }
         SR_TRY(compile_expr(ctx, &fn.input, &a->reg, tf, user, &fd.input));
         fd.in_is_double = fd.input.result_is_double;
-        // is any input column of the expression nullable?
+        // can the expression be NULL: a nullable input column, or a division (a zero divisor gives NULL)?
         bool nullable_in = false;
-        for (int k = 0; k < fn.input.num_nodes; k++)
+        for (int k = 0; k < fn.input.num_nodes; k++) {
             if (fn.input.nodes[k].op == SR_EX_COL) nullable_in |= nf(user, fn.input.nodes[k].slot_id);
+            if (fn.input.nodes[k].op == SR_EX_DIV) nullable_in = true;
+        }
         fd.track_n = nullable_in ? 1 : 0;
         const bool dbl = fd.in_is_double != 0;
         switch (fn.kind) {
@@ -1279,8 +1289,7 @@ static int32_t agg_compile(sr_agg* a, slot_type_fn tf, agg_nullable_fn nf, void*
                 fd.mode = srd::M_SUM_F64;
             else
                 fd.mode = (fd.result_type == SR_TYPE_DECIMAL128 || fd.result_type == SR_TYPE_LARGEINT) ? srd::M_SUM_I128 : srd::M_SUM_I64;
-            if (!dbl && srd::is_float_class(fn.input_type)) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "fn %d: input_type is floating but the expression is integer", f);
-            if (dbl && !srd::is_float_class(fn.input_type)) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "fn %d: input_type is integer but the expression is double", f);
+            SR_TRY(agg_check_input_class(ctx, f, dbl, fn.input_type));
             break;
         case SR_AGG_AVG:
             fd.mode = srd::M_AVG;
@@ -1306,9 +1315,11 @@ static int32_t agg_compile(sr_agg* a, slot_type_fn tf, agg_nullable_fn nf, void*
         }
         case SR_AGG_MIN:
             fd.mode = dbl ? srd::M_MIN_F64 : srd::M_MIN_I64;
+            SR_TRY(agg_check_input_class(ctx, f, dbl, fn.input_type));
             break;
         default:
             fd.mode = dbl ? srd::M_MAX_F64 : srd::M_MAX_I64;
+            SR_TRY(agg_check_input_class(ctx, f, dbl, fn.input_type));
             break;
         }
     }

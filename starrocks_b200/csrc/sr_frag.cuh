@@ -158,6 +158,15 @@ static int32_t frag_compile(sr_fragment* f) {
         SR_TRY(compile_expr(ctx, &f->exprs[k], &f->reg, frag_slot_type, &tc, &h.exprs[k]));
         if (h.exprs[k].result_is_double) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "filter expression %zu is not boolean", k);
     }
+    // the scan conjuncts run on fact rows ahead of every join, so each value they read must be a fact column: a join
+    // payload would be indexed by fact row.  Refused before the aggregate compiles, which sets up and clears its tables
+    for (size_t k = 0; k < f->reg.slots.size(); k++) {
+        if (f->staged.find(f->reg.slots[k]) >= 0) continue;
+        const FragPayload pl = frag_find_payload(f, f->reg.slots[k]);
+        if (pl.join >= 0)
+            return sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "scan conjunct reads slot %d, a payload of join %d: scan predicates and filter expressions name fact slots only",
+                           f->reg.slots[k], pl.join);
+    }
     h.num_preds = (int32_t)f->preds.size();
     h.num_exprs = (int32_t)f->exprs.size();
     h.num_joins = f->num_joins;
