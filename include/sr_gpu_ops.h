@@ -728,7 +728,8 @@ int32_t sr_xchg_hash(sr_xchg* x, const sr_chunk_view* in, uint32_t* hash_values,
  * and, for every fixed-width type (widths 1, 2, 4, 8 and 16: BOOLEAN ... LARGEINT, FLOAT, DOUBLE, DECIMAL128 -- the decode
  * moves bytes and does no arithmetic), the default encoding of those columns:
  *   BitShufflePageDecoder::next_batch        be/src/storage/rowset/bitshuffle_page.h (bitshuffle + LZ4 blocks)
- *   For BIT_SHUFFLE, `out` must be aligned to the value width (8 bytes for 16-byte values).
+ * For every encoding `out` must be aligned to the value width (8 bytes for 16-byte values), as any device column is
+ * (sr_col_view): SR_ERR_INVALID_ARGUMENT before anything is copied or launched otherwise.
  * `pages`: the BODIES of consecutive data pages of one column (after the page's checksum / null-map handling of
  * page_io.cpp), all in `mem`: SR_MEM_DEVICE, SR_MEM_HOST_PINNED (page-locked mapped memory, e.g. a registered page cache:
  * read in place over PCIe, the decode is the transfer) or SR_MEM_HOST (pageable: staged page by page).  The values of page
@@ -739,8 +740,7 @@ int32_t sr_xchg_hash(sr_xchg* x, const sr_chunk_view* in, uint32_t* hash_values,
  *   A data page is a 4-byte little-endian mode word (EncodingTypePB) and, with mode 5 (DICT_ENCODING), a BIT_SHUFFLE page
  *   of int32 codes.  Code k is stored as values[k] of the last sr_page_decoder_set_dict (SR_ERR_STATE when there is
  *   none); a code >= num_words is a corrupt page.  Mode 2 (PLAIN_ENCODING: the dictionary overflowed and the column
- *   fell back to plain string pages) gives SR_ERR_NOT_SUPPORTED when no page of the call is malformed.  `out` must be
- *   4-byte aligned.
+ *   fell back to plain string pages) gives SR_ERR_NOT_SUPPORTED when no page of the call is malformed.
  * SR_ERR_INVALID_ARGUMENT for a page that is not well formed (sizes, frame table, bit widths, the bitshuffle header, block
  * chain or LZ4 streams, the dictionary mode word or codes).  Asynchronous on the context stream except for one small
  * read-back of the per-page counts and, for FOR, BIT_SHUFFLE and DICT, one of the error flag at the end.  RLE pages and

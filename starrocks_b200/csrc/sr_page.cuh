@@ -63,6 +63,9 @@ __device__ __forceinline__ uint32_t page_le32(const uint8_t* p) {
 constexpr int BSHUF_BLOCK_BYTES = 8192;     // bshuf_default_block_size(s) * s for every width s in 1..16
 constexpr uint32_t BSHUF_MAX_STREAM = 8240; // LZ4_compressBound(8192)
 
+// the frames of a frame-of-reference page of n values, in 64 bits: n + 127 wraps a uint32 count from 2^32 - 127 on
+__device__ __forceinline__ unsigned long long for_frame_count(unsigned long long n) { return (n + 127) / 128; }
+
 // value count and frame (bitshuffle: block) count of every page; flags[0] |= 1 when a page cannot be a page of `encoding`,
 // |= 2 for a dictionary-column page in plain mode (the column's dictionary overflowed: a page of strings, not codes)
 __global__ void __launch_bounds__(256) k_page_footers(const PageDesc* __restrict__ pages, int32_t num_pages, int32_t encoding, int32_t elem_size,
@@ -102,7 +105,7 @@ __global__ void __launch_bounds__(256) k_page_footers(const PageDesc* __restrict
             const uint32_t fsz = pg.data[pg.size - 5];
             n = page_le32(pg.data + pg.size - 4);
             if (fsz != 128 && n != 0) bad = true; // every writer uses ForEncoder::FRAME_VALUE_NUM = 128
-            frames = (n + 127) / 128;
+            frames = for_frame_count(n);
             if (pg.size - 5 - (long long)frames * 2 < 0) bad = true;
         }
     }
@@ -124,7 +127,7 @@ __global__ void __launch_bounds__(FOR_FRAMES_BLOCK) k_for_frames(const PageDesc*
     const PageDesc pg = pages[blockIdx.x];
     if (pg.size < 5) return;
     const uint32_t n = page_le32(pg.data + pg.size - 4);
-    const uint32_t nf = (n + 127) / 128;
+    const uint32_t nf = (uint32_t)for_frame_count(n); // <= 2^25
     const long long meta = pg.size - 5 - (long long)nf * 2;
     if (meta < 0) return;
     if (threadIdx.x == 0) s_base = 0;
@@ -503,14 +506,15 @@ static int32_t pages_decode(sr_ctx* ctx, PageScratch* sc, int32_t encoding, int3
     if (encoding == SR_PAGE_DICT) {
         if (type != SR_TYPE_INT) return sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "dictionary page decode of type %d (TYPE_INT ids)", type);
         if (dict_words < 0) return sr_fail(ctx, SR_ERR_STATE, "dictionary pages decoded before sr_page_decoder_set_dict");
-        if ((uintptr_t)out % 4) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "output column not aligned to 4 bytes");
     } else if (encoding == SR_PAGE_BITSHUFFLE) {
         if (w == 0) return sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "bitshuffle page decode of type %d (fixed-width types)", type);
-        if ((uintptr_t)out % std::min(w, 8)) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "output column not aligned to %d bytes", std::min(w, 8));
     } else {
         if ((w != 4 && w != 8) || srd::is_float_class(type)) return sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "page decode of type %d (4- and 8-byte integer-class types)", type);
         if (encoding != SR_PAGE_PLAIN && encoding != SR_PAGE_FOR) return sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "page encoding %d", encoding);
     }
+    // one rule for every encoding: k_for_decode and the bitshuffle kernels store whole values where a lane's address is not
+    // vector-aligned, so a column off its natural alignment would be a misaligned store (plain pages follow the same rule)
+    if ((uintptr_t)out % std::min(w, 8)) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "output column not aligned to %d bytes", std::min(w, 8));
     if (num_pages < 0 || (num_pages > 0 && !pv)) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "pages");
     SR_TRY(mem_check(ctx, mem, "pages"));
     *out_rows = 0;
