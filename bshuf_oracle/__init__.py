@@ -1,4 +1,5 @@
-"""ctypes binding of the BIT_SHUFFLE page codec restated on the CPU (bshuf_oracle/bshuf_oracle.cpp).  TEST INFRASTRUCTURE ONLY.
+"""ctypes binding of the BIT_SHUFFLE page codec, the RLE codec at bit width 1 (BOOLEAN pages, RLE null maps) and the
+null maps of data pages, restated on the CPU (bshuf_oracle/bshuf_oracle.cpp).  TEST INFRASTRUCTURE ONLY.
 
 Only tests/, scripts/ and tools/ import this package: it writes the pages the device decoder is checked and measured
 against, and decodes them the way the reference does.  The product package (starrocks_b200) never imports it.
@@ -62,7 +63,8 @@ def lib():
         i32, i64, vp = C.c_int32, C.c_int64, C.c_void_p
         for name, res, args in (("bso_lz4_compress", i64, [vp, i64, vp, i64]), ("bso_lz4_decompress", i64, [vp, i64, vp, i64]),
                                 ("bso_trans_bit_elem", None, [vp, vp, i64, i32]), ("bso_untrans_bit_elem", None, [vp, vp, i64, i32]),
-                                ("bso_bshuf_encode", i64, [i32, vp, i64, vp, i64]), ("bso_bshuf_decode", i64, [i32, vp, i64, vp, i64])):
+                                ("bso_bshuf_encode", i64, [i32, vp, i64, vp, i64]), ("bso_bshuf_decode", i64, [i32, vp, i64, vp, i64]),
+                                ("bso_rle_encode", i64, [vp, i64, vp, i64]), ("bso_rle_decode", i64, [vp, i64, i64, vp])):
             getattr(L, name).restype = res
             getattr(L, name).argtypes = args
         _LIB = L
@@ -201,6 +203,68 @@ def binary_plain_page_decode(page):
     if any(a > b for a, b in zip(offs, offs[1:])):
         raise CorruptPage("word offsets")
     return [p[offs[i]:offs[i + 1]] for i in range(n)]
+
+
+# ---- RLE at bit width 1 (RleEncoder / RleDecoder, be/src/util/rle_encoding.h): BOOLEAN pages and RLE_NULL null maps ----
+NULL_BITSHUFFLE, NULL_RLE = 0, 1                # NullEncodingPB: BITSHUFFLE_NULL, RLE_NULL
+
+
+def rle_encode(values):
+    """RleEncoder stream of 0 / 1 values at bit width 1 (nonzero counts as 1)"""
+    v = np.ascontiguousarray(values, dtype=np.uint8)
+    cap = 2 * len(v) // 8 + 16                  # literal runs: 64 bytes per 63 groups; repeated runs: <= 6 bytes per >= 8 values
+    out = np.zeros(cap, dtype=np.uint8)
+    r = lib().bso_rle_encode(_ptr(v), len(v), out.ctypes.data, cap)
+    assert r >= 0
+    return out[:r]
+
+
+def rle_decode(stream, n):
+    """the first n values of an RLE stream at bit width 1 (uint8 0 / 1); CorruptPage for what RleDecoder cannot decode"""
+    s = np.ascontiguousarray(stream, dtype=np.uint8)
+    out = np.zeros(max(n, 1), dtype=np.uint8)
+    if lib().bso_rle_decode(_ptr(s), len(s), n, out.ctypes.data) != 0:
+        raise CorruptPage("RLE stream")
+    return out[:n]
+
+
+def rle_bool_page_encode(values):
+    """RLE page body of a BOOLEAN column (RlePageBuilder::finish): the uint32 LE value count, then the RLE stream"""
+    v = np.ascontiguousarray(values, dtype=np.uint8)
+    return np.concatenate([np.array([len(v)], dtype="<u4").view(np.uint8), rle_encode(v)])
+
+
+def rle_bool_page_decode(page):
+    p = np.ascontiguousarray(page, dtype=np.uint8)
+    if len(p) < 4:
+        raise CorruptPage("RLE page shorter than its count")
+    return rle_decode(p[4:], int(np.frombuffer(p[:4].tobytes(), dtype="<u4")[0]))
+
+
+def null_map_encode(flags, encoding):
+    """the null map of a data page whose rows carry `flags` (nonzero = NULL) -- empty when no row is NULL (the writer then
+    stores no map): bitshuffle::compress_lz4 of the flags padded to 8 (a BIT_SHUFFLE page of bytes without its 16-byte
+    header), or the RleEncoder stream"""
+    f = (np.ascontiguousarray(flags) != 0).astype(np.uint8)
+    if not f.any():
+        return np.zeros(0, dtype=np.uint8)
+    if encoding == NULL_RLE:
+        return rle_encode(f)
+    assert encoding == NULL_BITSHUFFLE
+    return bitshuffle_encode(f)[16:]
+
+
+def null_map_decode(nmap, num_rows, encoding):
+    """-> num_rows uint8 flags; an empty map is a page without NULLs.  CorruptPage for a malformed map"""
+    m = np.ascontiguousarray(nmap, dtype=np.uint8)
+    if len(m) == 0:
+        return np.zeros(num_rows, dtype=np.uint8)
+    if encoding == NULL_RLE:
+        return rle_decode(m, num_rows)
+    assert encoding == NULL_BITSHUFFLE
+    padded = (num_rows + 7) // 8 * 8
+    hdr = np.array([num_rows, 16 + len(m), padded, 1], dtype="<u4").view(np.uint8)
+    return bitshuffle_decode(np.concatenate([hdr, m]), 1)
 
 
 def system_lz4():

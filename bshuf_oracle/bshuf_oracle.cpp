@@ -25,6 +25,7 @@
 //   stream (never produced by an LZ4 compressor) is rejected here and on the device.
 #include <cstdint>
 #include <cstring>
+#include <algorithm>
 #include <vector>
 
 namespace {
@@ -165,9 +166,130 @@ void put_le32(uint8_t* p, uint32_t v) {
     for (int k = 0; k < 4; k++) p[k] = (uint8_t)(v >> (8 * k));
 }
 
+// RleEncoder<T> at bit width 1 (be/src/util/rle_encoding.h, the Kudu / Impala hybrid encoder): values are buffered in
+// groups of 8; 8 equal values in a row turn into a repeated run (ULEB128 header count << 1, then the value in one byte) that
+// lasts until the value changes; other groups go out bit-packed (one byte per group, least significant bit first) under a
+// one-byte header (groups << 1 | 1) reserved in front of them, a new one once 63 groups are written.  Flush writes what is
+// pending as a repeated run when it is all one value, else as a last literal group padded with zeros.
+struct RleEncoder1 {
+    std::vector<uint8_t> out;
+    uint8_t buf[8] = {0};
+    int nbuf = 0;
+    int64_t literal_count = 0, indicator = -1, repeat = 0;
+    uint8_t cur = 0;
+
+    void put_vlq(uint64_t v) {
+        while (v >= 0x80) {
+            out.push_back((uint8_t)(v | 0x80));
+            v >>= 7;
+        }
+        out.push_back((uint8_t)v);
+    }
+    void flush_literal(bool update) {
+        if (indicator < 0) {
+            indicator = (int64_t)out.size();
+            out.push_back(0);
+        }
+        if (nbuf > 0) {
+            uint8_t b = 0;
+            for (int i = 0; i < nbuf; i++) b |= (uint8_t)(buf[i] << i);
+            out.push_back(b);
+        }
+        nbuf = 0;
+        if (update) {
+            out[(size_t)indicator] = (uint8_t)(((literal_count + 7) / 8) << 1 | 1);
+            indicator = -1;
+            literal_count = 0;
+        }
+    }
+    void flush_repeated() {
+        put_vlq((uint64_t)repeat << 1);
+        out.push_back(cur);
+        nbuf = 0;
+        repeat = 0;
+    }
+    void flush_buffered() {
+        if (repeat >= 8) { // the buffered values belong to the repeated run
+            nbuf = 0;
+            if (literal_count != 0) flush_literal(true);
+            return;
+        }
+        literal_count += nbuf;
+        flush_literal((literal_count + 7) / 8 + 1 >= (1 << 6));
+        repeat = 0;
+    }
+    void put(uint8_t v) {
+        if (v == cur) {
+            if (++repeat > 8) return;
+        } else {
+            if (repeat >= 8) flush_repeated();
+            repeat = 1;
+            cur = v;
+        }
+        buf[nbuf] = v;
+        if (++nbuf == 8) flush_buffered();
+    }
+    void flush() {
+        if (literal_count > 0 || repeat > 0 || nbuf > 0) {
+            const bool all_repeat = literal_count == 0 && (repeat == nbuf || nbuf == 0);
+            if (repeat > 0 && all_repeat) {
+                flush_repeated();
+            } else {
+                literal_count += nbuf;
+                flush_literal(true);
+                repeat = 0;
+            }
+        }
+    }
+};
+
+// n values of an RLE stream at bit width 1 -> out; false for a malformed stream.  Stops at the count (RleDecoder reads
+// no further): refuses a header longer than 5 bytes or cut off, a zero-length run, a repeated value other than 0 / 1, a
+// run whose values up to the count lie past the end, and a stream that ends before the count.
+bool rle_decode1(const uint8_t* in, int64_t len, int64_t n, uint8_t* out) {
+    int64_t pos = 0, done = 0;
+    while (done < n) {
+        uint64_t h = 0;
+        bool more = true;
+        for (int hb = 0; hb < 5 && more && pos < len; hb++) {
+            const uint8_t c = in[pos++];
+            h |= (uint64_t)(c & 0x7F) << (7 * hb);
+            more = (c & 0x80) != 0;
+        }
+        const int64_t cnt = (int64_t)(h >> 1);
+        if (more || cnt == 0) return false;
+        if (h & 1) {
+            const int64_t take = std::min<int64_t>(8 * cnt, n - done);
+            if (pos + (take + 7) / 8 > len) return false;
+            for (int64_t i = 0; i < take; i++) out[done + i] = (in[pos + i / 8] >> (i % 8)) & 1;
+            pos += cnt;
+            done += take;
+        } else {
+            if (pos >= len || in[pos] > 1) return false;
+            const int64_t take = std::min<int64_t>(cnt, n - done);
+            memset(out + done, in[pos++], (size_t)take);
+            done += take;
+        }
+    }
+    return true;
+}
+
 } // namespace
 
 extern "C" {
+
+// n values (0 / 1) -> an RLE stream at bit width 1; -> its size, or -(bytes needed) when cap is too small
+int64_t bso_rle_encode(const uint8_t* values, int64_t n, uint8_t* out, int64_t cap) {
+    RleEncoder1 e;
+    for (int64_t i = 0; i < n; i++) e.put(values[i] ? 1 : 0);
+    e.flush();
+    if ((int64_t)e.out.size() > cap) return -(int64_t)e.out.size();
+    if (!e.out.empty()) memcpy(out, e.out.data(), e.out.size());
+    return (int64_t)e.out.size();
+}
+
+// the first n values of an RLE stream -> out; 0, or -1 for a malformed stream
+int64_t bso_rle_decode(const uint8_t* in, int64_t len, int64_t n, uint8_t* out) { return rle_decode1(in, len, n, out) ? 0 : -1; }
 
 // LZ4 block compress: -> compressed size, or -(bytes needed) when cap is too small
 int64_t bso_lz4_compress(const uint8_t* src, int64_t n, uint8_t* dst, int64_t cap) {

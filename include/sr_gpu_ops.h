@@ -730,8 +730,8 @@ int32_t sr_xchg_hash(sr_xchg* x, const sr_chunk_view* in, uint32_t* hash_values,
  *   BitShufflePageDecoder::next_batch        be/src/storage/rowset/bitshuffle_page.h (bitshuffle + LZ4 blocks)
  * For every encoding `out` must be aligned to the value width (8 bytes for 16-byte values), as any device column is
  * (sr_col_view): SR_ERR_INVALID_ARGUMENT before anything is copied or launched otherwise.
- * `pages`: the BODIES of consecutive data pages of one column (after the page's checksum / null-map handling of
- * page_io.cpp), all in `mem`: SR_MEM_DEVICE, SR_MEM_HOST_PINNED (page-locked mapped memory, e.g. a registered page cache:
+ * `pages`: the BODIES of consecutive data pages of one column (after the page's checksum handling of page_io.cpp, without
+ * the null map a nullable column's page ends with: sr_null_maps_decode), all in `mem`: SR_MEM_DEVICE, SR_MEM_HOST_PINNED (page-locked mapped memory, e.g. a registered page cache:
  * read in place over PCIe, the decode is the transfer) or SR_MEM_HOST (pageable: staged page by page).  The values of page
  * k follow those of page k - 1 in `out` (device memory, room for out_capacity values); *out_rows receives the total.
  * And, for TYPE_INT only, the data pages of a dictionary-encoded (DICT_ENCODING: CHAR / VARCHAR) column, decoded
@@ -743,13 +743,21 @@ int32_t sr_xchg_hash(sr_xchg* x, const sr_chunk_view* in, uint32_t* hash_values,
  *   fell back to plain string pages) gives SR_ERR_NOT_SUPPORTED when no page of the call is malformed.
  * SR_ERR_INVALID_ARGUMENT for a page that is not well formed (sizes, frame table, bit widths, the bitshuffle header, block
  * chain or LZ4 streams, the dictionary mode word or codes).  Asynchronous on the context stream except for one small
- * read-back of the per-page counts and, for FOR, BIT_SHUFFLE and DICT, one of the error flag at the end.  RLE pages and
- * plain-mode string pages are not covered: SR_ERR_NOT_SUPPORTED. */
+ * read-back of the per-page counts and, for FOR, BIT_SHUFFLE, DICT and RLE, one of the error flag at the end.
+ * And, for BOOLEAN only, RLE pages (the default encoding of BOOLEAN columns):
+ *   RlePageDecoder::next_batch               be/src/storage/rowset/rle_page.h (RlePageBuilder::finish writes the page)
+ *   A page is a little-endian uint32 value count, then an RleEncoder stream (be/src/util/rle_encoding.h) at bit width 1:
+ *   runs, each a ULEB128 header of at most 5 bytes h -- h & 1: (h >> 1) groups of 8 bit-packed values, one byte each, least
+ *   significant bit first; else (h >> 1) copies of the value in the next byte.  The decode stops at the count: values
+ *   and bytes past it are never read.  A header longer than 5 bytes or cut off, a run of length 0, a repeated value other
+ *   than 0 / 1, values up to the count past the page's end, or a stream that ends before the count is a malformed page.
+ * Other types with SR_PAGE_RLE, and plain-mode string pages, are not covered: SR_ERR_NOT_SUPPORTED. */
 typedef enum sr_page_encoding {
     SR_PAGE_PLAIN = 0,      /* EncodingTypePB::PLAIN_ENCODING */
     SR_PAGE_FOR = 1,        /* EncodingTypePB::FOR_ENCODING */
     SR_PAGE_BITSHUFFLE = 2, /* EncodingTypePB::BIT_SHUFFLE */
-    SR_PAGE_DICT = 3        /* EncodingTypePB::DICT_ENCODING */
+    SR_PAGE_DICT = 3,       /* EncodingTypePB::DICT_ENCODING */
+    SR_PAGE_RLE = 4         /* EncodingTypePB::RLE (SR_TYPE_BOOLEAN) */
 } sr_page_encoding;
 
 typedef struct sr_page_view {
@@ -769,6 +777,37 @@ int32_t sr_pages_decode(sr_page_decoder* dec, int32_t encoding, int32_t type, co
  * when the call returns (it synchronises the context stream).  A later call replaces the table: one table per segment, so
  * a caller decoding several segments into one column sets each segment's table and advances `out`. */
 int32_t sr_page_decoder_set_dict(sr_page_decoder* dec, const int32_t* values, int64_t num_words, int32_t mem);
+
+/* The null maps of a nullable column's data pages (page format 2: a page stores a value for every row, NULL rows included,
+ * and its body is `values | null map`, DataPageFooterPB.nullmap_size giving the map's length) decoded on the device into
+ * the uint8 null column (1 = NULL) that goes with the values sr_pages_decode makes of the same pages:
+ *   ParsedPage / PageDecoder null handling   be/src/storage/rowset/parsed_page.cpp, page_io.cpp
+ * One view per data page, in page order: the map's bytes and the page's num_values (footer).  size == 0: the page holds
+ * no NULL (the writer omits the map) and its rows get 0.  Page k's flags follow page k - 1's in out_nulls (device memory,
+ * room for out_capacity flags, any alignment), as sr_pages_decode places the values.
+ *   SR_NULL_BITSHUFFLE (NullEncodingPB::BITSHUFFLE_NULL): bitshuffle::compress_lz4 of the flags zero-padded to
+ *     ALIGN_UP(num_rows, 8), 1-byte elements -- the block chain of a BIT_SHUFFLE page without its 16-byte header, ending
+ *     exactly at `size`.
+ *   SR_NULL_RLE (NullEncodingPB::RLE_NULL): the RleEncoder stream at bit width 1 described at SR_PAGE_RLE, num_rows values.
+ * *out_rows: the rows of all pages; *out_null_count: the nonzero flags among them -- 0 lets the caller pass the batch with
+ * nulls = NULL (sr_col_view), which keeps the scan and fragment kernels on their paths for columns without NULLs.
+ * SR_ERR_NOT_SUPPORTED for another encoding; SR_ERR_INVALID_ARGUMENT for a negative size or row count, a row count past
+ * 2^32 - 1, missing data or more rows than out_capacity (before anything is copied or launched), and for a malformed map
+ * (after the read-back; nothing is written past the pages' rows).  Asynchronous on the context stream except for that one
+ * read-back of the error flag and the count. */
+typedef enum sr_null_encoding {
+    SR_NULL_BITSHUFFLE = 0, /* NullEncodingPB::BITSHUFFLE_NULL */
+    SR_NULL_RLE = 1         /* NullEncodingPB::RLE_NULL */
+} sr_null_encoding;
+
+typedef struct sr_null_map_view {
+    const void* data; /* the map's bytes in `mem` (sr_pages_decode's memory kinds) */
+    int64_t size;     /* DataPageFooterPB.nullmap_size; 0: no NULL in the page */
+    int64_t num_rows; /* the page's num_values */
+} sr_null_map_view;
+
+int32_t sr_null_maps_decode(sr_page_decoder* dec, int32_t null_encoding, const sr_null_map_view* maps, int32_t num_pages, int32_t mem, uint8_t* out_nulls,
+                            int64_t out_capacity, int64_t* out_rows, int64_t* out_null_count);
 
 /* ---------------------------------------------------------------------------------------
  * exchange wire format (SURVEY.md 8f-3): the bytes of ChunkPB.data as ProtobufChunkSerde::serialize_without_meta writes
@@ -822,7 +861,7 @@ int32_t sr_gather(sr_ctx* ctx, const void* src, int32_t type, const uint32_t* in
  * verify its own struct layouts at load time.  which: 0 sr_col_view, 1 sr_chunk_view,
  * 2 sr_chunk_out, 3 sr_pred, 4 sr_expr, 5 sr_scan_desc, 6 sr_join_desc, 7 sr_join_info,
  * 8 sr_agg_fn, 9 sr_agg_desc, 10 sr_frag_join, 11 sr_fragment_desc, 12 sr_part_desc, 13 sr_agg_state_array,
- * 14 sr_fragment_plan, 15 sr_rf_info.
+ * 14 sr_fragment_plan, 15 sr_rf_info, 16 sr_null_map_view.
  * returns -1 for an unknown index. */
 int32_t sr_abi_sizeof(int32_t which);
 

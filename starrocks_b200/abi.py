@@ -120,11 +120,16 @@ class sr_join_desc(C.Structure):
                 ("other_conjunct", sr_expr)]
 
 
-PAGE_PLAIN, PAGE_FOR, PAGE_BITSHUFFLE, PAGE_DICT = 0, 1, 2, 3
+PAGE_PLAIN, PAGE_FOR, PAGE_BITSHUFFLE, PAGE_DICT, PAGE_RLE = 0, 1, 2, 3, 4
+NULL_BITSHUFFLE, NULL_RLE = 0, 1
 
 
 class sr_page_view(C.Structure):
     _fields_ = [("data", C.c_void_p), ("size", C.c_int64)]
+
+
+class sr_null_map_view(C.Structure):
+    _fields_ = [("data", C.c_void_p), ("size", C.c_int64), ("num_rows", C.c_int64)]
 
 
 class sr_chunk_pb_meta(C.Structure):

@@ -1463,6 +1463,8 @@ int32_t sr_abi_sizeof(int32_t which) {
         return (int32_t)sizeof(sr_fragment_plan);
     case 15:
         return (int32_t)sizeof(sr_rf_info);
+    case 16:
+        return (int32_t)sizeof(sr_null_map_view);
     default:
         return -1;
     }
@@ -1553,6 +1555,13 @@ int32_t sr_pages_decode(sr_page_decoder* d, int32_t encoding, int32_t type, cons
     if (!d || !out_rows) return SR_ERR_INVALID_ARGUMENT;
     SR_BIND(d->ctx);
     return pages_decode(d->ctx, &d->scratch, encoding, type, pages, num_pages, mem, out, out_capacity, out_rows, (const int32_t*)d->dict.p, d->dict_words);
+}
+
+int32_t sr_null_maps_decode(sr_page_decoder* d, int32_t null_encoding, const sr_null_map_view* maps, int32_t num_pages, int32_t mem, uint8_t* out_nulls,
+                            int64_t out_capacity, int64_t* out_rows, int64_t* out_null_count) {
+    if (!d || !out_rows || !out_null_count) return SR_ERR_INVALID_ARGUMENT;
+    SR_BIND(d->ctx);
+    return null_maps_decode(d->ctx, &d->scratch, null_encoding, maps, num_pages, mem, out_nulls, out_capacity, out_rows, out_null_count);
 }
 
 int32_t sr_page_decoder_set_dict(sr_page_decoder* d, const int32_t* values, int64_t num_words, int32_t mem) {

@@ -37,6 +37,14 @@
 // in the segment's dictionary page.  k_page_footers checks the mode word and the embedded header, the host moves the page
 // descriptors past the mode word, and k_bshuf_decode_dict is k_bshuf_decode<4> with the store translating every code
 // through the decoder's table (sr_page_decoder_set_dict): the id column comes out in HBM.
+//
+//   RlePageDecoder               be/src/storage/rowset/rle_page.h; RleDecoder, be/src/util/rle_encoding.h
+// A BOOLEAN RLE page: a uint32 value count, then an RLE stream at bit width 1 (ULEB128 run headers: bit-packed groups of 8
+// or a repeated byte).  The null map of a nullable column's data page (page format 2) is that stream without the count
+// (RLE_NULL) or a BIT_SHUFFLE page of one-byte flags without its header (BITSHUFFLE_NULL); the row count comes from the
+// page footer.  k_rle_runs walks every page's run headers into descriptors, k_rle_expand writes the flags one aligned
+// 64-bit word per thread; bitshuffle maps reuse k_bshuf_blocks / k_bshuf_decode<1>, then k_null_zero_count zeroes the pages
+// without a map and counts the NULLs.
 #pragma once
 
 namespace srd {
@@ -97,6 +105,14 @@ __global__ void __launch_bounds__(256) k_page_footers(const PageDesc* __restrict
             const unsigned long long padded = page_le32(b + 8), blk = BSHUF_BLOCK_BYTES / elem_size;
             if (page_le32(b + 4) != (unsigned long long)size || padded != ((n + 7) & ~7ull) || page_le32(b + 12) != (uint32_t)elem_size) bad = true;
             frames = (padded + blk - 1) / blk; // blocks
+        }
+    } else if (encoding == SR_PAGE_RLE) {
+        // a uint32 value count, then the RLE stream; frames: the most runs the stream can hold (each takes >= 2 bytes)
+        if (pg.size < 4) {
+            bad = true;
+        } else {
+            n = page_le32(pg.data);
+            frames = min(n, (unsigned long long)(pg.size - 4) / 2);
         }
     } else {
         if (pg.size < 5) {
@@ -281,18 +297,20 @@ __device__ __forceinline__ uint32_t page_be32(const uint8_t* p) {
     return (uint32_t)p[0] << 24 | (uint32_t)p[1] << 16 | (uint32_t)p[2] << 8 | (uint32_t)p[3];
 }
 
-// one thread per page (headers already checked by k_page_footers): the chain of big-endian block lengths -> descriptors at
-// the page's frame_off.  A chain that overruns the page, claims more than 8240 bytes for a block or does not end at
-// compressed_size raises the flag; blocks from the first bad length on are skipped.
-__global__ void __launch_bounds__(256) k_bshuf_blocks(const PageDesc* __restrict__ pages, int32_t num_pages, int32_t elem_size, BshufBlock* __restrict__ blocks,
-                                                       int32_t* __restrict__ flags) {
+// one thread per page: the chain of big-endian block lengths, from byte `hdr` on, -> descriptors at the page's frame_off.
+// counts[2p], counts[2p + 1]: the page's value and block counts -- k_page_footers' reading of a page's 16-byte header (hdr =
+// 16), or the host's for a null map (hdr = 0: no header, the count from the page footer, no blocks when the map is empty).
+// A chain that overruns the page, claims more than 8240 bytes for a block or does not end at the page's end raises the
+// flag; blocks from the first bad length on are skipped.
+__global__ void __launch_bounds__(256) k_bshuf_blocks(const PageDesc* __restrict__ pages, int32_t num_pages, int32_t elem_size, int32_t hdr,
+                                                       const unsigned long long* __restrict__ counts, BshufBlock* __restrict__ blocks, int32_t* __restrict__ flags) {
     const int p = blockIdx.x * blockDim.x + threadIdx.x;
     if (p >= num_pages) return;
     const PageDesc pg = pages[p];
-    if (pg.size < 16) return;
-    const uint32_t n = page_le32(pg.data), padded = page_le32(pg.data + 8), blk = BSHUF_BLOCK_BYTES / elem_size;
-    const uint32_t nb = (uint32_t)(((unsigned long long)padded + blk - 1) / blk);
-    long long pos = 16;
+    if (pg.size < hdr) return;
+    const uint32_t n = (uint32_t)counts[2 * p], blk = BSHUF_BLOCK_BYTES / elem_size, nb = (uint32_t)counts[2 * p + 1];
+    const unsigned long long padded = ((unsigned long long)n + 7) & ~7ull;
+    long long pos = hdr;
     bool bad = false;
     for (uint32_t b = 0; b < nb; b++) {
         BshufBlock d;
@@ -304,7 +322,7 @@ __global__ void __launch_bounds__(256) k_bshuf_blocks(const PageDesc* __restrict
             if (c <= BSHUF_MAX_STREAM && c <= pg.size - pos - 4) {
                 d.src = pg.data + pos + 4;
                 d.clen = c;
-                d.elems = min(blk, padded - b * blk);
+                d.elems = (uint32_t)min((unsigned long long)blk, padded - (unsigned long long)b * blk);
                 d.n_out = min(d.elems, n - b * blk); // n > b * blk: padding is < 8 elements and a block holds >= 8
                 pos += 4 + c;
             } else {
@@ -491,6 +509,208 @@ __global__ void __launch_bounds__(BSHUF_DECODE_WARPS * 32) k_bshuf_decode_dict(c
     bshuf_decode_blocks<4, true>(blocks, num_blocks, (uint8_t*)out, flags, dict, dict_size);
 }
 
+// RLE at bit width 1 ----------------------------------------------------------------------------------------------------
+// One run of a page's stream, clipped to the page's value count.  Runs are stored in stream order and cover the page's
+// rows [0, covered) without gaps, so run j ends where run j + 1 starts (the last one at `covered`).
+struct RleRun {
+    const uint8_t* lit; // a bit-packed run: its bytes, value i at bit i % 8 of byte i / 8; nullptr: a repeated run
+    uint32_t row;       // page row of the run's first value
+    uint32_t value;     // a repeated run's value (0 or 1)
+};
+
+constexpr int RLE_RUNS_BLOCK = 128;
+constexpr int RLE_STAGE_BYTES = 4096;
+
+// one CTA per page: the page's bytes pass through shared memory in windows (coalesced word loads -- one pass over HBM or
+// PCIe), thread 0 walks the run headers (RleDecoder::ReadHeader) into descriptors at the page's frame_off.  counts[2p]: the
+// page's values; counts[2p + 1]: room for descriptors (>= the runs a stream of the page's size can hold).  meta[p] = (runs,
+// rows they cover).  The walk stops at the count and reads nothing past it; it raises the flag for a header longer than 5
+// bytes or cut off by the end, a zero-length run, a repeated value other than 0 / 1, a run whose values up to the count
+// lie past the end, and a stream that ends before the count.  empty_is_zero: a page of no bytes is a page without NULLs (a
+// null map) instead of a stream that ends at once.
+__global__ void __launch_bounds__(RLE_RUNS_BLOCK) k_rle_runs(const PageDesc* __restrict__ pages, const unsigned long long* __restrict__ counts, int32_t empty_is_zero,
+                                                             RleRun* __restrict__ runs, uint2* __restrict__ meta, int32_t* __restrict__ flags) {
+    __shared__ uint32_t s_buf[RLE_STAGE_BYTES / 4];
+    __shared__ long long s_pos; // page byte the next window starts at; -1: the walk is over
+    const PageDesc pg = pages[blockIdx.x];
+    const unsigned long long n = counts[2 * blockIdx.x], cap = counts[2 * blockIdx.x + 1];
+    RleRun* out = runs + pg.frame_off;
+    unsigned long long done = 0; // thread 0's walk: values so far, runs so far
+    uint32_t nr = 0;
+    bool bad = false;
+    if (threadIdx.x == 0) s_pos = (n == 0 || (pg.size == 0 && empty_is_zero)) ? -1 : 0;
+    __syncthreads();
+    for (;;) {
+        const long long pos = s_pos;
+        if (pos < 0) break;
+        // bytes [pos, pos + avail) of the page -> shared memory, whole words from the aligned address below them
+        const long long avail = max(0ll, min(pg.size - pos, (long long)RLE_STAGE_BYTES - 4));
+        const bool last = pg.size - pos <= (long long)RLE_STAGE_BYTES - 4; // the window reaches the page's end
+        const uintptr_t a0 = (uintptr_t)(pg.data + pos) & ~(uintptr_t)3;
+        const uint32_t skew = (uint32_t)((uintptr_t)(pg.data + pos) - a0);
+        const uint32_t nwords = avail > 0 ? (uint32_t)((skew + avail + 3) / 4) : 0;
+        for (uint32_t i = threadIdx.x; i < nwords; i += RLE_RUNS_BLOCK) s_buf[i] = (uint32_t)ldg_stream_s32((const uint32_t*)a0 + i);
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            const uint8_t* b = (const uint8_t*)s_buf + skew; // b[k]: page byte pos + k, k < avail
+            long long k = 0, next = -1;
+            while (done < n) {
+                if (!last && avail - k < 6) { // a header (<= 5 bytes) and a repeated value may cross the window: move it
+                    next = pos + k;
+                    break;
+                }
+                unsigned long long h = 0;
+                bool more = true;
+                for (int hb = 0; hb < 5 && more && k < avail; hb++) {
+                    const uint32_t c = b[k++];
+                    h |= (unsigned long long)(c & 0x7F) << (7 * hb);
+                    more = (c & 0x80) != 0;
+                }
+                const unsigned long long len = h >> 1, left = n - done;
+                if (more || len == 0 || nr >= cap) { // cut off or longer than 5 bytes; a zero-length run
+                    bad = true;
+                    break;
+                }
+                RleRun r;
+                r.row = (uint32_t)done;
+                r.value = 0;
+                if (h & 1) { // bit-packed: len groups of 8 values, one byte each; only the groups up to the count are read
+                    const unsigned long long take = min(8 * len, left);
+                    if (pos + k + (long long)((take + 7) / 8) > pg.size) {
+                        bad = true;
+                        break;
+                    }
+                    r.lit = pg.data + pos + k;
+                    k += (long long)len;
+                    done += take;
+                } else { // repeated: len copies of one byte
+                    if (k >= avail || b[k] > 1) {
+                        bad = true;
+                        break;
+                    }
+                    r.lit = nullptr;
+                    r.value = b[k++];
+                    done += min(len, left);
+                }
+                out[nr++] = r;
+            }
+            s_pos = next;
+        }
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) {
+        meta[blockIdx.x] = make_uint2(nr, (uint32_t)done);
+        if (bad) atomicOr(flags, 1);
+    }
+}
+
+// 8 flags (bit i of b) -> 8 bytes of 0 / 1, flag i in byte i
+__device__ __forceinline__ unsigned long long rle_expand8(uint32_t b) {
+    return (((((unsigned long long)b * 0x0101010101010101ull) & 0x8040201008040201ull) + 0x00406070787C7E7Full) >> 7) & 0x0101010101010101ull;
+}
+
+constexpr int RLE_EXPAND_BLOCK = 256;
+
+// grid (x, page): every thread makes one aligned 8-byte word of the output at a time: the run holding the word's first row
+// by a binary search of the page's runs, then the bits of that run and the ones after it (a bit-packed run gives its bits
+// straight from its bytes, a repeated run its value 8 times), expanded into bytes and stored as one 64-bit word; the page's
+// first and last words, shared with its neighbours, byte by byte.  Rows past the runs' coverage (an empty null map) are 0.
+// null_count (optional): += the 1s stored, a popcount per thread summed per warp.
+__global__ void __launch_bounds__(RLE_EXPAND_BLOCK) k_rle_expand(const PageDesc* __restrict__ pages, const unsigned long long* __restrict__ counts,
+                                                                 const RleRun* __restrict__ runs, const uint2* __restrict__ meta, uint8_t* __restrict__ out,
+                                                                 unsigned long long* __restrict__ null_count) {
+    const int p = blockIdx.y;
+    const PageDesc pg = pages[p];
+    const long long n = (long long)counts[2 * p];
+    const uint2 m = meta[p];
+    const RleRun* rr = runs + pg.frame_off;
+    uint8_t* dst = out + pg.row_off;
+    const long long skew = (long long)((uintptr_t)dst & 7);
+    const long long nw = (skew + n + 7) / 8; // words the page's rows touch
+    uint32_t ones = 0;
+    for (long long w = (long long)blockIdx.x * RLE_EXPAND_BLOCK + threadIdx.x; w < nw; w += (long long)gridDim.x * RLE_EXPAND_BLOCK) {
+        const long long r0 = 8 * w - skew; // page row of the word's byte 0
+        const long long lo = max(r0, 0ll), hi = min(r0 + 8, n);
+        uint32_t bits = 0; // bit r - lo: row r
+        int j = -1;
+        for (int a = 0, b = (int)m.x - 1; a <= b;) { // the last run starting at or before lo
+            const int c = (a + b) >> 1;
+            if ((long long)rr[c].row <= lo) {
+                j = c;
+                a = c + 1;
+            } else {
+                b = c - 1;
+            }
+        }
+        for (long long r = lo; j >= 0 && (uint32_t)j < m.x && r < hi;) {
+            const RleRun run = rr[j];
+            const long long end = min(hi, (long long)((uint32_t)j + 1 < m.x ? rr[j + 1].row : m.y));
+            if (r >= end) break; // past the runs' coverage (a stream refused part way)
+            uint32_t v;
+            if (run.lit) {
+                const uint32_t off = (uint32_t)(r - run.row), i = off >> 3;
+                v = run.lit[i];
+                if ((off & 7) + (end - r) > 8) v |= (uint32_t)run.lit[i + 1] << 8;
+                v >>= off & 7;
+            } else {
+                v = run.value ? 0xFFu : 0u;
+            }
+            bits |= (v & ((1u << (end - r)) - 1u)) << (r - lo);
+            r = end;
+            j++;
+        }
+        ones += __popc(bits);
+        if (lo == r0 && hi == r0 + 8) {
+            *(unsigned long long*)(dst + r0) = rle_expand8(bits);
+        } else {
+            const unsigned long long x = rle_expand8(bits << (lo - r0));
+            for (long long r = lo; r < hi; r++) dst[r] = (uint8_t)(x >> (8 * (r - r0)));
+        }
+    }
+    if (null_count) {
+        ones = __reduce_add_sync(SR_FULL_MASK, ones);
+        if ((threadIdx.x & 31) == 0 && ones) atomicAdd(null_count, (unsigned long long)ones);
+    }
+}
+
+constexpr int NULL_COUNT_BLOCK = 256;
+
+// bitshuffle null maps, after k_bshuf_decode<1>: grid (x, page): a page without a map (size 0) gets zeros, every other
+// page's flags are counted (nonzero bytes; a popcount per thread summed per warp into null_count).  16-byte words where the
+// page's rows cover them, bytes at its two ends.
+__global__ void __launch_bounds__(NULL_COUNT_BLOCK) k_null_zero_count(const PageDesc* __restrict__ pages, const unsigned long long* __restrict__ counts, uint8_t* __restrict__ out,
+                                                                      unsigned long long* __restrict__ null_count) {
+    const int p = blockIdx.y;
+    const PageDesc pg = pages[p];
+    const long long n = (long long)counts[2 * p];
+    const bool zero = pg.size == 0;
+    uint8_t* dst = out + pg.row_off;
+    const long long skew = (long long)((uintptr_t)dst & 15);
+    const long long nw = (skew + n + 15) / 16;
+    uint32_t ones = 0;
+    for (long long w = (long long)blockIdx.x * NULL_COUNT_BLOCK + threadIdx.x; w < nw; w += (long long)gridDim.x * NULL_COUNT_BLOCK) {
+        const long long r0 = 16 * w - skew;
+        if (r0 >= 0 && r0 + 16 <= n) {
+            uint4* q = (uint4*)(dst + r0);
+            if (zero) {
+                *q = make_uint4(0, 0, 0, 0);
+            } else {
+                const uint4 x = *q;
+                const uint32_t y[4] = {x.x, x.y, x.z, x.w};
+#pragma unroll
+                for (int t = 0; t < 4; t++) ones += __popc((((y[t] & 0x7F7F7F7Fu) + 0x7F7F7F7Fu) | y[t]) & 0x80808080u); // nonzero bytes
+            }
+        } else {
+            for (long long r = max(r0, 0ll); r < min(r0 + 16, n); r++) {
+                if (zero) dst[r] = 0;
+                else ones += dst[r] != 0;
+            }
+        }
+    }
+    ones = __reduce_add_sync(SR_FULL_MASK, ones);
+    if ((threadIdx.x & 31) == 0 && ones) atomicAdd(null_count, (unsigned long long)ones);
+}
+
 } // namespace srd
 
 // host side ------------------------------------------------------------------------------------------------------------
@@ -499,31 +719,15 @@ struct PageScratch {
     PinnedBuf host_pages, host_counts;
 };
 
-// dict / dict_words: the decoder's code -> value table (device memory; dict_words < 0: none set), read by SR_PAGE_DICT only
-static int32_t pages_decode(sr_ctx* ctx, PageScratch* sc, int32_t encoding, int32_t type, const sr_page_view* pv, int32_t num_pages, int32_t mem, void* out,
-                            int64_t out_capacity, int64_t* out_rows, const int32_t* dict, long long dict_words) {
-    const int w = srd::type_width(type);
-    if (encoding == SR_PAGE_DICT) {
-        if (type != SR_TYPE_INT) return sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "dictionary page decode of type %d (TYPE_INT ids)", type);
-        if (dict_words < 0) return sr_fail(ctx, SR_ERR_STATE, "dictionary pages decoded before sr_page_decoder_set_dict");
-    } else if (encoding == SR_PAGE_BITSHUFFLE) {
-        if (w == 0) return sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "bitshuffle page decode of type %d (fixed-width types)", type);
-    } else {
-        if ((w != 4 && w != 8) || srd::is_float_class(type)) return sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "page decode of type %d (4- and 8-byte integer-class types)", type);
-        if (encoding != SR_PAGE_PLAIN && encoding != SR_PAGE_FOR) return sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "page encoding %d", encoding);
-    }
-    // one rule for every encoding: k_for_decode and the bitshuffle kernels store whole values where a lane's address is not
-    // vector-aligned, so a column off its natural alignment would be a misaligned store (plain pages follow the same rule)
-    if ((uintptr_t)out % std::min(w, 8)) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "output column not aligned to %d bytes", std::min(w, 8));
-    if (num_pages < 0 || (num_pages > 0 && !pv)) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "pages");
-    SR_TRY(mem_check(ctx, mem, "pages"));
-    *out_rows = 0;
-    if (num_pages == 0) return SR_OK;
+// where the kernels read the pages: hp[p].data / .size of every page in sc->host_pages (the caller sets row_off / frame_off).
+// View: sr_page_view or sr_null_map_view (data, size).
+template <typename View>
+static int32_t stage_pages(sr_ctx* ctx, PageScratch* sc, const View* pv, int32_t num_pages, int32_t mem) {
     if (!sc->host_pages.reserve(sizeof(srd::PageDesc) * (size_t)num_pages) || !sc->host_counts.reserve(16 * (size_t)num_pages + 16))
         return sr_fail(ctx, SR_ERR_OUT_OF_MEMORY, "page tables");
     srd::PageDesc* hp = (srd::PageDesc*)sc->host_pages.p;
-    // where the kernels read the pages.  Host pages that lie back to back (a page cache hands out slices of large buffers) are
-    // merged into RUNS: one copy per run instead of one per page.
+    // Host pages that lie back to back (a page cache hands out slices of large buffers) are merged into RUNS: one copy per
+    // run instead of one per page.
     for (int p = 0; p < num_pages; p++)
         if (pv[p].size < 0 || (pv[p].size > 0 && !pv[p].data)) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "page %d", p);
     struct Run {
@@ -569,6 +773,53 @@ static int32_t pages_decode(sr_ctx* ctx, PageScratch* sc, int32_t encoding, int3
             hp[p].size = pv[p].size;
         }
     }
+    return SR_OK;
+}
+
+// RLE streams at bit width 1 (sc->pages and sc->counts on the device: values, room for runs; `runs` descriptors in all)
+// -> flags in out.  null_count: see k_rle_expand.
+static int32_t rle_launch(sr_ctx* ctx, PageScratch* sc, int32_t num_pages, long long runs, long long max_rows, int32_t empty_is_zero, uint8_t* out,
+                          unsigned long long* null_count) {
+    SR_TRY(sc->frames.reserve(ctx, sizeof(srd::RleRun) * (size_t)runs + sizeof(uint2) * (size_t)num_pages));
+    srd::RleRun* rr = (srd::RleRun*)sc->frames.p;
+    uint2* meta = (uint2*)(rr + runs);
+    const srd::PageDesc* pages = (const srd::PageDesc*)sc->pages.p;
+    const unsigned long long* counts = sc->counts.as<unsigned long long>();
+    srd::k_rle_runs<<<num_pages, srd::RLE_RUNS_BLOCK, 0, ctx->stream>>>(pages, counts, empty_is_zero, rr, meta, (int32_t*)sc->flags.p);
+    SR_LAUNCH_CHECK(ctx);
+    // about two words per thread of the longest page
+    const int gx = (int)std::min<long long>(std::max<long long>((max_rows + 16 * srd::RLE_EXPAND_BLOCK - 1) / (16 * srd::RLE_EXPAND_BLOCK), 1), 64);
+    for (int p0 = 0; p0 < num_pages; p0 += 65535) { // gridDim.y is limited to 65535
+        srd::k_rle_expand<<<dim3(gx, std::min(num_pages - p0, 65535)), srd::RLE_EXPAND_BLOCK, 0, ctx->stream>>>(pages + p0, counts + 2 * (size_t)p0, rr, meta + p0, out, null_count);
+        SR_LAUNCH_CHECK(ctx);
+    }
+    return SR_OK;
+}
+
+// dict / dict_words: the decoder's code -> value table (device memory; dict_words < 0: none set), read by SR_PAGE_DICT only
+static int32_t pages_decode(sr_ctx* ctx, PageScratch* sc, int32_t encoding, int32_t type, const sr_page_view* pv, int32_t num_pages, int32_t mem, void* out,
+                            int64_t out_capacity, int64_t* out_rows, const int32_t* dict, long long dict_words) {
+    const int w = srd::type_width(type);
+    if (encoding == SR_PAGE_DICT) {
+        if (type != SR_TYPE_INT) return sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "dictionary page decode of type %d (TYPE_INT ids)", type);
+        if (dict_words < 0) return sr_fail(ctx, SR_ERR_STATE, "dictionary pages decoded before sr_page_decoder_set_dict");
+    } else if (encoding == SR_PAGE_BITSHUFFLE) {
+        if (w == 0) return sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "bitshuffle page decode of type %d (fixed-width types)", type);
+    } else if (encoding == SR_PAGE_RLE) {
+        if (type != SR_TYPE_BOOLEAN) return sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "page encoding %d of type %d (RLE pages: BOOLEAN)", encoding, type);
+    } else {
+        if ((w != 4 && w != 8) || srd::is_float_class(type)) return sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "page decode of type %d (4- and 8-byte integer-class types)", type);
+        if (encoding != SR_PAGE_PLAIN && encoding != SR_PAGE_FOR) return sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "page encoding %d", encoding);
+    }
+    // one rule for every encoding: k_for_decode and the bitshuffle kernels store whole values where a lane's address is not
+    // vector-aligned, so a column off its natural alignment would be a misaligned store (plain pages follow the same rule)
+    if ((uintptr_t)out % std::min(w, 8)) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "output column not aligned to %d bytes", std::min(w, 8));
+    if (num_pages < 0 || (num_pages > 0 && !pv)) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "pages");
+    SR_TRY(mem_check(ctx, mem, "pages"));
+    *out_rows = 0;
+    if (num_pages == 0) return SR_OK;
+    SR_TRY(stage_pages(ctx, sc, pv, num_pages, mem));
+    srd::PageDesc* hp = (srd::PageDesc*)sc->host_pages.p;
     SR_TRY(sc->pages.reserve(ctx, sizeof(srd::PageDesc) * (size_t)num_pages));
     SR_TRY(sc->counts.reserve(ctx, 16 * (size_t)num_pages));
     SR_TRY(sc->flags.reserve(ctx, 16));
@@ -584,11 +835,13 @@ static int32_t pages_decode(sr_ctx* ctx, PageScratch* sc, int32_t encoding, int3
     const int32_t hflags = *(const int32_t*)(hc + 2 * (size_t)num_pages);
     if (hflags & 1)
         return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "a page is not a well-formed %s page",
-                       encoding == SR_PAGE_FOR ? "frame-of-reference" : encoding == SR_PAGE_PLAIN ? "plain" : encoding == SR_PAGE_DICT ? "dictionary data" : "bitshuffle");
+                       encoding == SR_PAGE_FOR ? "frame-of-reference" : encoding == SR_PAGE_PLAIN ? "plain" : encoding == SR_PAGE_DICT ? "dictionary data"
+                                                    : encoding == SR_PAGE_RLE ? "RLE" : "bitshuffle");
     if (hflags & 2) return sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "a dictionary data page in plain mode: the column fell back to plain pages");
-    long long rows = 0, frames = 0;
+    long long rows = 0, frames = 0, max_rows = 0;
     for (int p = 0; p < num_pages; p++) {
-        if (encoding == SR_PAGE_DICT) { // past the mode word: the bitshuffle page of codes (k_bshuf_blocks reads it as is)
+        // past the mode word: the bitshuffle page of codes (k_bshuf_blocks reads it as is); past an RLE page's value count
+        if (encoding == SR_PAGE_DICT || encoding == SR_PAGE_RLE) {
             hp[p].data += 4;
             hp[p].size -= 4;
         }
@@ -596,6 +849,7 @@ static int32_t pages_decode(sr_ctx* ctx, PageScratch* sc, int32_t encoding, int3
         hp[p].frame_off = frames;
         rows += (long long)hc[2 * p];
         frames += (long long)hc[2 * p + 1];
+        max_rows = std::max(max_rows, (long long)hc[2 * p]);
     }
     if (rows > out_capacity) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "the pages hold %lld values, the output column has room for %lld", rows, (long long)out_capacity);
     *out_rows = rows;
@@ -609,10 +863,18 @@ static int32_t pages_decode(sr_ctx* ctx, PageScratch* sc, int32_t encoding, int3
         }
         return SR_OK;
     }
+    if (encoding == SR_PAGE_RLE) {
+        SR_TRY(rle_launch(ctx, sc, num_pages, frames, max_rows, 0, (uint8_t*)out, nullptr));
+        SR_CUDA(ctx, cudaMemcpyAsync(hc, sc->flags.p, 8, cudaMemcpyDeviceToHost, ctx->stream));
+        SR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        if (*(const int32_t*)hc) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "an RLE page has a malformed run stream");
+        return SR_OK;
+    }
     if (encoding == SR_PAGE_BITSHUFFLE || encoding == SR_PAGE_DICT) {
         SR_TRY(sc->frames.reserve(ctx, sizeof(srd::BshufBlock) * (size_t)frames));
         srd::BshufBlock* blocks = (srd::BshufBlock*)sc->frames.p;
-        srd::k_bshuf_blocks<<<grid_for(num_pages, 256), 256, 0, ctx->stream>>>((const srd::PageDesc*)sc->pages.p, num_pages, w, blocks, (int32_t*)sc->flags.p);
+        srd::k_bshuf_blocks<<<grid_for(num_pages, 256), 256, 0, ctx->stream>>>((const srd::PageDesc*)sc->pages.p, num_pages, w, 16, sc->counts.as<unsigned long long>(), blocks,
+                                                                               (int32_t*)sc->flags.p);
         SR_LAUNCH_CHECK(ctx);
         const int bgrid = (int)std::min<long long>((frames + srd::BSHUF_DECODE_WARPS - 1) / srd::BSHUF_DECODE_WARPS, (long long)ctx->num_sms * 8);
         int32_t* flags = (int32_t*)sc->flags.p;
@@ -652,5 +914,77 @@ static int32_t pages_decode(sr_ctx* ctx, PageScratch* sc, int32_t encoding, int3
     SR_CUDA(ctx, cudaMemcpyAsync(hc, sc->flags.p, 8, cudaMemcpyDeviceToHost, ctx->stream));
     SR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     if (*(const int32_t*)hc) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "a frame-of-reference page has a corrupt frame table");
+    return SR_OK;
+}
+
+// the null maps of a run of data pages -> uint8 flags (1 = NULL) in out, page k's after page k - 1's
+static int32_t null_maps_decode(sr_ctx* ctx, PageScratch* sc, int32_t encoding, const sr_null_map_view* maps, int32_t num_pages, int32_t mem, uint8_t* out,
+                                int64_t out_capacity, int64_t* out_rows, int64_t* out_null_count) {
+    if (encoding != SR_NULL_BITSHUFFLE && encoding != SR_NULL_RLE) return sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "null map encoding %d", encoding);
+    if (num_pages < 0 || (num_pages > 0 && !maps)) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "null maps");
+    SR_TRY(mem_check(ctx, mem, "null maps"));
+    *out_rows = 0;
+    *out_null_count = 0;
+    // every row count is the page footer's: the whole layout is known before anything is copied
+    long long rows = 0, max_rows = 0;
+    for (int p = 0; p < num_pages; p++) {
+        if (maps[p].size < 0 || (maps[p].size > 0 && !maps[p].data) || maps[p].num_rows < 0 || maps[p].num_rows > (int64_t)UINT32_MAX)
+            return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "null map %d: %lld bytes, %lld rows", p, (long long)maps[p].size, (long long)maps[p].num_rows);
+        rows += maps[p].num_rows;
+        max_rows = std::max(max_rows, (long long)maps[p].num_rows);
+    }
+    if (rows > out_capacity) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "the null maps hold %lld rows, the output column has room for %lld", rows, (long long)out_capacity);
+    if (rows > 0 && !out) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "null output");
+    if (num_pages == 0) return SR_OK;
+    SR_TRY(stage_pages(ctx, sc, maps, num_pages, mem));
+    srd::PageDesc* hp = (srd::PageDesc*)sc->host_pages.p;
+    unsigned long long* hc = (unsigned long long*)sc->host_counts.p;
+    long long frames = 0, at = 0;
+    for (int p = 0; p < num_pages; p++) {
+        const unsigned long long n = (unsigned long long)maps[p].num_rows, size = (unsigned long long)maps[p].size;
+        hp[p].row_off = at;
+        hp[p].frame_off = frames;
+        hc[2 * p] = n;
+        // bitshuffle: the blocks of ALIGN_UP(n, 8) one-byte flags (none for an absent map); RLE: room for every run the map can hold
+        hc[2 * p + 1] = encoding == SR_NULL_BITSHUFFLE ? (size ? ((n + 7) / 8 * 8 + srd::BSHUF_BLOCK_BYTES - 1) / srd::BSHUF_BLOCK_BYTES : 0) : std::min(n, size / 2);
+        at += (long long)n;
+        frames += (long long)hc[2 * p + 1];
+    }
+    SR_TRY(sc->pages.reserve(ctx, sizeof(srd::PageDesc) * (size_t)num_pages));
+    SR_TRY(sc->counts.reserve(ctx, 16 * (size_t)num_pages));
+    SR_TRY(sc->flags.reserve(ctx, 16));
+    SR_CUDA(ctx, cudaMemsetAsync(sc->flags.p, 0, 16, ctx->stream)); // the error flag, then the null count
+    SR_CUDA(ctx, cudaMemcpyAsync(sc->pages.p, hp, sizeof(srd::PageDesc) * (size_t)num_pages, cudaMemcpyHostToDevice, ctx->stream));
+    SR_CUDA(ctx, cudaMemcpyAsync(sc->counts.p, hc, 16 * (size_t)num_pages, cudaMemcpyHostToDevice, ctx->stream));
+    int32_t* flags = (int32_t*)sc->flags.p;
+    unsigned long long* null_count = (unsigned long long*)((uint8_t*)sc->flags.p + 8);
+    if (encoding == SR_NULL_RLE) {
+        SR_TRY(rle_launch(ctx, sc, num_pages, frames, max_rows, 1, out, null_count));
+    } else {
+        // a map is bitshuffle::compress_lz4 of the padded flags: a BIT_SHUFFLE page of one-byte values without its header
+        const srd::PageDesc* pages = (const srd::PageDesc*)sc->pages.p;
+        SR_TRY(sc->frames.reserve(ctx, sizeof(srd::BshufBlock) * (size_t)frames));
+        srd::BshufBlock* blocks = (srd::BshufBlock*)sc->frames.p;
+        srd::k_bshuf_blocks<<<grid_for(num_pages, 256), 256, 0, ctx->stream>>>(pages, num_pages, 1, 0, sc->counts.as<unsigned long long>(), blocks, flags);
+        SR_LAUNCH_CHECK(ctx);
+        if (frames > 0) {
+            const int bgrid = (int)std::min<long long>((frames + srd::BSHUF_DECODE_WARPS - 1) / srd::BSHUF_DECODE_WARPS, (long long)ctx->num_sms * 8);
+            srd::k_bshuf_decode<1><<<bgrid, srd::BSHUF_DECODE_WARPS * 32, 0, ctx->stream>>>(blocks, frames, out, flags);
+            SR_LAUNCH_CHECK(ctx);
+        }
+        const int gx = (int)std::min<long long>(std::max<long long>((max_rows + 32 * srd::NULL_COUNT_BLOCK - 1) / (32 * srd::NULL_COUNT_BLOCK), 1), 64);
+        for (int p0 = 0; p0 < num_pages; p0 += 65535) { // gridDim.y is limited to 65535
+            srd::k_null_zero_count<<<dim3(gx, std::min(num_pages - p0, 65535)), srd::NULL_COUNT_BLOCK, 0, ctx->stream>>>(pages + p0, sc->counts.as<unsigned long long>() + 2 * (size_t)p0,
+                                                                                                                       out, null_count);
+            SR_LAUNCH_CHECK(ctx);
+        }
+    }
+    unsigned long long* back = hc + 2 * (size_t)num_pages; // the 16 spare bytes of host_counts
+    SR_CUDA(ctx, cudaMemcpyAsync(back, sc->flags.p, 16, cudaMemcpyDeviceToHost, ctx->stream));
+    SR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    if (*(const int32_t*)back)
+        return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, encoding == SR_NULL_RLE ? "a null map has a malformed RLE stream" : "a null map has a corrupt block chain or LZ4 stream");
+    *out_rows = rows;
+    *out_null_count = (int64_t)back[1];
     return SR_OK;
 }

@@ -168,6 +168,7 @@ def lib():
         "sr_page_decoder_destroy": (None, [vp]),
         "sr_pages_decode": (i32, [vp, i32, i32, vp, i32, i32, vp, i64, vp]),
         "sr_page_decoder_set_dict": (i32, [vp, vp, i64, i32]),
+        "sr_null_maps_decode": (i32, [vp, i32, vp, i32, i32, vp, i64, vp, vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)
@@ -193,7 +194,7 @@ EXPORTED_SYMBOLS = [
     "sr_xchg_destroy", "sr_xchg_partition", "sr_xchg_hash", "sr_gather", "sr_memcpy", "sr_abi_sizeof", "sr_bandwidth_probe", "sr_flush_l2",
     "sr_chunk_serialized_size", "sr_chunk_serialize", "sr_serde_create", "sr_serde_destroy", "sr_chunk_deserialize",
     "sr_host_alloc", "sr_host_free", "sr_event_create", "sr_event_destroy", "sr_event_record", "sr_event_query", "sr_event_sync",
-    "sr_page_decoder_create", "sr_page_decoder_destroy", "sr_pages_decode", "sr_page_decoder_set_dict",
+    "sr_page_decoder_create", "sr_page_decoder_destroy", "sr_pages_decode", "sr_page_decoder_set_dict", "sr_null_maps_decode",
 ]
 
 
@@ -592,7 +593,8 @@ def chunk_serialize(ctx, chunk, row_begin=0, row_end=None):
 
 
 class PageDecoder:
-    """sr_page_decoder: frame-of-reference / plain / bitshuffle data pages -> a device column; dictionary data pages -> ids"""
+    """sr_page_decoder: frame-of-reference / plain / bitshuffle / RLE data pages -> a device column; dictionary data pages ->
+    ids; the pages' null maps -> the uint8 null column"""
 
     def __init__(self, ctx):
         self.ctx = ctx
@@ -627,6 +629,22 @@ class PageDecoder:
             a = np.ascontiguousarray(values, dtype=np.int32)
             ptr, n = (a.ctypes.data if a.size else None), a.size
         self.ctx.check(lib().sr_page_decoder_set_dict(self.h, ptr, n, mem))
+
+    def decode_nulls(self, encoding, maps, out_ptr, capacity, mem=abi.MEM_HOST):
+        """maps: one per data page, (uint8 numpy array, num_rows) with host memory or (pointer, size, num_rows) triples;
+        out_ptr: device pointer of the uint8 null column.  -> (rows, null_count)"""
+        views = (abi.sr_null_map_view * max(1, len(maps)))()
+        keep = []
+        for k, m in enumerate(maps):
+            if len(m) == 3:
+                views[k].data, views[k].size, views[k].num_rows = m
+            else:
+                a = np.ascontiguousarray(m[0], dtype=np.uint8)
+                keep.append(a)
+                views[k].data, views[k].size, views[k].num_rows = (a.ctypes.data if a.size else None), a.size, m[1]
+        rows, nulls = C.c_int64(0), C.c_int64(0)
+        self.ctx.check(lib().sr_null_maps_decode(self.h, encoding, views, len(maps), mem, out_ptr, capacity, C.byref(rows), C.byref(nulls)))
+        return rows.value, nulls.value
 
 
 class Serde:

@@ -1,6 +1,6 @@
 """Segment page decode on the device (SURVEY.md 8f-4): throughput of sr_pages_decode on SSB-shaped key columns.
 
-    python tools/page_decode_bench.py [--rows 50000000] [--page-rows 65536] [--encoding for|bitshuffle|both|dict]
+    python tools/page_decode_bench.py [--rows 50000000] [--page-rows 65536] [--encoding for|bitshuffle|both|dict|nulls|rle]
 
 Encodes synthetic lineorder key columns on the host -- frame-of-reference pages with the (reference-pinned) oracle encoder,
 BIT_SHUFFLE pages (bitshuffle + LZ4, StarRocks' default for these types) with the CPU codec in bshuf_oracle -- then times
@@ -10,8 +10,17 @@ only the encoded bytes cross the bus), and checks every decoded column against t
 --encoding dict: low-cardinality string columns (7, 25 and 256 words, codes drawn uniformly) written as dictionary data
 pages (mode word + bitshuffle page of int32 codes) and decoded into global ids through a per-segment table, timed next to
 BIT_SHUFFLE pages of the same codes decoded as plain int32 -- the difference is the mode word and the translation.
+
+--encoding nulls: the null maps of nullable columns (0 %, 0.1 %, 1 %, 10 %, 50 % random NULLs and runs of ~1000, as
+BITSHUFFLE_NULL and RLE_NULL maps; a page without NULL has no map) decoded by sr_null_maps_decode from device and from
+page-locked host memory, timed next to the H2D copy of the decoded uint8 null column from page-locked memory -- what a
+caller that decodes the maps on the CPU moves instead.
+
+--encoding rle: BOOLEAN columns as RLE pages -- random, runs of ~5000, and alternating runs of 8 (the worst case of the
+serial run-header walk: one header per two bytes of page).
 """
 import argparse
+import ctypes as C
 import json
 import os
 import sys
@@ -32,10 +41,12 @@ def main():
     ap.add_argument("--page-rows", type=int, default=65_536)
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--repeat", type=int, default=8, help="decode the encoded pages this many times over into one column (amortises the per-call costs without more host encoding)")
-    ap.add_argument("--encoding", choices=["for", "bitshuffle", "both", "dict"], default="for")
+    ap.add_argument("--encoding", choices=["for", "bitshuffle", "both", "dict", "nulls", "rle"], default="for")
     args = ap.parse_args()
     if args.encoding == "dict":
         return dict_bench(args)
+    if args.encoding in ("nulls", "rle"):
+        return bool_bench(args)
     n = args.rows
     rng = np.random.default_rng(1)
     cols = {"lo_custkey (22 bits)": rng.integers(1, 3_000_000, n, dtype=np.int32), "lo_suppkey (18 bits)": rng.integers(1, 200_000, n, dtype=np.int32),
@@ -94,6 +105,93 @@ def _time(dec, code, views, out, rows, mem, reps):
         best = min(best, e0.elapsed_time(e1))
     assert got == rows
     return best
+
+
+def _power_limit():
+    import subprocess
+    try:
+        return subprocess.run(["nvidia-smi", "-i", str(torch.cuda.current_device()), "--query-gpu=power.limit", "--format=csv,noheader"],
+                              capture_output=True, text=True, timeout=30).stdout.strip()
+    except OSError:
+        return "unknown"
+
+
+def _best_ms(fn, reps):
+    best = 1e9
+    for _ in range(reps):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        torch.cuda.synchronize()
+        e0.record()
+        fn()
+        e1.record()
+        torch.cuda.synchronize()
+        best = min(best, e0.elapsed_time(e1))
+    return best
+
+
+def bool_bench(args):
+    """--encoding nulls / rle: one byte per row out, a fraction of a bit per row in"""
+    n, R, P = args.rows, args.repeat, args.page_rows
+    rng = np.random.default_rng(3)
+    ctx = gpu.Context(0)
+    dec = gpu.PageDecoder(ctx)
+    out = torch.empty(n * R, dtype=torch.uint8, device="cuda")
+    parts = [(lo, min(lo + P, n)) for lo in range(0, n, P)]
+    res = []
+    if args.encoding == "nulls":
+        host_col = torch.empty(n * R, dtype=torch.uint8).pin_memory()
+        h2d_ms = _best_ms(lambda: out.copy_(host_col, non_blocking=True), args.reps)
+        clustered = np.zeros(n, np.uint8)
+        for st in rng.integers(0, n, n // 10_000):
+            clustered[st:st + 1000] = 1
+        columns = [("%g%% random" % (100 * f), (rng.random(n) < f).astype(np.uint8)) for f in (0.0, 0.001, 0.01, 0.1, 0.5)]
+        columns.append(("runs of ~1000 (%.1f%%)" % (100 * clustered.mean()), clustered))
+        cases = [(name, f, label, enc) for name, f in columns for label, enc in (("bitshuffle", bshuf_oracle.NULL_BITSHUFFLE), ("rle", bshuf_oracle.NULL_RLE))]
+    else:
+        columns = [("random", rng.integers(0, 2, n).astype(np.uint8)), ("runs of ~5000", np.repeat(rng.integers(0, 2, n // 5000 + 1), 5000)[:n].astype(np.uint8)),
+                   ("alternating runs of 8", np.repeat(np.arange(n // 8 + 1) % 2, 8)[:n].astype(np.uint8))]
+        cases = [(name, f, "rle_page", None) for name, f in columns]
+    for name, f, label, enc in cases:
+        t0 = time.perf_counter()
+        if enc is None:
+            bufs = [bshuf_oracle.rle_bool_page_encode(f[a:b]) for a, b in parts]
+        else:
+            bufs = [bshuf_oracle.null_map_encode(f[a:b], enc) for a, b in parts]
+        enc_s = time.perf_counter() - t0
+        total = sum(len(b) for b in bufs)
+        blob = torch.from_numpy(np.concatenate([np.pad(b, (0, (-len(b)) % 16)) for b in bufs] + [np.zeros(16, np.uint8)]))
+        offs = np.cumsum([0] + [len(b) + (-len(b)) % 16 for b in bufs])
+        dblob, pblob = blob.cuda(), blob.pin_memory()
+        line = {"column": name, "encoding": label, "rows": n * R, "pages": len(bufs) * R, "bits_per_row": 8.0 * total / n}
+        want = int(f.sum()) * R
+        for where, base, mem in (("device", dblob.data_ptr(), abi.MEM_DEVICE), ("pinned_host", pblob.data_ptr(), abi.MEM_HOST_PINNED)):
+            out.fill_(0xA5)
+            # the view array is built once, outside the timed window: the window holds the library call alone
+            rows, nulls = C.c_int64(0), C.c_int64(0)
+            if enc is None:
+                views = (abi.sr_page_view * (len(bufs) * R))(*[abi.sr_page_view(base + int(offs[k]), len(b)) for k, b in enumerate(bufs)] * R)
+                def call():
+                    ctx.check(gpu.lib().sr_pages_decode(dec.h, abi.PAGE_RLE, abi.TYPE_BOOLEAN, views, len(views), mem, out.data_ptr(), n * R, C.byref(rows)))
+            else:
+                views = (abi.sr_null_map_view * (len(bufs) * R))(*[abi.sr_null_map_view(base + int(offs[k]), len(b), b1 - a1)
+                                                                  for k, (b, (a1, b1)) in enumerate(zip(bufs, parts))] * R)
+                def call():
+                    ctx.check(gpu.lib().sr_null_maps_decode(dec.h, enc, views, len(views), mem, out.data_ptr(), n * R, C.byref(rows), C.byref(nulls)))
+            ms = _best_ms(call, args.reps)
+            ok = rows.value == n * R and (enc is None or nulls.value == want) and bool((out.view(R, n).cpu().numpy() == f[None, :]).all())
+            line[where] = {"ms": ms, "g_rows_per_s": n * R / ms / 1e6, "page_gbs": total * R / ms / 1e6, "bit_exact": ok}
+        if enc is not None:
+            line["vs_h2d_copy_of_null_column"] = {lbl: h2d_ms / line[lbl]["ms"] for lbl in ("device", "pinned_host")}
+        line["host_encode_s"] = enc_s
+        res.append(line)
+        del dblob, pblob
+    dec.close()
+    head = {"workload": "null map decode (sr_null_maps_decode)" if args.encoding == "nulls" else "BOOLEAN RLE page decode (sr_pages_decode, SR_PAGE_RLE)",
+            "device": torch.cuda.get_device_properties(0).name, "power_limit": _power_limit(), "page_rows": P}
+    if args.encoding == "nulls":
+        head["h2d_copy_of_uint8_null_column"] = {"ms": h2d_ms, "g_rows_per_s": n * R / h2d_ms / 1e6, "gbs": n * R / h2d_ms / 1e6}
+    head["columns"] = res
+    print(json.dumps(head))
 
 
 def dict_bench(args):
