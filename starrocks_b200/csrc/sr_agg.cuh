@@ -1028,6 +1028,21 @@ __global__ void __launch_bounds__(EMIT_BLOCK) k_agg_emit(const AggDev* __restric
 // ---------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------
+// the table's status block in device memory (sr_agg::counters), read back whole by agg_fetch_status
+struct AggCounters {
+    unsigned long long ngroups;   // AggDev::ngroups
+    int32_t flags[2];             // AggDev::flags: [0] overflow (a row or slot was not placed), [1] a key outside the dense range
+    unsigned long long unused0[2];
+    unsigned long long part_fail; // the radix-partitioned push: buckets, then records, the table refused
+    unsigned long long part_ovf;  // the radix-partitioned push: records that found their bucket's region full
+    unsigned long long refused;   // rows or merged slots a full slice refused, re-applied by agg_retry_refused
+    unsigned long long unused1;
+};
+static_assert(sizeof(AggCounters) == 64, "AggCounters layout");
+static_assert(offsetof(AggCounters, ngroups) == 0 && offsetof(AggCounters, flags) == 8, "AggCounters layout");
+static_assert(offsetof(AggCounters, part_fail) == 32 && offsetof(AggCounters, part_ovf) == 40, "AggCounters layout");
+static_assert(offsetof(AggCounters, refused) == 48 && offsetof(AggCounters, unused1) == 56, "AggCounters layout");
+
 struct sr_agg {
     sr_ctx* ctx = nullptr;
     sr_agg_desc desc;
@@ -1036,11 +1051,9 @@ struct sr_agg {
     VReg reg;
     srd::AggDev host; // host mirror of the device descriptor
     DevBuf dev;       // AggDev on device
-    // counters: [0] ngroups, [1] flags, [4] / [5] the partitioned push's fail / overflow counts, [6] the fail count of
-    // agg_retry_rows and the merge
-    DevBuf hkeys, slab /* every state array, laid out by agg_state_arrays */, counters;
-    DevBuf fail_list;       // rows (or merged slots) the table refused, for agg_retry_rows and the merge
-    ColBufs retry_cols[2];  // agg_retry_rows: the refused rows gathered, alternately
+    DevBuf hkeys, slab /* every state array, laid out by agg_state_arrays */, counters /* one AggCounters */;
+    DevBuf fail_list;       // rows (or merged slots) the table refused, for agg_retry_refused
+    ColBufs retry_cols[2];  // agg_push_rows: the refused rows gathered, alternately
     DevBuf late_accn[SR_MAX_AGG_FNS]; // accn of a function whose input turned nullable after the slab was laid out
     DevBuf slots_tmp;
     // radix-partitioned push (sr_agg_part.cuh): bucket histogram / bases / cursors, tile list, staged records, retry lists
@@ -1070,6 +1083,8 @@ struct sr_agg {
         for (sr_agg* c : distinct) delete c;
     }
 };
+
+static AggCounters* agg_counters(sr_agg* a) { return a->counters.as<AggCounters>(); }
 
 static int32_t agg_result_type(const sr_agg_fn& f) {
     switch (f.kind) {
@@ -1194,10 +1209,11 @@ static int32_t agg_alloc_tables(sr_ctx* ctx, srd::AggDev* h, uint64_t cap, DevBu
 static int32_t agg_setup_tables(sr_agg* a, uint64_t cap) {
     sr_ctx* ctx = a->ctx;
     srd::AggDev& h = a->host;
-    SR_TRY(a->counters.reserve(ctx, 64));
-    SR_CUDA(ctx, cudaMemsetAsync(a->counters.p, 0, 64, ctx->stream));
-    h.ngroups = a->counters.as<unsigned long long>();
-    h.flags = (int32_t*)(a->counters.as<unsigned long long>() + 1);
+    SR_TRY(a->counters.reserve(ctx, sizeof(AggCounters)));
+    AggCounters* c = agg_counters(a);
+    SR_CUDA(ctx, cudaMemsetAsync(c, 0, sizeof(AggCounters), ctx->stream));
+    h.ngroups = &c->ngroups;
+    h.flags = c->flags;
     SR_TRY(agg_alloc_tables(ctx, &h, cap, &a->hkeys, &a->slab));
     // shared-memory accumulation for small dense tables -- including the single state of a query without GROUP BY
     // inside a fused fragment (every surviving row would otherwise hit the same global address with an atomic; the
@@ -1399,15 +1415,40 @@ static int32_t agg_grow(sr_agg* a, uint64_t new_cap) {
     return agg_upload(a);
 }
 
-// read ngroups + flags (synchronises)
-static int32_t agg_read_counters(sr_agg* a, uint64_t* ngroups, int32_t* overflow, int32_t* bad_range) {
+static const uint64_t kAggMaxSlots = 1ull << 33;
+
+// The growth policy of a hash table, which every path that grows it follows: the smallest cap * factor^k (k >= 1 when
+// `force`) whose admission limit (cap / 2, agg_alloc_tables) takes the ngroups_host groups held plus `need` more, reached
+// with one rehash.  The capacity decides where every group lands, and groups are emitted in slot order.
+static int32_t agg_grow_to_fit(sr_agg* a, uint64_t need, uint64_t factor, bool force) {
+    uint64_t cap = force ? a->host.cap * factor : a->host.cap;
+    while ((uint64_t)a->ngroups_host + need > cap / 2 && cap <= kAggMaxSlots) cap *= factor;
+    if (cap == a->host.cap) return SR_OK;
+    if (cap > kAggMaxSlots) return sr_fail(a->ctx, SR_ERR_OUT_OF_MEMORY, "aggregate table would exceed 2^33 slots; push smaller batches");
+    return agg_grow(a, cap);
+}
+
+static int32_t agg_clear_flags(sr_agg* a) {
+    SR_CUDA(a->ctx, cudaMemsetAsync(agg_counters(a)->flags, 0, sizeof(AggCounters::flags), a->ctx->stream));
+    return SR_OK;
+}
+
+// enqueue a copy of the status block into pinned memory, without synchronising: *st is valid after the next
+// synchronisation of the stream
+static int32_t agg_fetch_status(sr_agg* a, const AggCounters** st) {
     sr_ctx* ctx = a->ctx;
-    SR_CUDA(ctx, cudaMemcpyAsync(ctx->pinned + 8, a->counters.p, 16, cudaMemcpyDeviceToHost, ctx->stream));
-    SR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    *ngroups = ctx->pinned[8];
-    const int32_t* fl = (const int32_t*)(ctx->pinned + 9);
-    *overflow = fl[0];
-    *bad_range = fl[1];
+    SR_CUDA(ctx, cudaMemcpyAsync(ctx->pinned + 8, agg_counters(a), sizeof(AggCounters), cudaMemcpyDeviceToHost, ctx->stream));
+    *st = (const AggCounters*)(ctx->pinned + 8);
+    return SR_OK;
+}
+
+// the status block (synchronises); refreshes ngroups_host
+static int32_t agg_read_status(sr_agg* a, AggCounters* st) {
+    const AggCounters* p;
+    SR_TRY(agg_fetch_status(a, &p));
+    SR_CUDA(a->ctx, cudaStreamSynchronize(a->ctx->stream));
+    *st = *p;
+    a->ngroups_host = (int64_t)st->ngroups;
     return SR_OK;
 }
 
@@ -1453,8 +1494,6 @@ static int32_t agg_check_nullability(sr_agg* a, const VTab& vt) {
 
 #include "sr_agg_part_host.cuh"
 
-static unsigned long long* agg_fail_count(sr_agg* a) { return a->counters.as<unsigned long long>() + 6; }
-
 // the rows index[0, m) of the columns `vt` reads at the kernel's own row, gathered into `bufs`: `out` reads the same
 // values at rows [0, m) (values read at a join's build row stay where they are)
 static int32_t vtab_gather(sr_ctx* ctx, const VTab& vt, const uint32_t* index, int64_t m, ColBufs* bufs, VTab* out) {
@@ -1475,35 +1514,45 @@ static int32_t vtab_gather(sr_ctx* ctx, const VTab& vt, const uint32_t* index, i
     return SR_OK;
 }
 
-// A one-pass kernel has run over the rows of `vt`, appending the rows a full 256-slot slice refused (they applied nothing)
-// to a->fail_list, counted at agg_fail_count(a).  While there are any: grow the table so that they fit even if each is a
-// new group (a full slice refuses rows below the admission limit, so at least double: its keys then split between two
-// slices), gather them into a chunk of their own and run launch(sub_vt, rows, fail_list, fail_count) over it, which
-// refuses into the same list -- the gather has read it by then.  Leaves ngroups_host current and the flags clear.
-template <typename Launch>
-static int32_t agg_retry_rows(sr_agg* a, const VTab& vt, Launch&& launch) {
-    sr_ctx* ctx = a->ctx;
-    VTab cur = vt;
-    for (int k = 0;; k ^= 1) {
-        SR_CUDA(ctx, cudaMemcpyAsync(ctx->pinned + 8, a->counters.p, 56, cudaMemcpyDeviceToHost, ctx->stream));
-        SR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        a->ngroups_host = (int64_t)ctx->pinned[8];
-        const uint64_t failed = ctx->pinned[8 + 6];
-        if (failed == 0) {
-            if (((const int32_t*)(ctx->pinned + 9))[0]) return sr_fail(ctx, SR_ERR_STATE, "aggregate hash table overflow (internal)");
+// A launch has appended the entries (rows, merged slots, selection entries) that a full 256-slot slice refused -- they
+// applied nothing -- to a list, counted at agg_counters(a)->refused.  While there are any: grow the table so that they fit
+// even if each is a new group (a full slice refuses entries below the admission limit, so at least double: its keys then
+// split between two slices), zero the count and run relaunch(refused) over them, which refuses into the count again.
+// Leaves ngroups_host current and the flags clear.
+template <typename Relaunch>
+static int32_t agg_retry_refused(sr_agg* a, Relaunch&& relaunch) {
+    while (true) {
+        AggCounters st;
+        SR_TRY(agg_read_status(a, &st));
+        if (st.refused == 0) {
+            if (st.flags[0]) return sr_fail(a->ctx, SR_ERR_STATE, "aggregate hash table overflow (internal)");
             return SR_OK;
         }
-        uint64_t cap = a->host.cap * 2;
-        while ((uint64_t)a->ngroups_host + failed > cap / 2) cap *= 2;
-        if (cap > (1ull << 33)) return sr_fail(ctx, SR_ERR_OUT_OF_MEMORY, "aggregate table would exceed 2^33 slots; push smaller batches");
-        SR_CUDA(ctx, cudaMemsetAsync((uint8_t*)a->counters.p + 8, 0, 8, ctx->stream)); // overflow / range flags
-        SR_TRY(agg_grow(a, cap));
-        VTab sub;
-        SR_TRY(vtab_gather(ctx, cur, a->fail_list.as<uint32_t>(), (int64_t)failed, &a->retry_cols[k], &sub));
-        cur = sub;
-        SR_CUDA(ctx, cudaMemsetAsync(agg_fail_count(a), 0, 8, ctx->stream));
-        SR_TRY(launch(cur, (int64_t)failed, a->fail_list.as<uint32_t>(), agg_fail_count(a)));
+        SR_TRY(agg_clear_flags(a));
+        SR_TRY(agg_grow_to_fit(a, st.refused, 2, true));
+        SR_CUDA(a->ctx, cudaMemsetAsync(&agg_counters(a)->refused, 0, sizeof(st.refused), a->ctx->stream));
+        SR_TRY(relaunch(st.refused));
     }
+}
+
+// launch(vt, n, fail_rows, fail_count), a one-pass kernel over rows [0, n) of `vt` that appends the rows it refuses to
+// fail_rows, then the same kernel over the refused rows gathered into a chunk of their own (which refuses into the same
+// list: the gather has read it by then) until none is refused
+template <typename Launch>
+static int32_t agg_push_rows(sr_agg* a, const VTab& vt, int64_t n, Launch&& launch) {
+    sr_ctx* ctx = a->ctx;
+    SR_TRY(a->fail_list.reserve(ctx, sizeof(uint32_t) * (size_t)n));
+    SR_CUDA(ctx, cudaMemsetAsync(&agg_counters(a)->refused, 0, sizeof(AggCounters::refused), ctx->stream));
+    SR_TRY(launch(vt, n, a->fail_list.as<uint32_t>(), &agg_counters(a)->refused));
+    VTab cur = vt;
+    int k = 0;
+    return agg_retry_refused(a, [&](uint64_t m) -> int32_t {
+        VTab sub;
+        SR_TRY(vtab_gather(ctx, cur, a->fail_list.as<uint32_t>(), (int64_t)m, &a->retry_cols[k], &sub));
+        cur = sub;
+        k ^= 1;
+        return launch(cur, (int64_t)m, a->fail_list.as<uint32_t>(), &agg_counters(a)->refused);
+    });
 }
 
 static int32_t agg_push_vtab(sr_agg* a, const VTab& vt, int64_t n) {
@@ -1540,34 +1589,67 @@ static int32_t agg_push_vtab(sr_agg* a, const VTab& vt, int64_t n) {
     }
     if ((uint64_t)a->ngroups_host + (uint64_t)n <= h.limit) {
         // below the admission limit: one fused pass; the rows a full slice refuses are pushed again after a growth
-        SR_TRY(a->fail_list.reserve(ctx, sizeof(uint32_t) * (size_t)n));
-        SR_CUDA(ctx, cudaMemsetAsync(agg_fail_count(a), 0, 8, ctx->stream));
-        const auto launch = [&](const VTab& v, int64_t m, uint32_t* fail_rows, unsigned long long* fail_count) -> int32_t {
+        return agg_push_rows(a, vt, n, [&](const VTab& v, int64_t m, uint32_t* fail_rows, unsigned long long* fail_count) -> int32_t {
             srd::k_agg_push<false><<<std::min(grid_for(m, srd::AGG_BLOCK), ctx->num_sms * 8), srd::AGG_BLOCK, 0, ctx->stream>>>(
                     (const srd::AggDev*)a->dev.p, v, m, nullptr, nullptr, fail_rows, fail_count);
             SR_LAUNCH_CHECK(ctx);
             return SR_OK;
-        };
-        SR_TRY(launch(vt, n, a->fail_list.as<uint32_t>(), agg_fail_count(a)));
-        return agg_retry_rows(a, vt, launch);
+        });
     }
     // two passes: find/insert slots (growing the table until every row is placed), then update
     SR_TRY(a->slots_tmp.reserve(ctx, sizeof(int64_t) * (size_t)n));
     while (true) {
         srd::k_agg_push<false><<<grid, srd::AGG_BLOCK, 0, ctx->stream>>>((const srd::AggDev*)a->dev.p, vt, n, a->slots_tmp.as<long long>(), nullptr, nullptr, nullptr);
         SR_LAUNCH_CHECK(ctx);
-        uint64_t ng;
-        int32_t ovf, bad;
-        SR_TRY(agg_read_counters(a, &ng, &ovf, &bad));
-        a->ngroups_host = (int64_t)ng;
-        if (!ovf) break;
-        if (a->host.cap >= (1ull << 33)) return sr_fail(ctx, SR_ERR_OUT_OF_MEMORY, "aggregate table would exceed 2^33 slots");
-        SR_CUDA(ctx, cudaMemsetAsync((uint8_t*)a->counters.p + 8, 0, 8, ctx->stream));
-        SR_TRY(agg_grow(a, a->host.cap * 4));
+        AggCounters st;
+        SR_TRY(agg_read_status(a, &st));
+        if (!st.flags[0]) break;
+        SR_TRY(agg_clear_flags(a));
+        SR_TRY(agg_grow_to_fit(a, 0, 4, true));
     }
     srd::k_agg_push<false><<<grid, srd::AGG_BLOCK, 0, ctx->stream>>>((const srd::AggDev*)a->dev.p, vt, n, nullptr, a->slots_tmp.as<long long>(), nullptr, nullptr);
     SR_LAUNCH_CHECK(ctx);
     return SR_OK;
+}
+
+// merge the states of `o` (compiled, same descriptor) into `a`
+static int32_t agg_merge(sr_agg* a, sr_agg* o) {
+    sr_ctx* ctx = a->ctx;
+    if (!a->compiled) { // adopt other's compiled layout with fresh tables
+        a->reg = o->reg;
+        a->host = o->host;
+        SR_TRY(agg_setup_tables(a, o->host.cap));
+    }
+    const srd::AggDev& oh = o->host;
+    const bool hash = !a->host.dense && a->host.num_keys > 0;
+    for (int f = 0; f < oh.num_fns; f++)
+        if (oh.fns[f].track_n && !a->host.fns[f].track_n && a->host.fns[f].mode != srd::M_COUNT_STAR && a->host.fns[f].mode != srd::M_COUNT)
+            SR_TRY(agg_start_track_n(a, f));
+    if (hash) {
+        AggCounters ost;
+        SR_TRY(agg_read_status(o, &ost));
+        SR_TRY(agg_grow_to_fit(a, ost.ngroups, 4, false));
+    }
+    a->table_touched = true;
+    const auto merge = [&](const unsigned long long* slots_in, uint64_t total) -> int32_t {
+        srd::k_agg_merge<<<std::min(grid_for((int64_t)total, 256), ctx->num_sms * 16), 256, 0, ctx->stream>>>(
+                (const srd::AggDev*)o->dev.p, (const srd::AggDev*)a->dev.p, slots_in, total, a->fail_list.as<unsigned long long>(), &agg_counters(a)->refused);
+        SR_LAUNCH_CHECK(ctx);
+        return SR_OK;
+    };
+    const uint64_t total = srd::agg_slots(oh);
+    if (!hash) return merge(nullptr, total);
+    // a slot of `o` that a full 256-slot slice refuses merges nothing: it is listed and merged again after a growth
+    SR_TRY(a->fail_list.reserve(ctx, sizeof(uint64_t) * (size_t)total));
+    SR_CUDA(ctx, cudaMemsetAsync(&agg_counters(a)->refused, 0, sizeof(AggCounters::refused), ctx->stream));
+    SR_TRY(merge(nullptr, total));
+    DevBuf retry;
+    return agg_retry_refused(a, [&](uint64_t m) -> int32_t {
+        // the refused slots become the input, the old input list takes the next refusals
+        SR_TRY(retry.reserve(ctx, sizeof(uint64_t) * (size_t)m));
+        std::swap(a->fail_list, retry);
+        return merge(retry.as<unsigned long long>(), m);
+    });
 }
 
 static int32_t agg_finish_output(sr_agg* a) {
@@ -1614,15 +1696,13 @@ static int32_t agg_finish_output(sr_agg* a) {
     SR_TRY(a->block_offsets.reserve(ctx, sizeof(uint64_t) * (size_t)blocks));
     srd::k_agg_count<<<blocks, srd::EMIT_BLOCK, 0, ctx->stream>>>((const srd::AggDev*)a->dev.p, total, a->block_counts.as<uint32_t>());
     SR_LAUNCH_CHECK(ctx);
-    // one synchronisation: the table's status counters are read back with the row count
-    SR_CUDA(ctx, cudaMemcpyAsync(ctx->pinned + 8, a->counters.p, 16, cudaMemcpyDeviceToHost, ctx->stream));
+    // one synchronisation: the table's status is read back with the row count
+    const AggCounters* st;
+    SR_TRY(agg_fetch_status(a, &st));
     int64_t rows = 0;
     SR_TRY(scan_counts(ctx, &a->scan_scratch, a->block_counts.as<uint32_t>(), blocks, a->block_offsets.as<uint64_t>(), &rows));
-    {
-        const int32_t* fl = (const int32_t*)(ctx->pinned + 9);
-        if (fl[1]) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "a group-by value fell outside the declared group_min/group_max range");
-        if (fl[0]) return sr_fail(ctx, SR_ERR_STATE, "aggregate hash table overflow (internal)");
-    }
+    if (st->flags[1]) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "a group-by value fell outside the declared group_min/group_max range");
+    if (st->flags[0]) return sr_fail(ctx, SR_ERR_STATE, "aggregate hash table overflow (internal)");
     const int nc = d.num_group_keys + d.num_fns;
     a->out_cols.resize(nc); // kept across finish/reset cycles: a repeated query pays no cudaMalloc/cudaFree
     srd::EmitArgs ea;

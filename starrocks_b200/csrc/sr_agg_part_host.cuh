@@ -65,17 +65,15 @@ static uint64_t aggp_region_cap(double mean) {
 // admission limit or a full slice -- grow the table and re-apply them.  Leaves ngroups_host current.
 static int32_t aggp_apply_l2_drain(sr_agg* a, const srd::PartPlan& pl, const unsigned long long* rec, int64_t max_records) {
     sr_ctx* ctx = a->ctx;
-    unsigned long long* fail_count = a->counters.as<unsigned long long>() + 4;
+    unsigned long long* fail_count = &agg_counters(a)->part_fail;
     while (true) {
-        SR_CUDA(ctx, cudaMemcpyAsync(ctx->pinned + 8, a->counters.p, 48, cudaMemcpyDeviceToHost, ctx->stream));
-        SR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        a->ngroups_host = (int64_t)ctx->pinned[8];
-        const uint64_t failed = ctx->pinned[8 + 4];
+        AggCounters st;
+        SR_TRY(agg_read_status(a, &st));
+        const uint64_t failed = st.part_fail;
         if (failed == 0) break;
-        if (a->host.cap >= (1ull << 33)) return sr_fail(ctx, SR_ERR_OUT_OF_MEMORY, "aggregate table would exceed 2^33 slots");
-        SR_CUDA(ctx, cudaMemsetAsync((uint8_t*)a->counters.p + 8, 0, 8, ctx->stream)); // overflow / range flags
-        SR_CUDA(ctx, cudaMemsetAsync(fail_count, 0, 8, ctx->stream));
-        SR_TRY(agg_grow(a, a->host.cap * 2));
+        SR_TRY(agg_clear_flags(a));
+        SR_CUDA(ctx, cudaMemsetAsync(fail_count, 0, sizeof(st.part_fail), ctx->stream));
+        SR_TRY(agg_grow_to_fit(a, 0, 2, true));
         SR_TRY(a->part_fail64b.reserve(ctx, sizeof(uint64_t) * (size_t)std::min<int64_t>((int64_t)failed, max_records)));
         const int agrid = std::min(grid_for((int64_t)failed, srd::AGG_BLOCK), ctx->num_sms * 8);
         srd::k_aggp_apply_l2<<<agrid, srd::AGG_BLOCK, 0, ctx->stream>>>((const srd::AggDev*)a->dev.p, pl, rec, 0, (int64_t)failed, a->part_fail64.as<uint64_t>(), 0, 0,
@@ -179,12 +177,12 @@ static int32_t agg_push_partitioned(sr_agg* a, const VTab& vt, int64_t n, bool f
         uint32_t* cursor1 = cursor + P;
         unsigned long long* rec_final = a->part_rec[0].as<unsigned long long>();
         unsigned long long* rec_mid = pl.bits2 ? a->part_rec[1].as<unsigned long long>() : nullptr;
-        unsigned long long* fail_count = a->counters.as<unsigned long long>() + 4;
-        unsigned long long* ovf_count = a->counters.as<unsigned long long>() + 5;
+        unsigned long long* fail_count = &agg_counters(a)->part_fail;
+        unsigned long long* ovf_count = &agg_counters(a)->part_ovf;
         const srd::AggDev* dev = (const srd::AggDev*)a->dev.p;
         const int grid2 = ctx->num_sms * 2;
         SR_CUDA(ctx, cudaMemsetAsync(cursor, 0, sizeof(uint32_t) * ((size_t)P + F1), ctx->stream));
-        SR_CUDA(ctx, cudaMemsetAsync(fail_count, 0, 16, ctx->stream));
+        SR_CUDA(ctx, cudaMemsetAsync(fail_count, 0, sizeof(AggCounters::part_fail) + sizeof(AggCounters::part_ovf), ctx->stream)); // and ovf_count
         srd::ScatterArgs sa;
         memset(&sa, 0, sizeof(sa));
         sa.row_base = done;
@@ -236,12 +234,11 @@ static int32_t agg_push_partitioned(sr_agg* a, const VTab& vt, int64_t n, bool f
             SR_LAUNCH_CHECK(ctx);
         }
         fresh = false;
-        SR_CUDA(ctx, cudaMemcpyAsync(ctx->pinned + 8, a->counters.p, 48, cudaMemcpyDeviceToHost, ctx->stream));
-        SR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        a->ngroups_host = (int64_t)ctx->pinned[8];
-        failed_buckets = ctx->pinned[8 + 4];
-        overflowed = std::min<uint64_t>(ctx->pinned[8 + 5], (uint64_t)m);
-        SR_CUDA(ctx, cudaMemsetAsync(fail_count, 0, 8, ctx->stream));
+        AggCounters st;
+        SR_TRY(agg_read_status(a, &st));
+        failed_buckets = st.part_fail;
+        overflowed = std::min<uint64_t>(st.part_ovf, (uint64_t)m);
+        SR_CUDA(ctx, cudaMemsetAsync(fail_count, 0, sizeof(st.part_fail), ctx->stream));
         if (!smem_mode || failed_buckets > 0 || overflowed > 0) SR_TRY(a->part_fail64.reserve(ctx, sizeof(uint64_t) * (size_t)m));
         if (!smem_mode || failed_buckets > 0) {
             // global-atomics apply: every bucket, or the buckets with a slice that filled up (after a growth)
@@ -253,8 +250,7 @@ static int32_t agg_push_partitioned(sr_agg* a, const VTab& vt, int64_t n, bool f
             }
             SR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
             if (smem_mode) {
-                if (a->host.cap >= (1ull << 33)) return sr_fail(ctx, SR_ERR_OUT_OF_MEMORY, "aggregate table would exceed 2^33 slots");
-                SR_TRY(agg_grow(a, a->host.cap * 2));
+                SR_TRY(agg_grow_to_fit(a, 0, 2, true));
             } else {
                 todo.resize((size_t)P);
                 for (int b = 0; b < P; b++) todo[(size_t)b] = (uint32_t)b;
@@ -280,10 +276,7 @@ static int32_t agg_push_partitioned(sr_agg* a, const VTab& vt, int64_t n, bool f
             SR_TRY(aggp_apply_l2_drain(a, pl, a->part_ovf.as<unsigned long long>(), m));
         }
         // keep the load below the admission limit for the pushes that follow
-        while ((uint64_t)a->ngroups_host > a->host.limit) {
-            if (a->host.cap >= (1ull << 33)) return sr_fail(ctx, SR_ERR_OUT_OF_MEMORY, "aggregate table would exceed 2^33 slots");
-            SR_TRY(agg_grow(a, a->host.cap * 2));
-        }
+        SR_TRY(agg_grow_to_fit(a, 0, 2, false));
         a->partitioned_pushes++;
         done += m;
     }

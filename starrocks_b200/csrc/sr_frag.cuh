@@ -513,11 +513,11 @@ static int32_t frag_plan_pass_grids(sr_fragment* f) {
 }
 
 // slots of pass_counters (64-bit words): the entry count of every selection vector a push writes (the streaming pass's,
-// then one per gather pass), and the two fail counters of the final pass's hash-table retries (live and spare)
+// then one per gather pass), and the entry count of the input of a hash-table retry of the final pass
 constexpr int PASS_CNT_SEL = 0;
-constexpr int PASS_CNT_FAIL = 8;
+constexpr int PASS_CNT_RETRY = 8;
 constexpr int PASS_CNT_WORDS = 16;
-static_assert(PASS_CNT_SEL + SR_MAX_FRAG_JOINS <= PASS_CNT_FAIL && PASS_CNT_FAIL + 2 <= PASS_CNT_WORDS, "pass counter layout");
+static_assert(PASS_CNT_SEL + SR_MAX_FRAG_JOINS <= PASS_CNT_RETRY && PASS_CNT_RETRY + 1 <= PASS_CNT_WORDS, "pass counter layout");
 
 // selection-vector mode; reach_pred0: the sampled fraction of the rows that pass scan conjunct 0
 static int32_t frag_plan_passes(sr_fragment* f, double reach_pred0) {
@@ -691,10 +691,7 @@ static int32_t frag_push(sr_fragment* f, const sr_chunk_view* fact) {
         // from the sampled survivor estimate (x2 + slack) and re-apply the rows the table refused after growing it.
         uint64_t want = (uint64_t)n;
         if (f->selective) want = std::min<uint64_t>((uint64_t)n, (uint64_t)((double)n * std::min(1.0, f->est_rate) * 2.0) + (1u << 16));
-        while ((uint64_t)a->ngroups_host + want > a->host.limit) {
-            if (a->host.cap >= (1ull << 33)) return sr_fail(ctx, SR_ERR_OUT_OF_MEMORY, "aggregate table would exceed 2^33 slots; push smaller batches");
-            SR_TRY(agg_grow(a, a->host.cap * 4));
-        }
+        SR_TRY(agg_grow_to_fit(a, want, 4, false));
     }
     if (f->selective) {
         const srd::FragDev* fdev = (const srd::FragDev*)f->dev.p;
@@ -740,39 +737,26 @@ static int32_t frag_push(sr_fragment* f, const sr_chunk_view* fact) {
             k++;
         }
         SR_CUDA(ctx, cudaEventRecord(f->ev[2], ctx->stream));
-        // hash table: rows it refuses go to the other selection buffer (free by now) and are retried after a growth
-        if (hash) SR_TRY(f->sel[cur ^ 1].reserve(ctx, sizeof(srd::SelEntry) * ((size_t)n + slack)));
-        unsigned long long* fail_count = cnt + PASS_CNT_FAIL;
-        unsigned long long* spare_count = fail_count + 1;
-        SR_TRY(frag_launch_final(f, vt, f->sel[cur].as<srd::SelEntry>(), sel_count + k, hash ? f->sel[cur ^ 1].as<srd::SelEntry>() : nullptr, fail_count));
+        // hash table: entries it refuses go to the other selection buffer (free by now) and are retried after a growth
+        unsigned long long* refused = &agg_counters(a)->refused;
+        if (hash) {
+            SR_TRY(f->sel[cur ^ 1].reserve(ctx, sizeof(srd::SelEntry) * ((size_t)n + slack)));
+            SR_CUDA(ctx, cudaMemsetAsync(refused, 0, sizeof(*refused), ctx->stream));
+        }
+        SR_TRY(frag_launch_final(f, vt, f->sel[cur].as<srd::SelEntry>(), sel_count + k, hash ? f->sel[cur ^ 1].as<srd::SelEntry>() : nullptr, refused));
         SR_CUDA(ctx, cudaEventRecord(f->ev[3], ctx->stream));
         f->timed_push = true;
-        if (hash) {
-            while (true) {
-                uint64_t ng;
-                int32_t ovf, bad;
-                SR_CUDA(ctx, cudaMemcpyAsync(ctx->pinned + 16, fail_count, 8, cudaMemcpyDeviceToHost, ctx->stream));
-                SR_TRY(agg_read_counters(a, &ng, &ovf, &bad)); // synchronises
-                a->ngroups_host = (int64_t)ng;
-                const uint64_t failed = ctx->pinned[16];
-                if (failed == 0) break;
-                // grow so that the refused rows fit even if each of them is a new group, then re-apply them
-                SR_CUDA(ctx, cudaMemsetAsync((uint8_t*)a->counters.p + 8, 0, 8, ctx->stream)); // overflow / range flags
-                // (always at least doubled: a refused row of a one-to-many join may bring several new groups, and a
-                // full 256-slot slice refuses rows below the admission limit)
-                uint64_t cap = a->host.cap * 2;
-                while ((uint64_t)a->ngroups_host + failed > cap / 2) cap *= 2;
-                if (cap > (1ull << 33)) return sr_fail(ctx, SR_ERR_OUT_OF_MEMORY, "aggregate table would exceed 2^33 slots; push smaller batches");
-                SR_TRY(agg_grow(a, cap));
-                // the fail list and its counter become the input, the old input buffer and the spare counter the new
-                // fail list; the launch runs the kernel of the first one (a hash aggregate's, see frag_launch_final)
-                cur ^= 1;
-                std::swap(fail_count, spare_count);
-                SR_CUDA(ctx, cudaMemsetAsync(fail_count, 0, 8, ctx->stream));
-                SR_TRY(frag_launch_final(f, vt, f->sel[cur].as<srd::SelEntry>(), spare_count, f->sel[cur ^ 1].as<srd::SelEntry>(), fail_count));
-            }
-        }
-        return SR_OK;
+        if (!hash) return SR_OK;
+        // the refused entries become the input and the old input buffer the fail list; the launch runs the kernel of the
+        // first one (a hash aggregate's, see frag_launch_final).  The kernels read the input's entry count from the
+        // device, where the loop has zeroed the table's count, so it is copied in from the host.
+        unsigned long long* retry_count = cnt + PASS_CNT_RETRY;
+        return agg_retry_refused(a, [&](uint64_t m) -> int32_t {
+            ctx->pinned[16] = m;
+            SR_CUDA(ctx, cudaMemcpyAsync(retry_count, ctx->pinned + 16, sizeof(m), cudaMemcpyHostToDevice, ctx->stream));
+            cur ^= 1;
+            return frag_launch_final(f, vt, f->sel[cur].as<srd::SelEntry>(), retry_count, f->sel[cur ^ 1].as<srd::SelEntry>(), refused);
+        });
     }
     // a hash table refuses a row only when its 256-slot slice is full (the table was sized for every row being a new
     // group): the refused fact rows are gathered and run through the cascade again after a growth.  That is exact because
@@ -790,8 +774,5 @@ static int32_t frag_push(sr_fragment* f, const sr_chunk_view* fact) {
         return SR_OK;
     };
     if (!hash) return launch(vt, n, nullptr, nullptr);
-    SR_TRY(a->fail_list.reserve(ctx, sizeof(uint32_t) * (size_t)n));
-    SR_CUDA(ctx, cudaMemsetAsync(agg_fail_count(a), 0, 8, ctx->stream));
-    SR_TRY(launch(vt, n, a->fail_list.as<uint32_t>(), agg_fail_count(a)));
-    return agg_retry_rows(a, vt, launch);
+    return agg_push_rows(a, vt, n, launch);
 }

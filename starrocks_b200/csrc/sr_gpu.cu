@@ -858,7 +858,7 @@ static int32_t agg_reset_impl(sr_agg* a) {
     for (sr_agg* c : a->distinct)
         if (c) SR_TRY(agg_reset_impl(c));
     if (!a->compiled) return SR_OK;
-    SR_CUDA(ctx, cudaMemsetAsync(a->counters.p, 0, 64, ctx->stream));
+    SR_CUDA(ctx, cudaMemsetAsync(agg_counters(a), 0, sizeof(AggCounters), ctx->stream));
     return agg_init_tables(ctx, a->host);
 }
 
@@ -988,11 +988,9 @@ int64_t sr_agg_current_groups(sr_agg* a) {
     sr_ctx* ctx = a->ctx;
     SR_BIND(ctx);
     if (!a->compiled || a->host.dense || a->host.num_keys == 0) return 0;
-    uint64_t ng;
-    int32_t ovf, bad;
-    SR_TRY(agg_read_counters(a, &ng, &ovf, &bad));
-    a->ngroups_host = (int64_t)ng;
-    return (int64_t)ng;
+    AggCounters st;
+    SR_TRY(agg_read_status(a, &st));
+    return (int64_t)st.ngroups;
 }
 
 // the body of sr_agg_convert_to_states; *vt_out receives the bound value table of the staged chunk
@@ -1110,55 +1108,7 @@ int32_t sr_agg_merge(sr_agg* a, sr_agg* o) {
     if (desc_has_distinct(&a->desc)) return sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "COUNT(DISTINCT) states do not merge; shuffle on the group keys instead");
     if (!o->compiled) return SR_OK; // nothing was pushed into `other`
     if (memcmp(&a->desc, &o->desc, sizeof(sr_agg_desc)) != 0) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "merge needs identical descriptors");
-    if (!a->compiled) { // adopt other's compiled layout with fresh tables
-        a->reg = o->reg;
-        a->host = o->host;
-        SR_TRY(agg_setup_tables(a, o->host.cap));
-    }
-    const srd::AggDev& oh = o->host;
-    const bool hash = !a->host.dense && a->host.num_keys > 0;
-    for (int f = 0; f < oh.num_fns; f++)
-        if (oh.fns[f].track_n && !a->host.fns[f].track_n && a->host.fns[f].mode != srd::M_COUNT_STAR && a->host.fns[f].mode != srd::M_COUNT)
-            SR_TRY(agg_start_track_n(a, f));
-    if (hash) {
-        uint64_t ng_o;
-        int32_t ovf, bad;
-        SR_TRY(agg_read_counters(o, &ng_o, &ovf, &bad));
-        while ((uint64_t)a->ngroups_host + ng_o > a->host.limit) SR_TRY(agg_grow(a, a->host.cap * 4));
-    }
-    a->table_touched = true;
-    // a slot of `o` that a full 256-slot slice refuses merges nothing: it is listed and merged again after a growth
-    uint64_t total = srd::agg_slots(oh);
-    const unsigned long long* slots_in = nullptr;
-    unsigned long long* fail_count = agg_fail_count(a);
-    DevBuf retry;
-    if (hash) SR_TRY(a->fail_list.reserve(ctx, sizeof(uint64_t) * (size_t)total));
-    while (true) {
-        if (hash) SR_CUDA(ctx, cudaMemsetAsync(fail_count, 0, 8, ctx->stream));
-        srd::k_agg_merge<<<std::min(grid_for((int64_t)total, 256), ctx->num_sms * 16), 256, 0, ctx->stream>>>(
-                (const srd::AggDev*)o->dev.p, (const srd::AggDev*)a->dev.p, slots_in, total, a->fail_list.as<unsigned long long>(), fail_count);
-        SR_LAUNCH_CHECK(ctx);
-        if (!hash) return SR_OK;
-        SR_CUDA(ctx, cudaMemcpyAsync(ctx->pinned + 8, a->counters.p, 56, cudaMemcpyDeviceToHost, ctx->stream));
-        SR_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        a->ngroups_host = (int64_t)ctx->pinned[8];
-        const uint64_t failed = ctx->pinned[8 + 6];
-        if (failed == 0) {
-            if (((const int32_t*)(ctx->pinned + 9))[0]) return sr_fail(ctx, SR_ERR_STATE, "aggregate hash table overflow during merge (internal)");
-            return SR_OK;
-        }
-        // at least doubled: the refused keys of a full slice then split between two slices
-        uint64_t cap = a->host.cap * 2;
-        while ((uint64_t)a->ngroups_host + failed > cap / 2) cap *= 2;
-        if (cap > (1ull << 33)) return sr_fail(ctx, SR_ERR_OUT_OF_MEMORY, "aggregate table would exceed 2^33 slots");
-        SR_CUDA(ctx, cudaMemsetAsync((uint8_t*)a->counters.p + 8, 0, 8, ctx->stream)); // overflow / range flags
-        SR_TRY(agg_grow(a, cap));
-        // the refused slots become the input, the old input list takes the next refusals
-        SR_TRY(retry.reserve(ctx, sizeof(uint64_t) * (size_t)failed));
-        std::swap(a->fail_list, retry);
-        slots_in = retry.as<unsigned long long>();
-        total = failed;
-    }
+    return agg_merge(a, o);
 }
 
 // ------------------------------------------------------------------ fragment
