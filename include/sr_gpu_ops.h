@@ -665,8 +665,8 @@ typedef struct sr_fragment_plan {
     double pred_rate; /* fraction of sampled rows passing the scan conjuncts */
 } sr_fragment_plan;
 #define SR_FINAL_PASS_NONE 0    /* no push yet, or the fused cascade kernel */
-#define SR_FINAL_PASS_GENERIC 1 /* k_frag_gather_agg: any join, aggregate and expression */
-#define SR_FINAL_PASS_EXPAND 2  /* k_frag_gather_agg_expand: one-to-many joins */
+#define SR_FINAL_PASS_GENERIC 1 /* k_frag_gather_agg<EXPAND = false>: any join, aggregate and expression */
+#define SR_FINAL_PASS_EXPAND 2  /* k_frag_gather_agg<EXPAND = true>: one-to-many joins */
 #define SR_FINAL_PASS_DENSE 3   /* k_frag_final_dense: slot-digit directories, batched rows, dense shared-memory aggregate */
 int32_t sr_fragment_get_plan(sr_fragment* frag, sr_fragment_plan* plan);
 /* device time of the passes of the LAST push in selection-vector mode (CUDA events on the context's

@@ -51,9 +51,10 @@ section("k_frag_stream_tests<false> (streaming pass, LDG form): 128-bit streamin
         "k_frag_stream_testsILb0", [r"LDG\.E\.NA\.128", r"@P\d\s+LDG\.E\.CONSTANT", r"VIMNMX|VIADDMNMX", r"STG\.E\.64", r"VOTE|POPC"])
 section("k_frag_gather_join (selection-vector pass of one join): sector gathers of the key column through the selection vector", "k_frag_gather_join",
         [r"LDG", r"STG", r"VOTE|POPC", r"ATOMG"], 16)
-section("k_frag_gather_agg<SMEM_AGG=true> (final pass): dependent gathers, shared-memory accumulators (ATOMS / REDS on 32-bit halves)", "k_frag_gather_aggILb1ELb0",
+section("k_frag_gather_agg<SMEM_AGG=true> (final pass): dependent gathers, shared-memory accumulators (ATOMS / REDS on 32-bit halves)", "k_frag_gather_aggILb1ELb0ELb0",
         [r"ATOMS|REDS|RED\.", r"LDG\.E\.CONSTANT", r"LDG\.E\.NA"])
-section("k_frag_gather_agg_expand (final pass with one-to-many joins): chain walk through next[] (LDG.E.CONSTANT), global reductions", "k_frag_gather_agg_expand",
+section("k_frag_gather_agg<EXPAND=true> (final pass with one-to-many joins): chain walk through next[] (LDG.E.CONSTANT), global reductions",
+        "k_frag_gather_aggILb0ELb0ELb1",
         [r"LDG\.E\.CONSTANT", r"RED\.|ATOMG"], 16)
 section("k_aggp_scatter<2, CHUNK_SIMPLE> (level-1 scatter of the partitioned aggregate): streaming loads, shared-memory rank atomics (ATOMS), 128-bit record "
         "stores, L2 prefetch of the next tile (CCTL)", "k_aggp_scatterILi2ELi2", [r"ATOMS", r"ATOMG", r"STG\.E\.128", r"CCTL|PREFETCH", r"LDG\.E\.NA"])

@@ -65,7 +65,7 @@ struct sr_fragment {
     int cascade_grid = 0;
     // selective mode (sr_frag_pass.cuh): streaming pass -> gather passes -> final pass, planned by frag_plan_passes
     bool selective = false;
-    bool expand = false; // some INNER join has duplicate build keys: selection-vector passes + k_frag_gather_agg_expand
+    bool expand = false; // some INNER join has duplicate build keys: selection-vector passes + k_frag_gather_agg<false, SINGLE, true>
     srd::PassDev pass;
     std::vector<int> gather_joins; // probe positions that get a pass of their own
     DevBuf sel[2], pass_counters;
@@ -484,6 +484,20 @@ static void frag_plan_final_vals(sr_fragment* f) {
     f->pass.num_final_vals = (int8_t)std::min<size_t>(need.size(), 127);
 }
 
+// the instantiation of the generic final pass (k_frag_gather_agg) that runs this fragment, and its dynamic shared memory
+struct FinalKernel {
+    void (*fn)(const srd::FragDev*, const srd::AggDev*, const srd::PassDev, const VTab, const srd::SelEntry*, const unsigned long long*, srd::SelEntry*,
+               unsigned long long*);
+    size_t smem;
+};
+static FinalKernel frag_final_kernel(const sr_fragment* f) {
+    const bool single = f->agg->host.num_keys == 0;
+    if (f->expand) return {single ? srd::k_frag_gather_agg<false, true, true> : srd::k_frag_gather_agg<false, false, true>, 0};
+    if (single) return {srd::k_frag_gather_agg<false, true, false>, 0};
+    if (f->smem_agg) return {srd::k_frag_gather_agg<true, false, false>, f->agg->smem_bytes};
+    return {srd::k_frag_gather_agg<false, false, false>, 0};
+}
+
 // launch grids of the passes (and the dynamic shared-memory limit of the streaming kernels)
 static int32_t frag_plan_pass_grids(sr_fragment* f) {
     sr_ctx* ctx = f->ctx;
@@ -499,14 +513,8 @@ static int32_t frag_plan_pass_grids(sr_fragment* f) {
     // gather passes: exactly one wave of resident CTAs (grid-stride loops; a partial second wave only adds a tail)
     int gj = 0, ga = 0;
     SR_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&gj, srd::k_frag_gather_join, srd::GATHER_BLOCK, 0));
-    if (f->expand)
-        SR_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ga, srd::k_frag_gather_agg_expand, srd::GATHER_BLOCK, 0));
-    else if (f->agg->host.num_keys == 0)
-        SR_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ga, srd::k_frag_gather_agg<false, true>, srd::GATHER_BLOCK, 0));
-    else if (f->smem_agg)
-        SR_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ga, srd::k_frag_gather_agg<true>, srd::GATHER_BLOCK, f->agg->smem_bytes));
-    else
-        SR_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ga, srd::k_frag_gather_agg<false>, srd::GATHER_BLOCK, 0));
+    const FinalKernel fk = frag_final_kernel(f);
+    SR_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ga, fk.fn, srd::GATHER_BLOCK, fk.smem));
     f->gather_grid = std::max(gj, 1) * ctx->num_sms;
     f->final_grid = std::max(ga, 1) * ctx->num_sms;
     return SR_OK;
@@ -624,9 +632,10 @@ static int32_t frag_plan(sr_fragment* f, const VTab& vt, int64_t n) {
     return SR_OK;
 }
 
-// The final pass of selective mode over the selection vector `in` (its entry count at `in_count`).  A hash aggregate is
-// neither dense nor kept in shared memory and has group keys, so it always runs k_frag_gather_agg_expand or
-// k_frag_gather_agg<false>: the two that append the rows its table refuses to `fail_list` (counted at `fail_count`).
+// The final pass of selective mode over the selection vector `in` (its entry count at `in_count`): k_frag_final_dense
+// when the push allows it, else the instantiation of k_frag_gather_agg that frag_final_kernel picks.  A hash aggregate is
+// neither dense nor kept in shared memory and has group keys, so it always runs k_frag_gather_agg<false, false, EXPAND>,
+// which appends the rows its table refuses to `fail_list` (counted at `fail_count`).
 static int32_t frag_launch_final(sr_fragment* f, const VTab& vt, const srd::SelEntry* in, const unsigned long long* in_count, srd::SelEntry* fail_list,
                                  unsigned long long* fail_count) {
     sr_ctx* ctx = f->ctx;
@@ -650,14 +659,10 @@ static int32_t frag_launch_final(sr_fragment* f, const VTab& vt, const srd::SelE
         fp.flags = ah.flags;
         fp.rows_passed = f->host.rows_passed;
         srd::k_frag_final_dense<srd::FINAL_ROWS><<<f->final_dense_grid, srd::GATHER_BLOCK, a->smem_bytes, ctx->stream>>>(fp, in, in_count);
-    } else if (f->expand)
-        srd::k_frag_gather_agg_expand<<<f->final_grid, srd::GATHER_BLOCK, 0, ctx->stream>>>(fdev, adev, pass, vt, in, in_count, fail_list, fail_count);
-    else if (ah.num_keys == 0)
-        srd::k_frag_gather_agg<false, true><<<f->final_grid, srd::GATHER_BLOCK, 0, ctx->stream>>>(fdev, adev, pass, vt, in, in_count, nullptr, nullptr);
-    else if (f->smem_agg)
-        srd::k_frag_gather_agg<true><<<f->final_grid, srd::GATHER_BLOCK, a->smem_bytes, ctx->stream>>>(fdev, adev, pass, vt, in, in_count, nullptr, nullptr);
-    else
-        srd::k_frag_gather_agg<false><<<f->final_grid, srd::GATHER_BLOCK, 0, ctx->stream>>>(fdev, adev, pass, vt, in, in_count, fail_list, fail_count);
+    } else {
+        const FinalKernel fk = frag_final_kernel(f);
+        fk.fn<<<f->final_grid, srd::GATHER_BLOCK, fk.smem, ctx->stream>>>(fdev, adev, pass, vt, in, in_count, fail_list, fail_count);
+    }
     SR_LAUNCH_CHECK(ctx);
     return SR_OK;
 }

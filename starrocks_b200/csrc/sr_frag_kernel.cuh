@@ -139,6 +139,47 @@ __device__ __forceinline__ bool frag_join_hit(const FragJoinDev& fj, const uint3
     return join_lookup(fj.j, key) != 0;
 }
 
+// bitmap / hash test against the global copies only (gather passes do not stage bitmaps)
+__device__ __forceinline__ bool join_hit_global(const FragJoinDev& fj, int64_t key) {
+    if (fj.use_bitmap) {
+        if (key < fj.j.min_value || key > fj.j.max_value) return false;
+        const uint64_t idx = (uint64_t)(key - fj.j.min_value);
+        return (__ldg(fj.j.bitmap + (idx >> 5)) >> (idx & 31)) & 1u;
+    }
+    return join_lookup(fj.j, key) != 0;
+}
+
+// The joins of one row that reached a final pass, in probe order: joins [first_test, S) are tested (a NULL key, a key
+// without a build row or a clear bitmap bit fails the row), and every join whose payload is read downstream (need_head)
+// is looked up.  Fills ld.bidx with the build rows found and, when `head` is given, head[j] with the same chain heads (0
+// for a join not looked up).  Returns whether the row passed.  `joins` and `S` are read through references: the cascade
+// keeps them in its per-warp state in local memory, and re-reading them there per join keeps copies out of k_fragment's
+// registers (capped at 64, already spilling) across the walk.
+__device__ __forceinline__ bool frag_final_joins(const FragJoinDev* const& joins, const int& S, int first_test, FragLoader& ld, uint32_t* head) {
+    bool ok = true;
+#pragma unroll 1
+    for (int j = 0; j < S && ok; j++) {
+        if (head) head[j] = 0;
+        const bool test = j >= first_test;
+        if (!test && !joins[j].need_head) continue;
+        int64_t key;
+        const bool nul = ld.load(joins[j].key_value_id, key);
+        if (test && nul) {
+            ok = false;
+            break;
+        }
+        if (joins[j].need_head || !joins[j].use_bitmap) {
+            const uint32_t h = join_lookup(joins[j].j, key);
+            ld.bidx[j] = h;
+            if (head) head[j] = h;
+            if (test && h == 0) ok = false;
+        } else if (test) {
+            if (!join_hit_global(joins[j], key)) ok = false;
+        }
+    }
+    return ok;
+}
+
 // everything a warp needs to run the cascade (kept in registers / shared memory)
 struct Cascade {
     const VTab& vt;
@@ -186,14 +227,7 @@ struct Cascade {
     __device__ __forceinline__ void consume_final(uint32_t row32, bool valid) {
         if (valid) {
             FragLoader ld{vt, (int64_t)row32, {0, 0, 0, 0, 0, 0}, -1, 0};
-#pragma unroll 1
-            for (int j = 0; j < S; j++) {
-                if (joins[j].need_head) {
-                    int64_t key;
-                    ld.load(joins[j].key_value_id, key);
-                    ld.bidx[j] = join_lookup(joins[j].j, key);
-                }
-            }
+            frag_final_joins(joins, S, S, ld, nullptr); // the queue stages tested every join: lookups only
             const long long slot = agg_find_slot(ad, ld);
             if (slot >= 0) {
                 if (shared_acc)

@@ -69,16 +69,6 @@ __device__ __forceinline__ SelEntry sel_make(uint32_t row, int32_t carry) { retu
 
 #define SR_FINAL_PREFETCH 8
 
-// bitmap / hash test against the global copies only (gather passes do not stage bitmaps)
-__device__ __forceinline__ bool join_hit_global(const FragJoinDev& fj, int64_t key) {
-    if (fj.use_bitmap) {
-        if (key < fj.j.min_value || key > fj.j.max_value) return false;
-        const uint64_t idx = (uint64_t)(key - fj.j.min_value);
-        return (__ldg(fj.j.bitmap + (idx >> 5)) >> (idx & 31)) & 1u;
-    }
-    return join_lookup(fj.j, key) != 0;
-}
-
 // bitmap word of a row that is still alive (alive_bit != 0) and whose index lies in the table's range; 0 otherwise.  The
 // predicate is formed inside the asm block from the raw operands: handing a C++ bool in costs a select to 0 / 1 and a
 // compare back (ncu: 6.6 instructions per row on this line of the issue-bound streaming pass)
@@ -553,16 +543,40 @@ __global__ void __launch_bounds__(GATHER_BLOCK) k_frag_gather_join(const FragDev
 // Five CTAs per SM (48 registers) balance resident warps against spills.
 constexpr int GATHER_AGG_MIN_BLOCKS = 5;
 
+// the next combination of chain entries of a row's expanding joins, like an odometer: advance the last expanding join,
+// carry into the one before it when its chain ends.  False when every chain is back at its head.
+__device__ __forceinline__ bool frag_next_combination(const FragJoinDev* joins, int S, FragLoader& ld, const uint32_t* head) {
+#pragma unroll 1
+    for (int j = S - 1; j >= 0; j--) {
+        if (!joins[j].expand) continue;
+        const uint32_t nx = __ldg(joins[j].j.next + ld.bidx[j]);
+        if (nx) {
+            ld.bidx[j] = nx;
+            return true;
+        }
+        ld.bidx[j] = head[j];
+    }
+    return false;
+}
+
 // final pass: remaining joins inline, payload lookups, aggregate update.  SINGLE: no GROUP BY (its register state
 // would only cost the grouped instantiations spills).
-template <bool SMEM_AGG, bool SINGLE = false>
+// EXPAND: some joins have duplicate build keys (reference: JoinHashMap::_probe_from_ht one-to-many walk,
+// be/src/exec/join/join_hash_map.hpp:718-795 -- every probe row is emitted once per entry of the build chain of its
+// key).  The probe output is never materialised: the thread that owns a surviving fact row walks the chains of its
+// expanding joins like an odometer (last join fastest) and applies the aggregate once per combination, reading the
+// payload columns at the current chain entries, into global accumulators.
+template <bool SMEM_AGG, bool SINGLE, bool EXPAND>
 __global__ void __launch_bounds__(GATHER_BLOCK, GATHER_AGG_MIN_BLOCKS) k_frag_gather_agg(const FragDev* __restrict__ fdp, const AggDev* __restrict__ adp, const __grid_constant__ PassDev pd,
                                                                    const __grid_constant__ VTab vt, const SelEntry* __restrict__ sel_in,
                                                                    const unsigned long long* __restrict__ n_in_ptr, SelEntry* __restrict__ fail_list,
                                                                    unsigned long long* __restrict__ fail_count) {
+    static_assert(!(SMEM_AGG && EXPAND), "the expanding form accumulates in global memory");
     // Hash aggregate tables are sized from the SAMPLED survivor estimate, not for the worst case "every row is a new
     // group" (a 65 M-row batch would allocate and clear a 13 GB table for 0.2 M groups).  A row the table cannot admit
     // (admission limit) is appended to fail_list; the host grows the table and runs this kernel again over that list.
+    // A row is applied with all its combinations or not at all: with one combination its slot is found and applied in
+    // one step; with EXPAND a first walk only finds / inserts the group slots, so a refused row has applied nothing.
     extern __shared__ __align__(16) uint32_t smem[];
     __shared__ FragJoinDev s_joins[SR_MAX_FRAG_JOINS];
     const FragDev& fd = *fdp;
@@ -585,9 +599,8 @@ __global__ void __launch_bounds__(GATHER_BLOCK, GATHER_AGG_MIN_BLOCKS) k_frag_ga
     // kept in L2, so for host-resident input the prefetch only doubles the PCIe requests.
     const unsigned long long n_in = *n_in_ptr;
     unsigned long long passed = 0;
-    constexpr bool single = SINGLE;
     SingleAcc sacc;
-    if (single) single_acc_init(ad, sacc);
+    if (SINGLE) single_acc_init(ad, sacc);
     unsigned long long w_begin, w_end;
     warp_sel_range(n_in, w_begin, w_end);
     for (unsigned long long i = w_begin + lane_id(); i < w_end; i += 32) {
@@ -597,48 +610,50 @@ __global__ void __launch_bounds__(GATHER_BLOCK, GATHER_AGG_MIN_BLOCKS) k_frag_ga
         // (a variant that fetches every fact value of the row in one burst before the dependent lookups costs more
         // issue slots and registers than the latency it hides)
         FragLoader ld{vt, (int64_t)row, {0, 0, 0, 0, 0, 0}, pd.carry_join >= 0 ? (int32_t)pd.carry_value_id : -1, sel_carry(entry)};
-        bool ok = true;
-#pragma unroll 1
-        for (int j = 0; j < S && ok; j++) {
-            const FragJoinDev& fj = s_joins[j];
-            const bool test = j >= pd.final_first_join;
-            if (!test && !fj.need_head) continue;
-            int64_t key;
-            const bool nul = ld.load(fj.key_value_id, key);
-            if (test && nul) {
-                ok = false;
-                break;
-            }
-            if (fj.need_head || !fj.use_bitmap) {
-                const uint32_t head = join_lookup(fj.j, key);
-                ld.bidx[j] = head;
-                if (test && head == 0) ok = false;
-            } else if (test) {
-                if (!join_hit_global(fj, key)) ok = false;
-            }
-        }
-        if (!ok) continue;
-        if (single) { // no GROUP BY: the state lives in the thread, not behind an atomic
-            single_acc_row(ad, sacc, ld);
-        } else if (hash_table) {
+        uint32_t head[EXPAND ? SR_MAX_FRAG_JOINS : 1];
+        if (!frag_final_joins(s_joins, S, pd.final_first_join, ld, EXPAND ? head : nullptr)) continue;
+        auto hash_slot = [&]() {
             HKey key;
             agg_pack_key(ad, ld, key);
             bool inserted;
             const long long slot = agg_find_slot_key(ad, key, inserted, known_groups);
             agg_count_new_groups(ad, inserted, known_groups);
-            if (slot < 0) {
-                if (fail_list) fail_list[atomicAdd(fail_count, 1ull)] = entry; // retried after the table has grown
+            return slot;
+        };
+        if (EXPAND && hash_table) {
+            // a first walk only finds / inserts the group slots of every combination (the second finds the same slots:
+            // tables never shrink in between)
+            bool refused = false;
+            do {
+                refused = hash_slot() < 0;
+            } while (!refused && frag_next_combination(s_joins, S, ld, head));
+            if (refused) {
+                if (fail_list) fail_list[atomicAdd(fail_count, 1ull)] = entry;
                 continue;
             }
-            agg_apply_row<SMEM_AGG>(ad, acc, slot, ld);
-        } else {
-            const long long slot = agg_find_slot(ad, ld);
-            if (slot >= 0) agg_apply_row<SMEM_AGG>(ad, acc, slot, ld);
+#pragma unroll 1
+            for (int j = 0; j < S; j++) ld.bidx[j] = head[j]; // the odometer ends on the heads anyway; keeps the second walk independent of that
         }
-        passed++;
+        while (true) {
+            if (SINGLE) { // no GROUP BY: the state lives in the thread, not behind an atomic
+                single_acc_row(ad, sacc, ld);
+            } else if (hash_table) {
+                const long long slot = hash_slot();
+                if (slot < 0) {
+                    if (fail_list) fail_list[atomicAdd(fail_count, 1ull)] = entry; // retried after the table has grown
+                    break;
+                }
+                agg_apply_row<SMEM_AGG>(ad, acc, slot, ld);
+            } else {
+                const long long slot = agg_find_slot(ad, ld);
+                if (slot >= 0) agg_apply_row<SMEM_AGG>(ad, acc, slot, ld);
+            }
+            passed++;
+            if (!EXPAND || !frag_next_combination(s_joins, S, ld, head)) break;
+        }
     }
     __syncwarp();
-    if (single) single_acc_flush(ad, sacc);
+    if (SINGLE) single_acc_flush(ad, sacc);
     if (SMEM_AGG) {
         __syncthreads();
         acc_smem_flush(ad, acc);
@@ -887,113 +902,6 @@ __global__ void __launch_bounds__(GATHER_BLOCK, FINAL_MIN_BLOCKS) k_frag_final_d
     }
     const unsigned long long total = warp_sum((unsigned long long)passed);
     if (lane_id() == 0 && total) atomicAdd(fp.rows_passed, total);
-}
-
-// Final pass of a fragment with one-to-many joins (reference: JoinHashMap::_probe_from_ht one-to-many walk,
-// be/src/exec/join/join_hash_map.hpp:718-795 -- every probe row is emitted once per entry of the build chain of its
-// key).  The probe output is never materialised: the thread that owns a surviving fact row walks the chains of its
-// expanding joins like an odometer (last join fastest) and applies the aggregate once per combination, reading the
-// payload columns at the current chain entries.  Hash-table aggregate: a first walk only finds / inserts the group
-// slots; when the table refuses one, nothing of the row has been applied yet and the row goes to the retry list
-// (a row is either applied with all its combinations or not at all).
-__global__ void __launch_bounds__(GATHER_BLOCK) k_frag_gather_agg_expand(const FragDev* __restrict__ fdp, const AggDev* __restrict__ adp, const __grid_constant__ PassDev pd,
-                                                                          const __grid_constant__ VTab vt, const SelEntry* __restrict__ sel_in,
-                                                                          const unsigned long long* __restrict__ n_in_ptr, SelEntry* __restrict__ fail_list,
-                                                                          unsigned long long* __restrict__ fail_count) {
-    __shared__ FragJoinDev s_joins[SR_MAX_FRAG_JOINS];
-    const FragDev& fd = *fdp;
-    const AggDev& ad = *adp;
-    const int S = fd.num_joins;
-    const bool single = ad.num_keys == 0;
-    const bool hash_table = !ad.dense && ad.num_keys > 0;
-    unsigned long long known_groups = hash_table && fail_list ? *(volatile unsigned long long*)ad.ngroups : 0ull;
-    smem_copy(s_joins, fd.joins, S);
-    AccPtrs acc;
-    acc_ptrs_global(ad, acc);
-    __syncthreads();
-    const unsigned long long n_in = *n_in_ptr;
-    unsigned long long passed = 0;
-    SingleAcc sacc;
-    if (single) single_acc_init(ad, sacc);
-    unsigned long long w_begin, w_end;
-    warp_sel_range(n_in, w_begin, w_end);
-    for (unsigned long long i = w_begin + lane_id(); i < w_end; i += 32) {
-        const SelEntry entry = sel_in[i];
-        const uint32_t row = sel_row(entry);
-        if (row == SEL_INVALID) continue;
-        FragLoader ld{vt, (int64_t)row, {0, 0, 0, 0, 0, 0}, pd.carry_join >= 0 ? (int32_t)pd.carry_value_id : -1, sel_carry(entry)};
-        uint32_t head[SR_MAX_FRAG_JOINS];
-        bool ok = true;
-#pragma unroll 1
-        for (int j = 0; j < S && ok; j++) {
-            const FragJoinDev& fj = s_joins[j];
-            head[j] = 0;
-            const bool test = j >= pd.final_first_join;
-            if (!test && !fj.need_head) continue;
-            int64_t key;
-            const bool nul = ld.load(fj.key_value_id, key);
-            if (test && nul) {
-                ok = false;
-                break;
-            }
-            if (fj.need_head || !fj.use_bitmap) {
-                head[j] = join_lookup(fj.j, key);
-                ld.bidx[j] = head[j];
-                if (test && head[j] == 0) ok = false;
-            } else if (test) {
-                if (!join_hit_global(fj, key)) ok = false;
-            }
-        }
-        if (!ok) continue;
-        bool refused = false;
-#pragma unroll 1
-        for (int phase = hash_table ? 0 : 1; phase < 2 && !refused; phase++) {
-            while (true) {
-                if (single) {
-                    single_acc_row(ad, sacc, ld);
-                } else if (hash_table) {
-                    HKey key;
-                    agg_pack_key(ad, ld, key);
-                    bool inserted;
-                    const long long slot = agg_find_slot_key(ad, key, inserted, known_groups);
-                    agg_count_new_groups(ad, inserted, known_groups);
-                    if (slot < 0) {
-                        refused = true;
-                        break;
-                    }
-                    if (phase == 1) agg_apply_row<false>(ad, acc, slot, ld);
-                } else {
-                    const long long slot = agg_find_slot(ad, ld);
-                    if (slot >= 0) agg_apply_row<false>(ad, acc, slot, ld);
-                }
-                if (phase == 1) passed++;
-                // next combination: advance the last expanding join, carry into the one before it when its chain ends
-                int j = S - 1;
-#pragma unroll 1
-                for (; j >= 0; j--) {
-                    if (!s_joins[j].expand) continue;
-                    const uint32_t nx = __ldg(s_joins[j].j.next + ld.bidx[j]);
-                    if (nx) {
-                        ld.bidx[j] = nx;
-                        break;
-                    }
-                    ld.bidx[j] = head[j];
-                }
-                if (j < 0) break;
-            }
-            if (refused) {
-                // phase 0 only (phase 1 finds the slots phase 0 created; tables never shrink in between)
-                if (fail_list) fail_list[atomicAdd(fail_count, 1ull)] = entry;
-            } else if (phase == 0) {
-#pragma unroll 1
-                for (int j = 0; j < S; j++) ld.bidx[j] = head[j]; // the odometer ends on the heads anyway; keeps the second walk independent of that
-            }
-        }
-    }
-    __syncwarp();
-    if (single) single_acc_flush(ad, sacc);
-    passed = warp_sum(passed);
-    if (lane_id() == 0 && passed) atomicAdd(fd.rows_passed, passed);
 }
 
 } // namespace srd
