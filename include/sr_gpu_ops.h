@@ -83,15 +83,17 @@ int32_t sr_type_width(int32_t type);
  *   cudaHostRegister, e.g. a registered ColumnAllocator pool).
  * One rule for all entry points:
  *  1. An unknown kind is refused with SR_ERR_INVALID_ARGUMENT before any copy, allocation or launch.
- *  2. Only sr_fragment_push (the fact columns) and sr_pages_decode (the pages) read SR_MEM_HOST_PINNED buffers IN PLACE
- *     over PCIe: the fragment fetches a column only for the 32-byte sectors holding rows that survived the earlier
- *     joins, so far fewer bytes cross the bus than a full H2D copy.  Where a buffer is read in place, memory that is not
- *     page-locked and mapped is refused with SR_ERR_INVALID_ARGUMENT.  Every other entry point treats SR_MEM_HOST_PINNED
- *     exactly like SR_MEM_HOST, for inputs and for outputs.
+ *  2. Only sr_fragment_push (the fact columns), sr_fragment_push_chunks (the chunks' columns) and sr_pages_decode (the
+ *     pages) read SR_MEM_HOST_PINNED buffers IN PLACE over PCIe: the fragment fetches a column only for the 32-byte
+ *     sectors holding rows that survived the earlier joins, so far fewer bytes cross the bus than a full H2D copy;
+ *     sr_fragment_push_chunks reads every column the fragment needs in full, once, with device loads.  Where a buffer is
+ *     read in place, memory that is not page-locked and mapped is refused with SR_ERR_INVALID_ARGUMENT.  Every other
+ *     entry point treats SR_MEM_HOST_PINNED exactly like SR_MEM_HOST, for inputs and for outputs.
  *  3. A call that writes its result into host memory (either host kind) synchronises before it returns; a result
  *     handed back in host memory (sr_chunk_out.mem) is reported as SR_MEM_HOST.
  *  4. Host inputs: a call waits for the copies of its host inputs before it returns, so that the caller may free or
- *     reuse them, except sr_fragment_push, sr_agg_push and sr_agg_push_selective on a dense or single-state table,
+ *     reuse them, except sr_fragment_push, sr_fragment_push_chunks, sr_agg_push and sr_agg_push_selective on a dense or
+ *     single-state table,
  *     sr_scan_evaluate with a device selection, sr_xchg_hash with device outputs and sr_chunk_serialize into device
  *     memory.  After one of these a page-locked input (pageable memory may be reused at once), and after any call a
  *     buffer read in place, must stay valid and unmodified until the next synchronising call on the context
@@ -644,6 +646,26 @@ void sr_fragment_destroy(sr_fragment* frag);
  * every HashJoinProbeOperator in turn, AggregateBlockingSinkOperator::push_chunk -- with no chunk materialised in between.
  * consume one batch of fact rows (one morsel: any number of rows). */
 int32_t sr_fragment_push(sr_fragment* frag, const sr_chunk_view* fact);
+/* The rows of chunks[0], chunks[1], ... in that order, pushed as one batch: same result, rows_passed and plan as
+ * sr_fragment_push of their concatenation -- the form a scan that hands out chunks of at most chunk_size rows, each in
+ * its own column buffers, pushes without first copying them into one batch on the host.
+ *  - Every chunk carries the same set of (slot_id, type); the column order may differ.  Each chunk's own `mem` is
+ *    honoured: SR_MEM_DEVICE and SR_MEM_HOST_PINNED columns are gathered into one device batch by one kernel launch
+ *    (pinned columns are read over PCIe, in full); SR_MEM_HOST columns are copied H2D straight to their place in that
+ *    batch, which is correct but slow: one small copy per chunk column.  Only the slots the fragment reads are moved.
+ *  - A column is nullable in the batch when any chunk of the call has nulls != NULL for it; the chunks without a null
+ *    column contribute zeros.  When no chunk has one, the batch column has none either, so the NOT NULL kernel paths
+ *    stay eligible exactly as for a contiguous push.
+ *  - Refused with SR_ERR_INVALID_ARGUMENT before any allocation, copy or launch: num_chunks < 0, chunks == NULL with
+ *    num_chunks > 0, an unknown mem kind, chunks of different schemas, negative rows, data == NULL with rows > 0, a device
+ *    or pinned column that is not naturally aligned (see sr_col_view), pinned memory that is not page-locked and mapped.
+ *    A total of 0xFFFFFFF0 rows or more: SR_ERR_NOT_SUPPORTED, before any column is looked at.
+ *  - Pinned pointers are resolved through the library's registry of the ranges made by sr_host_alloc and
+ *    sr_host_register (no driver call); a pointer outside it costs one driver lookup per allocation and call.
+ *  - Zero chunks, or only empty ones, behave like a zero-row sr_fragment_push (the first push still plans).
+ *  - sr_mem rules 2 and 4: the call only queues work; pinned and device chunk buffers must stay valid and unchanged until
+ *    an event recorded after the call has completed, or until the next synchronising call. */
+int32_t sr_fragment_push_chunks(sr_fragment* frag, const sr_chunk_view* chunks, int32_t num_chunks);
 /* the aggregate the fragment feeds (owned by the fragment): finish / pull / merge through
  * the sr_agg_* calls. */
 sr_agg* sr_fragment_agg(sr_fragment* frag);
@@ -881,6 +903,15 @@ int32_t sr_memcpy(sr_ctx* ctx, void* dst, const void* src, int64_t bytes, int32_
  * ------------------------------------------------------------------------------------- */
 int32_t sr_host_alloc(sr_ctx* ctx, int64_t bytes, void** ptr);
 int32_t sr_host_free(sr_ctx* ctx, void* ptr);
+/* Page-lock and map caller memory (cudaHostRegister, mapped | portable): the hook for a pinned ColumnAllocator pool,
+ * whose buffers are then valid as SR_MEM_HOST_PINNED columns.  Refused (SR_ERR_INVALID_ARGUMENT): bytes <= 0, a range
+ * overlapping one already registered or allocated by sr_host_alloc.  sr_host_unregister takes the pointer passed to
+ * sr_host_register and refuses any other; the GPU must no longer read the range (sync or an event first). */
+int32_t sr_host_register(sr_ctx* ctx, void* ptr, int64_t bytes);
+int32_t sr_host_unregister(sr_ctx* ctx, void* ptr);
+/* 1 if [ptr, ptr + bytes) lies inside one range from sr_host_alloc or sr_host_register, 0 if not.  A host lookup in the
+ * library's registry (process-wide, like the portable allocations it records): no driver call, no context lock. */
+int32_t sr_host_is_mapped(sr_ctx* ctx, const void* ptr, int64_t bytes);
 typedef struct sr_event sr_event;
 sr_event* sr_event_create(sr_ctx* ctx);
 void sr_event_destroy(sr_event* ev);

@@ -36,6 +36,7 @@
 
 #include "sr_frag_kernel.cuh"
 #include "sr_frag_pass.cuh"
+#include "sr_gather.cuh"
 
 // ---------------------------------------------------------------------------------------
 // host side
@@ -84,6 +85,7 @@ struct sr_fragment {
     int32_t final_pass = SR_FINAL_PASS_NONE; // the final pass of the last push
     cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
     bool timed_push = false;
+    ChunkGather chunk_gather; // sr_fragment_push_chunks: the batch a list of chunks is gathered into
     ~sr_fragment() {
         for (int e = 0; e < 4; e++)
             if (ev[e]) cudaEventDestroy(ev[e]);
@@ -780,4 +782,130 @@ static int32_t frag_push(sr_fragment* f, const sr_chunk_view* fact) {
     };
     if (!hash) return launch(vt, n, nullptr, nullptr);
     return agg_push_rows(a, vt, n, launch);
+}
+
+// the fact slots the fragment reads: scan conjuncts, probe keys, group keys and aggregate inputs (a slot of the list the
+// fact chunk does not carry is a join payload)
+static void frag_read_slots(const sr_fragment* f, std::vector<int32_t>* slots) {
+    slots->clear();
+    const auto expr_slots = [&](const sr_expr& e) {
+        for (int k = 0; k < std::min<int32_t>(e.num_nodes, SR_MAX_EXPR_NODES); k++)
+            if (e.nodes[k].op == SR_EX_COL) slots->push_back(e.nodes[k].slot_id);
+    };
+    for (const sr_pred& p : f->preds) slots->push_back(p.slot_id);
+    for (const sr_expr& e : f->exprs) expr_slots(e);
+    for (int j = 0; j < f->num_joins; j++) slots->push_back(f->joins[j].probe_key_slot);
+    const sr_agg_desc& d = f->agg->desc;
+    for (int k = 0; k < std::min<int32_t>(d.num_group_keys, SR_MAX_GROUP_KEYS); k++) slots->push_back(d.group_slots[k]);
+    for (int q = 0; q < std::min<int32_t>(d.num_fns, SR_MAX_AGG_FNS); q++) {
+        if (d.fns[q].kind != SR_AGG_COUNT_STAR) expr_slots(d.fns[q].input);
+        if (d.fns[q].kind == SR_AGG_AVG_MERGE) slots->push_back(d.fns[q].reserved);
+    }
+}
+
+// sr_fragment_push_chunks: validate the whole list, gather the columns the fragment reads into one device batch (one
+// k_chunk_gather launch for the device and pinned columns, H2D copies for pageable ones), and push that batch
+static int32_t frag_push_chunks(sr_fragment* f, const sr_chunk_view* chunks, int32_t num_chunks) {
+    sr_ctx* ctx = f->ctx;
+    if (num_chunks < 0 || (chunks == nullptr && num_chunks > 0)) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "chunk list of %d chunks at %p", num_chunks, (const void*)chunks);
+    if (f->agg->finished) return sr_fail(ctx, SR_ERR_STATE, "fragment push after sink_finish");
+    // headers first: the row total is refused before any column is looked at
+    int64_t total = 0;
+    for (int32_t c = 0; c < num_chunks; c++) {
+        SR_TRY(mem_check(ctx, chunks[c].mem, "chunk"));
+        if (chunks[c].num_rows < 0) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "chunk %d has %lld rows", c, (long long)chunks[c].num_rows);
+        if (chunks[c].num_cols < 0 || (chunks[c].num_cols > 0 && chunks[c].cols == nullptr))
+            return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "chunk %d: %d columns at %p", c, chunks[c].num_cols, (const void*)chunks[c].cols);
+        total += chunks[c].num_rows;
+        if (total >= 0xFFFFFFF0ll) return sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "fragment batch of more than 2^32 rows; push smaller chunk lists");
+    }
+    if (num_chunks == 0) {
+        if (f->compiled) return SR_OK; // a zero-row push of a planned fragment does nothing
+        const sr_chunk_view none{nullptr, 0, SR_MEM_DEVICE, 0};
+        return frag_push(f, &none);
+    }
+    // schema: chunk 0's columns; every chunk carries the same (slot, type) set, in any order.  col_of[c * ncols + k]:
+    // chunk c's column of schema column k
+    const sr_chunk_view& c0 = chunks[0];
+    const int ncols = c0.num_cols;
+    std::vector<const sr_col_view*> col_of((size_t)num_chunks * ncols);
+    for (int32_t c = 0; c < num_chunks; c++) {
+        const sr_chunk_view& ch = chunks[c];
+        if (ch.num_cols != ncols) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "chunk %d has %d columns, chunk 0 has %d", c, ch.num_cols, ncols);
+        for (int k = 0; k < ncols; k++) {
+            const sr_col_view& s = c0.cols[k];
+            const sr_col_view* m = (ch.cols[k].slot_id == s.slot_id) ? &ch.cols[k] : find_col(&ch, s.slot_id);
+            if (!m || m->type != s.type) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "chunk %d: slot %d missing or of another type than in chunk 0", c, s.slot_id);
+            const int w = srd::type_width(m->type);
+            if (w == 0) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "unknown column type %d (slot %d)", m->type, m->slot_id);
+            if (ch.num_rows > 0 && m->data == nullptr) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "chunk %d: null data pointer (slot %d)", c, m->slot_id);
+            const bool in_place = ch.mem == SR_MEM_DEVICE || (ch.mem == SR_MEM_HOST_PINNED && ch.num_rows > 0);
+            if (in_place && !col_aligned(m->data, w))
+                return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "chunk %d: slot %d column at %p is not %d-byte aligned", c, m->slot_id, m->data, std::min(w, 8));
+            col_of[(size_t)c * ncols + k] = m;
+        }
+    }
+    std::vector<int32_t> read;
+    frag_read_slots(f, &read);
+    std::vector<int> moved; // schema columns gathered into the batch
+    std::vector<bool> nullable;
+    for (int k = 0; k < ncols; k++) {
+        if (std::find(read.begin(), read.end(), c0.cols[k].slot_id) == read.end()) continue;
+        bool nl = false;
+        for (int32_t c = 0; c < num_chunks && !nl; c++) nl = col_of[(size_t)c * ncols + k]->nulls != nullptr;
+        moved.push_back(k);
+        nullable.push_back(nl);
+    }
+    // device aliases of the pinned buffers: resolved (and refused) before anything is allocated, copied or launched
+    PinnedResolver pinned;
+    std::vector<const void*> src((size_t)num_chunks * moved.size() * 2, nullptr); // [c][m][data, nulls]
+    for (int32_t c = 0; c < num_chunks; c++) {
+        const sr_chunk_view& ch = chunks[c];
+        if (ch.num_rows == 0) continue;
+        for (size_t m = 0; m < moved.size(); m++) {
+            const sr_col_view* col = col_of[(size_t)c * ncols + moved[m]];
+            const void** s = &src[((size_t)c * moved.size() + m) * 2];
+            s[0] = col->data;
+            s[1] = col->nulls;
+            if (ch.mem != SR_MEM_HOST_PINNED) continue;
+            SR_TRY(pinned.resolve(ctx, col->data, (size_t)ch.num_rows * srd::type_width(col->type), col->slot_id, &s[0]));
+            if (col->nulls) SR_TRY(pinned.resolve(ctx, col->nulls, (size_t)ch.num_rows, col->slot_id, &s[1]));
+        }
+    }
+    // the batch: one grow-only (data, nulls) pair per moved column, filled chunk after chunk
+    ChunkGather& g = f->chunk_gather;
+    g.cols.resize((int)moved.size());
+    std::vector<sr_col_view> view(moved.size());
+    for (size_t m = 0; m < moved.size(); m++) {
+        const sr_col_view& s = c0.cols[moved[m]];
+        void* data;
+        uint8_t* nulls;
+        SR_TRY(g.cols.reserve(ctx, (int)m, total, srd::type_width(s.type), nullable[m], &data, &nulls));
+        view[m] = sr_col_view{data, nulls, s.type, s.slot_id};
+    }
+    std::vector<srd::GatherPiece> pieces;
+    int64_t row = 0;
+    for (int32_t c = 0; c < num_chunks; c++) {
+        const sr_chunk_view& ch = chunks[c];
+        const size_t r = (size_t)ch.num_rows;
+        if (r == 0) continue;
+        for (size_t m = 0; m < moved.size(); m++) {
+            const int w = srd::type_width(view[m].type);
+            const void* const* s = &src[((size_t)c * moved.size() + m) * 2];
+            uint8_t* dst = (uint8_t*)view[m].data + (size_t)row * w;
+            uint8_t* dst_nulls = nullable[m] ? (uint8_t*)view[m].nulls + row : nullptr;
+            if (ch.mem == SR_MEM_HOST) { // pageable: straight to its place in the batch
+                SR_CUDA(ctx, cudaMemcpyAsync(dst, s[0], r * w, cudaMemcpyHostToDevice, ctx->stream));
+                if (dst_nulls && s[1]) SR_CUDA(ctx, cudaMemcpyAsync(dst_nulls, s[1], r, cudaMemcpyHostToDevice, ctx->stream));
+            } else {
+                gather_pieces(&pieces, s[0], dst, r * w);
+                if (dst_nulls && s[1]) gather_pieces(&pieces, s[1], dst_nulls, r);
+            }
+            if (dst_nulls && !s[1]) gather_pieces(&pieces, nullptr, dst_nulls, r);
+        }
+        row += (int64_t)r;
+    }
+    SR_TRY(g.launch(ctx, pieces));
+    const sr_chunk_view batch{view.data(), (int32_t)view.size(), SR_MEM_DEVICE, total};
+    return frag_push(f, &batch);
 }

@@ -264,13 +264,67 @@ int32_t sr_host_alloc(sr_ctx* ctx, int64_t bytes, void** ptr) {
         cudaGetLastError();
         return sr_fail(ctx, SR_ERR_OUT_OF_MEMORY, "cudaHostAlloc(%lld) failed: %s", (long long)bytes, cudaGetErrorString(e));
     }
+    void* dev = nullptr;
+    SR_CUDA(ctx, cudaHostGetDevicePointer(&dev, *ptr, 0));
+    HostRegistry& reg = host_registry();
+    std::lock_guard<std::mutex> lk(reg.mu);
+    reg.ranges[(uintptr_t)*ptr] = HostRange{(size_t)bytes, (uintptr_t)dev, false};
     return SR_OK;
 }
 
 int32_t sr_host_free(sr_ctx* ctx, void* ptr) {
     SR_BIND(ctx);
-    if (ptr) SR_CUDA(ctx, cudaFreeHost(ptr));
+    if (!ptr) return SR_OK;
+    {
+        HostRegistry& reg = host_registry();
+        std::lock_guard<std::mutex> lk(reg.mu);
+        auto it = reg.ranges.find((uintptr_t)ptr);
+        if (it != reg.ranges.end() && !it->second.registered) reg.ranges.erase(it);
+    }
+    SR_CUDA(ctx, cudaFreeHost(ptr));
     return SR_OK;
+}
+
+int32_t sr_host_register(sr_ctx* ctx, void* ptr, int64_t bytes) {
+    SR_BIND(ctx);
+    if (!ptr || bytes <= 0) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "sr_host_register(%p, %lld)", ptr, (long long)bytes);
+    HostRegistry& reg = host_registry();
+    std::lock_guard<std::mutex> lk(reg.mu);
+    if (reg.overlaps((uintptr_t)ptr, (size_t)bytes))
+        return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "sr_host_register: [%p, +%lld) overlaps a page-locked range already known", ptr, (long long)bytes);
+    cudaError_t e = cudaHostRegister(ptr, (size_t)bytes, cudaHostRegisterMapped | cudaHostRegisterPortable);
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        return sr_fail(ctx, e == cudaErrorHostMemoryAlreadyRegistered || e == cudaErrorInvalidValue ? SR_ERR_INVALID_ARGUMENT : SR_ERR_CUDA,
+                       "cudaHostRegister(%p, %lld) failed: %s", ptr, (long long)bytes, cudaGetErrorString(e));
+    }
+    void* dev = nullptr;
+    if ((e = cudaHostGetDevicePointer(&dev, ptr, 0)) != cudaSuccess) {
+        cudaGetLastError();
+        cudaHostUnregister(ptr);
+        return sr_fail(ctx, SR_ERR_CUDA, "cudaHostGetDevicePointer(%p) failed: %s", ptr, cudaGetErrorString(e));
+    }
+    reg.ranges[(uintptr_t)ptr] = HostRange{(size_t)bytes, (uintptr_t)dev, true};
+    return SR_OK;
+}
+
+int32_t sr_host_unregister(sr_ctx* ctx, void* ptr) {
+    SR_BIND(ctx);
+    HostRegistry& reg = host_registry();
+    std::lock_guard<std::mutex> lk(reg.mu);
+    auto it = reg.ranges.find((uintptr_t)ptr);
+    if (it == reg.ranges.end() || !it->second.registered) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "sr_host_unregister(%p): not a range from sr_host_register", ptr);
+    reg.ranges.erase(it);
+    SR_CUDA(ctx, cudaHostUnregister(ptr));
+    return SR_OK;
+}
+
+// no context lock and no driver call: the registry has its own
+int32_t sr_host_is_mapped(sr_ctx* ctx, const void* ptr, int64_t bytes) {
+    if (!ctx || bytes < 0) return SR_ERR_INVALID_ARGUMENT;
+    HostRegistry& reg = host_registry();
+    std::lock_guard<std::mutex> lk(reg.mu);
+    return ptr && reg.find((uintptr_t)ptr, (size_t)bytes) ? 1 : 0;
 }
 
 struct sr_event {
@@ -1187,6 +1241,12 @@ int32_t sr_fragment_push(sr_fragment* frag, const sr_chunk_view* fact) {
     if (!frag || !fact) return SR_ERR_INVALID_ARGUMENT;
     SR_BIND(frag->ctx);
     return frag_push(frag, fact);
+}
+
+int32_t sr_fragment_push_chunks(sr_fragment* frag, const sr_chunk_view* chunks, int32_t num_chunks) {
+    if (!frag) return SR_ERR_INVALID_ARGUMENT;
+    SR_BIND(frag->ctx);
+    return frag_push_chunks(frag, chunks, num_chunks);
 }
 
 sr_agg* sr_fragment_agg(sr_fragment* frag) {

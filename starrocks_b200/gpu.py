@@ -141,6 +141,7 @@ def lib():
         "sr_fragment_create": (vp, [vp, vp]),
         "sr_fragment_destroy": (None, [vp]),
         "sr_fragment_push": (i32, [vp, vp]),
+        "sr_fragment_push_chunks": (i32, [vp, vp, i32]),
         "sr_fragment_agg": (vp, [vp]),
         "sr_fragment_rows_passed": (i64, [vp]),
         "sr_xchg_create": (vp, [vp, vp]),
@@ -159,6 +160,9 @@ def lib():
         "sr_chunk_deserialize": (i32, [vp, vp, i64, i32, vp, vp]),
         "sr_host_alloc": (i32, [vp, i64, vp]),
         "sr_host_free": (i32, [vp, vp]),
+        "sr_host_register": (i32, [vp, vp, i64]),
+        "sr_host_unregister": (i32, [vp, vp]),
+        "sr_host_is_mapped": (i32, [vp, vp, i64]),
         "sr_event_create": (vp, [vp]),
         "sr_event_destroy": (None, [vp]),
         "sr_event_record": (i32, [vp]),
@@ -188,12 +192,12 @@ EXPORTED_SYMBOLS = [
     "sr_join_probe_indexes", "sr_join_key_hash", "sr_agg_create", "sr_agg_destroy", "sr_agg_push",
     "sr_agg_sink_finish", "sr_agg_num_groups", "sr_agg_pull", "sr_agg_merge", "sr_agg_two_phase_descs", "sr_agg_convert_to_states", "sr_agg_push_selective", "sr_agg_current_groups", "sr_agg_dense_state", "sr_agg_reset", "sr_fragment_reset", "sr_fragment_get_plan", "sr_fragment_last_pass_ms",
     "sr_fragment_create",
-    "sr_fragment_destroy", "sr_fragment_push", "sr_fragment_agg", "sr_fragment_rows_passed", "sr_xchg_create",
+    "sr_fragment_destroy", "sr_fragment_push", "sr_fragment_push_chunks", "sr_fragment_agg", "sr_fragment_rows_passed", "sr_xchg_create",
     "sr_join_build_runtime_filter", "sr_rf_create", "sr_rf_insert", "sr_rf_destroy", "sr_rf_get_info", "sr_rf_copy_directory",
     "sr_rf_merge_directory", "sr_rf_evaluate", "sr_scan_add_runtime_filter", "sr_scan_get_rf_stats", "sr_scan_set_rf_adaptive", "sr_rf_copy_in_values", "sr_rf_merge_in_values",
     "sr_xchg_destroy", "sr_xchg_partition", "sr_xchg_hash", "sr_gather", "sr_memcpy", "sr_abi_sizeof", "sr_bandwidth_probe", "sr_flush_l2",
     "sr_chunk_serialized_size", "sr_chunk_serialize", "sr_serde_create", "sr_serde_destroy", "sr_chunk_deserialize",
-    "sr_host_alloc", "sr_host_free", "sr_event_create", "sr_event_destroy", "sr_event_record", "sr_event_query", "sr_event_sync",
+    "sr_host_alloc", "sr_host_free", "sr_host_register", "sr_host_unregister", "sr_host_is_mapped", "sr_event_create", "sr_event_destroy", "sr_event_record", "sr_event_query", "sr_event_sync",
     "sr_page_decoder_create", "sr_page_decoder_destroy", "sr_pages_decode", "sr_page_decoder_set_dict", "sr_null_maps_decode",
 ]
 
@@ -242,6 +246,20 @@ class Context:
 
     def flush_l2(self):
         self.check(lib().sr_flush_l2(self.h))
+
+    def host_register(self, ptr, nbytes=None):
+        """page-lock and map `nbytes` of host memory at `ptr` (an int, or a numpy array: its whole buffer); its slices are
+        then valid as MEM_HOST_PINNED columns"""
+        if isinstance(ptr, np.ndarray):
+            ptr, nbytes = ptr.ctypes.data, ptr.nbytes
+        self.check(lib().sr_host_register(self.h, ptr, nbytes))
+
+    def host_unregister(self, ptr):
+        self.check(lib().sr_host_unregister(self.h, ptr.ctypes.data if isinstance(ptr, np.ndarray) else ptr))
+
+    def host_is_mapped(self, ptr, nbytes):
+        """True when [ptr, ptr + nbytes) lies inside one range from sr_host_alloc or sr_host_register"""
+        return bool(self.check(lib().sr_host_is_mapped(self.h, ptr, nbytes)))
 
     def bandwidth_probe(self, dev_ptr, nbytes):
         out = C.c_uint64(0)
@@ -553,6 +571,11 @@ class Fragment:
 
     def push(self, chunk):
         self.ctx.check(lib().sr_fragment_push(self.h, chunk.ref()))
+
+    def push_chunks(self, chunks):
+        """the rows of `chunks` (abi.Chunk, each in its own memory kind) in order, pushed as one batch"""
+        views = (abi.sr_chunk_view * max(1, len(chunks)))(*[c.view for c in chunks])
+        self.ctx.check(lib().sr_fragment_push_chunks(self.h, views, len(chunks)))
 
     def reset(self):
         self.ctx.check(lib().sr_fragment_reset(self.h))

@@ -11,7 +11,7 @@
 // result rows are on the host: it contains the chunk copies, every byte crossing PCIe and the result D2H.
 // Prints one JSON line; exit code 0 only if the groups equal a row-at-a-time evaluation done while generating the data.
 //
-//   operator_e2e_bench [rows=600000000] [dop=0 (hardware threads, capped at 32)] [batch_rows=4194304]
+//   operator_e2e_bench [rows=600000000] [dop=0 (hardware threads, capped at 32)] [batch_rows=4194304] [--pool pageable|pinned]
 #include <chrono>
 #include <cstdio>
 #include <cstdlib>
@@ -48,16 +48,26 @@ std::vector<ChunkPtr> split(const ChunkPtr& whole, size_t chunk_size) {
 }
 
 // the scan side of a probe pipeline: one shard of lineorder in plain host arrays (the storage layer's decoded pages);
-// pull_chunk materialises the next <= chunk_size rows as a Chunk of six Int32Columns (one copy: what page decoding writes)
+// pull_chunk materialises the next <= chunk_size rows as a Chunk of six Int32Columns (one copy: what page decoding writes):
+// into pageable vectors by default, or into BorrowedColumns sliced from a registered PinnedArena (--pool pinned: the
+// columns of a scan over a pinned ColumnAllocator pool, which the fused sink forwards without a host copy)
 class MemoryChunkSource final : public SourceOperator {
 public:
-    MemoryChunkSource(int32_t seq, const std::vector<int32_t>* cols, size_t rows) : SourceOperator(nullptr, 3, "memory_chunk_source", 3, false, seq), _cols(cols), _rows(rows) {}
+    MemoryChunkSource(int32_t seq, const std::vector<int32_t>* cols, size_t rows, std::shared_ptr<PinnedArena> arena)
+            : SourceOperator(nullptr, 3, "memory_chunk_source", 3, false, seq), _cols(cols), _rows(rows), _arena(std::move(arena)) {}
     bool has_output() const override { return _next < _rows; }
     bool is_finished() const override { return _next >= _rows; }
     StatusOr<ChunkPtr> pull_chunk(RuntimeState* state) override {
         const size_t n = std::min<size_t>((size_t)state->chunk_size(), _rows - _next);
         auto c = std::make_shared<Chunk>();
         for (int k = 0; k < 6; k++) {
+            if (_arena) {
+                auto col = _arena->column(SR_TYPE_INT, n);
+                if (!col) return Status::InternalError("pinned arena full");
+                memcpy(col->mutable_raw_data(), _cols[k].data() + _next, n * sizeof(int32_t));
+                c->append_column(col, (SlotId)k);
+                continue;
+            }
             auto col = std::make_shared<Int32Column>(SR_TYPE_INT);
             col->get_data().assign(_cols[k].begin() + (long)_next, _cols[k].begin() + (long)(_next + n));
             c->append_column(col, (SlotId)k);
@@ -69,6 +79,7 @@ public:
 private:
     const std::vector<int32_t>* _cols;
     size_t _rows, _next = 0;
+    std::shared_ptr<PinnedArena> _arena;
 };
 
 class ResultSink final : public Operator {
@@ -129,9 +140,18 @@ using Groups = std::map<std::pair<int32_t, int32_t>, std::pair<int64_t, int64_t>
 } // namespace
 
 int main(int argc, char** argv) {
-    const size_t n_fact = argc > 1 ? (size_t)atoll(argv[1]) : 600000000ull;
-    int dop = argc > 2 ? atoi(argv[2]) : 0;
-    const size_t batch_rows = argc > 3 ? (size_t)atoll(argv[3]) : (size_t)1 << 22;
+    std::vector<const char*> pos;
+    bool pinned_pool = false;
+    for (int a = 1; a < argc; a++) {
+        if (std::string(argv[a]) == "--pool" && a + 1 < argc) {
+            pinned_pool = std::string(argv[++a]) == "pinned";
+            continue;
+        }
+        pos.push_back(argv[a]);
+    }
+    const size_t n_fact = pos.size() > 0 ? (size_t)atoll(pos[0]) : 600000000ull;
+    int dop = pos.size() > 1 ? atoi(pos[1]) : 0;
+    const size_t batch_rows = pos.size() > 2 ? (size_t)atoll(pos[2]) : (size_t)1 << 22;
     if (dop <= 0) dop = (int)std::min(32u, std::max(1u, std::thread::hardware_concurrency()));
     const int n_cust = 3000000, n_supp = 200000, n_part = 1400000, n_dates = 2556; // SSB SF100 dimensions
     sr_ctx* ctx = sr_ctx_create(0, nullptr);
@@ -280,7 +300,17 @@ int main(int argc, char** argv) {
     std::vector<std::shared_ptr<GpuFragmentSinkOperator>> sinks;
     std::vector<std::unique_ptr<PipelineDriver>> drivers;
     for (int t = 0; t < dop; t++) {
-        auto src = std::make_shared<MemoryChunkSource>(t, &shard_cols[(size_t)t * 6], shard_rows[(size_t)t]);
+        std::shared_ptr<PinnedArena> arena;
+        if (pinned_pool) { // one registered arena per shard, sized for its chunks (outside the timed region)
+            std::string err;
+            const size_t chunks = shard_rows[(size_t)t] / 4096 + 1;
+            arena = PinnedArena::create(ctx, shard_rows[(size_t)t] * 6 * sizeof(int32_t) + chunks * 6 * PinnedArena::ALIGN, &err);
+            if (!arena) {
+                fprintf(stderr, "%s\n", err.c_str());
+                return 2;
+            }
+        }
+        auto src = std::make_shared<MemoryChunkSource>(t, &shard_cols[(size_t)t * 6], shard_rows[(size_t)t], arena);
         auto sink = std::make_shared<GpuFragmentSinkOperator>(nullptr, 8, 8, t, fragment, batch_rows);
         sinks.push_back(sink);
         drivers.push_back(std::make_unique<PipelineDriver>(Operators{src, sink}));
@@ -319,20 +349,25 @@ int main(int argc, char** argv) {
         d2h += (int64_t)c->num_rows() * 24;
     }
     const bool ok = got == expect;
-    int64_t batches = 0, bytes = 0, append_ns = 0, push_ns = 0, stalls = 0;
+    int64_t batches = 0, bytes = 0, append_ns = 0, push_ns = 0, stalls = 0, fwd_chunks = 0, fwd_rows = 0;
     for (auto& s : sinks) {
+        fwd_chunks += s->unique_metrics()->get_counter("ForwardedChunks")->value();
+        fwd_rows += s->unique_metrics()->get_counter("ForwardedRows")->value();
         batches += s->unique_metrics()->get_counter("FragmentBatches")->value();
         bytes += s->unique_metrics()->get_counter("PinnedBatchBytes")->value();
         append_ns += s->unique_metrics()->get_counter("AppendChunkTime")->value();
         push_ns += s->unique_metrics()->get_counter("FragmentPushTime")->value();
         stalls += s->unique_metrics()->get_counter("NeedInputFalseBothBatchesInFlight")->value();
     }
-    printf("{\"path\": \"C++ operators: %d x (MemoryChunkSource -> GpuFragmentSinkOperator) sharing one GpuFragment, 4096-row chunks, pinned double-buffered "
-           "batches of %zu rows read in place by the fragment kernels\", \"rows\": %zu, \"dop\": %d, \"seconds\": %.6f, \"probe_seconds\": %.6f, "
+    const std::string path = pinned_pool ? "4096-row chunks in registered pinned arenas forwarded in lists of " + std::to_string(batch_rows) +
+                                                   " rows to sr_fragment_push_chunks (gathered on the device)"
+                                         : "4096-row chunks, pinned double-buffered batches of " + std::to_string(batch_rows) + " rows read in place by the fragment kernels";
+    printf("{\"path\": \"C++ operators: %d x (MemoryChunkSource -> GpuFragmentSinkOperator) sharing one GpuFragment, %s\", \"pool\": \"%s\", "
+           "\"forwarded_chunks\": %lld, \"forwarded_rows\": %lld, \"rows\": %zu, \"dop\": %d, \"seconds\": %.6f, \"probe_seconds\": %.6f, "
            "\"rows_per_s\": %.1f, \"build_seconds\": %.4f, \"groups\": %zu, \"matches_row_at_a_time_evaluation\": %s, \"h2d_bytes_offered\": %lld, "
            "\"d2h_bytes\": %lld, \"fragment_batches\": %lld, \"append_chunk_cpu_seconds_all_threads\": %.4f, \"fragment_push_call_seconds_all_threads\": %.4f, "
            "\"need_input_false_polls\": %lld, \"gpu_launches\": %lld}\n",
-           dop, batch_rows, n_fact, dop, total_s, probe_s, (double)n_fact / total_s, build_s, got.size(), ok ? "true" : "false", (long long)bytes, (long long)d2h,
+           dop, path.c_str(), pinned_pool ? "pinned" : "pageable", (long long)fwd_chunks, (long long)fwd_rows, n_fact, dop, total_s, probe_s, (double)n_fact / total_s, build_s, got.size(), ok ? "true" : "false", (long long)bytes, (long long)d2h,
            (long long)batches, append_ns / 1e9, push_ns / 1e9, (long long)stalls, (long long)(sr_ctx_kernel_launches(ctx) - launches0));
     fprintf(stderr, "%s\n%s\n", sinks[0]->unique_metrics()->to_string().c_str(), sinks[0]->common_metrics()->to_string().c_str());
     for (auto& d : drivers) d->close(&state);

@@ -9,7 +9,10 @@
 // BE's own classes; the adapters only need raw_data()/null data()/size()/slot ids.
 #pragma once
 
+#include <algorithm>
+#include <atomic>
 #include <cstdint>
+#include <cstdlib>
 #include <cstring>
 #include <memory>
 #include <stdexcept>
@@ -72,9 +75,83 @@ using DoubleColumn = FixedLengthColumn<double>;
 using UInt8Column = FixedLengthColumn<uint8_t>;
 using NullColumn = UInt8Column;
 
+// A fixed-length column over memory it does not own: the reference's ContainerResource-backed columns
+// (be/src/column/container_resource.h:24), which is how the buffers of a pinned ColumnAllocator pool appear in a chunk.
+// `owner` keeps the memory alive (a slice of a PinnedArena, say); the column cannot grow past the borrowed rows.
+class BorrowedColumn final : public Column {
+public:
+    BorrowedColumn(int32_t logical_type, void* data, size_t rows, std::shared_ptr<const void> owner)
+            : _type(logical_type), _data((uint8_t*)data), _rows(rows), _cap(rows), _owner(std::move(owner)) {}
+    size_t size() const override { return _rows; }
+    int32_t logical_type() const override { return _type; }
+    const uint8_t* raw_data() const override { return _data; }
+    uint8_t* mutable_raw_data() override { return _data; }
+    void resize(size_t n) override {
+        if (n > _cap) throw std::runtime_error("BorrowedColumn: cannot grow past the " + std::to_string(_cap) + " borrowed rows");
+        _rows = n;
+    }
+    size_t type_size() const override { return (size_t)sr_type_width(_type); }
+
+private:
+    int32_t _type;
+    uint8_t* _data;
+    size_t _rows, _cap;
+    std::shared_ptr<const void> _owner;
+};
+
+// One page-locked, device-mapped arena (sr_host_register) handing out aligned slices: the pinned ColumnAllocator pool
+// of INTEGRATION.md section 3 in miniature.  A slice is never returned to the arena; the arena is unregistered and freed
+// when the last column borrowing from it is gone (every slice holds the arena).
+class PinnedArena : public std::enable_shared_from_this<PinnedArena> {
+public:
+    static constexpr size_t ALIGN = 64;
+    // StatusOr-free factory: nullptr and the library's message in *err when the registration fails
+    static std::shared_ptr<PinnedArena> create(sr_ctx* ctx, size_t bytes, std::string* err) {
+        auto a = std::shared_ptr<PinnedArena>(new PinnedArena(ctx, bytes));
+        if (!a->_base) {
+            *err = "PinnedArena: out of host memory";
+            return nullptr;
+        }
+        if (sr_host_register(ctx, a->_base, (int64_t)a->_cap) != SR_OK) {
+            *err = std::string("PinnedArena: ") + sr_last_error(ctx);
+            return nullptr;
+        }
+        a->_registered = true;
+        return a;
+    }
+    ~PinnedArena() {
+        if (_registered) sr_host_unregister(_ctx, _base);
+        free(_base);
+    }
+    // `bytes` at an ALIGN-byte boundary, or nullptr when the arena is full (thread-safe)
+    void* slice(size_t bytes) {
+        const size_t want = (bytes + ALIGN - 1) & ~(ALIGN - 1);
+        size_t off = _used.fetch_add(want);
+        if (off + want > _cap) return nullptr;
+        return _base + off;
+    }
+    // a column of `rows` values of `logical_type` in a fresh slice (nullptr when full)
+    std::shared_ptr<BorrowedColumn> column(int32_t logical_type, size_t rows) {
+        void* p = slice(std::max<size_t>(rows, 1) * (size_t)sr_type_width(logical_type));
+        return p ? std::make_shared<BorrowedColumn>(logical_type, p, rows, shared_from_this()) : nullptr;
+    }
+    size_t capacity() const { return _cap; }
+
+private:
+    PinnedArena(sr_ctx* ctx, size_t bytes) : _ctx(ctx), _cap((std::max<size_t>(bytes, 1) + 4095) & ~(size_t)4095) {
+        _base = (uint8_t*)aligned_alloc(4096, _cap);
+    }
+    sr_ctx* _ctx;
+    size_t _cap;
+    uint8_t* _base = nullptr;
+    bool _registered = false;
+    std::atomic<size_t> _used{0};
+};
+
+// the data column and the uint8 null column (1 = NULL): owned (NullColumn) or borrowed (BorrowedColumn) buffers
 class NullableColumn final : public Column {
 public:
-    NullableColumn(ColumnPtr data, std::shared_ptr<NullColumn> nulls) : _data(std::move(data)), _nulls(std::move(nulls)) {}
+    NullableColumn(ColumnPtr data, ColumnPtr nulls) : _data(std::move(data)), _nulls(std::move(nulls)) {}
     size_t size() const override { return _data->size(); }
     bool is_nullable() const override { return true; }
     bool is_binary() const override { return _data->is_binary(); }
@@ -88,11 +165,11 @@ public:
     }
     size_t type_size() const override { return _data->type_size(); }
     const ColumnPtr& data_column() const { return _data; }
-    const std::shared_ptr<NullColumn>& null_column() const { return _nulls; }
+    const ColumnPtr& null_column() const { return _nulls; }
 
 private:
     ColumnPtr _data;
-    std::shared_ptr<NullColumn> _nulls;
+    ColumnPtr _nulls;
 };
 
 inline ColumnPtr make_column(int32_t logical_type, size_t rows) {

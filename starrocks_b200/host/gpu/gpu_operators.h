@@ -190,6 +190,77 @@ private:
     bool _in_flight = false;
 };
 
+// Chunks handed to the library as they are: every data and null buffer lies in a page-locked range the library knows
+// (sr_host_is_mapped: a registered ColumnAllocator pool), so no byte is copied on the host.  The list keeps the ChunkPtrs
+// of its chunks until the event recorded behind their sr_fragment_push_chunks has completed.
+class ForwardedChunkList {
+public:
+    ForwardedChunkList() = default;
+    ForwardedChunkList(const ForwardedChunkList&) = delete;
+    ForwardedChunkList& operator=(const ForwardedChunkList&) = delete;
+    ~ForwardedChunkList() {
+        if (_event) sr_event_destroy(_event);
+    }
+    // true when the chunk can be forwarded: fixed-length columns whose buffers all lie in page-locked mapped ranges
+    static bool forwardable(sr_ctx* ctx, const Chunk& c) {
+        const size_t n = c.num_rows();
+        for (size_t i = 0; i < c.num_columns(); i++) {
+            const Column& col = *c.get_column_by_index(i);
+            if (col.is_binary() || sr_host_is_mapped(ctx, col.raw_data(), (int64_t)(n * col.type_size())) != 1) return false;
+            if (col.is_nullable() && sr_host_is_mapped(ctx, col.null_data(), (int64_t)n) != 1) return false;
+        }
+        return true;
+    }
+    Status add(sr_ctx* ctx, const ChunkPtr& c) {
+        if (!_event) {
+            _ctx = ctx;
+            _event = sr_event_create(ctx);
+            if (!_event) return sr_to_status(ctx, sr_last_error_code(ctx));
+        }
+        _chunks.push_back(c);
+        _rows += c->num_rows();
+        return Status::OK();
+    }
+    size_t rows() const { return _in_flight ? 0 : _rows; }
+    size_t num_chunks() const { return _chunks.size(); }
+    // one sr_fragment_push_chunks of the whole list, an event behind it
+    Status submit(sr_fragment* frag) {
+        _cols.resize(_chunks.size());
+        _views.clear();
+        for (size_t k = 0; k < _chunks.size(); k++) {
+            sr_chunk_view v = make_chunk_view(*_chunks[k], &_cols[k]);
+            v.mem = SR_MEM_HOST_PINNED;
+            _views.push_back(v);
+        }
+        RETURN_IF_SR_ERROR(_ctx, sr_fragment_push_chunks(frag, _views.data(), (int32_t)_views.size()));
+        RETURN_IF_SR_ERROR(_ctx, sr_event_record(_event));
+        _in_flight = true;
+        return Status::OK();
+    }
+    bool busy() { // non-blocking; releases the chunks once the library is done with them
+        if (_in_flight && sr_event_query(_event) != 0) release();
+        return _in_flight;
+    }
+    void wait() {
+        if (_in_flight) sr_event_sync(_event);
+        release();
+    }
+
+private:
+    void release() {
+        _in_flight = false;
+        _chunks.clear();
+        _rows = 0;
+    }
+    sr_ctx* _ctx = nullptr;
+    sr_event* _event = nullptr;
+    std::vector<ChunkPtr> _chunks;
+    std::vector<std::vector<sr_col_view>> _cols;
+    std::vector<sr_chunk_view> _views;
+    size_t _rows = 0;
+    bool _in_flight = false;
+};
+
 // counters every GPU operator keeps in its _unique_metrics, sampled from the context at the operator's life-cycle points
 struct GpuOpCounters {
     RuntimeProfile::Counter* launches = nullptr;
@@ -1036,11 +1107,14 @@ private:
 };
 using GpuFragmentPtr = std::shared_ptr<GpuFragment>;
 
-// The fused sink.  push_chunk never waits for the GPU: chunks are copied into one of two page-locked batches (the copy a
-// ColumnAllocator-backed scan would not even need); a full batch is handed to sr_fragment_push, which only queues work
-// (the fragment kernels read the batch IN PLACE over PCIe), an event is recorded behind it and the operator switches to
-// the other batch.  need_input() turns false only while BOTH batches are in flight -- polled by the driver, no blocking
-// call (operator.h:100-118) -- and pending_finish() keeps the driver from finishing until the queued work has drained.
+// The fused sink.  push_chunk never waits for the GPU.  A chunk whose buffers all lie in a registered page-locked pool
+// (ForwardedChunkList::forwardable) is forwarded: its ChunkPtr joins the current slot's list and a full list goes to
+// sr_fragment_push_chunks, which gathers it on the device.  Any other chunk is copied into one of two page-locked batches
+// (PinnedChunkBatch) and a full batch goes to sr_fragment_push, which reads it IN PLACE over PCIe.  A slot holds one kind
+// at a time: a chunk of the other kind hands the current slot over first.  After each push an event is recorded and the
+// operator switches to the other slot.  need_input() turns false only while BOTH slots are in flight -- polled by the
+// driver, no blocking call (operator.h:100-118) -- and pending_finish() keeps the driver from finishing until the queued
+// work has drained.
 class GpuFragmentSinkOperator final : public OperatorWithDependency {
 public:
     GpuFragmentSinkOperator(OperatorFactory* f, int32_t id, int32_t plan_node_id, int32_t seq, GpuFragmentPtr frag, size_t batch_rows = 1 << 22)
@@ -1049,6 +1123,8 @@ public:
         _push_timer = ADD_TIMER(_unique_metrics.get(), "FragmentPushTime"); // host time of the (asynchronous) library call
         _batches_counter = ADD_COUNTER(_unique_metrics.get(), "FragmentBatches", TUnit::UNIT);
         _bytes_counter = ADD_COUNTER(_unique_metrics.get(), "PinnedBatchBytes", TUnit::BYTES);
+        _forwarded_chunks_counter = ADD_COUNTER(_unique_metrics.get(), "ForwardedChunks", TUnit::UNIT);
+        _forwarded_rows_counter = ADD_COUNTER(_unique_metrics.get(), "ForwardedRows", TUnit::UNIT);
         _no_buffer_counter = ADD_COUNTER(_unique_metrics.get(), "NeedInputFalseBothBatchesInFlight", TUnit::UNIT);
         _gpu.init(_unique_metrics.get());
         _frag->add_sink();
@@ -1058,29 +1134,36 @@ public:
     bool need_input() const override {
         if (_finished) return false;
         auto* self = const_cast<GpuFragmentSinkOperator*>(this);
-        if (!_batch[_cur].initialised()) return true;
-        if (_batch[_cur].room() > 0 && !self->_batch[_cur].busy()) return true;
-        const bool ok = !self->_batch[_cur ^ 1].busy(); // the current batch is full: the other one must be free to switch
+        if (_rows(_cur) < _batch_rows && !self->_busy(_cur)) return true;
+        const bool ok = !self->_busy(_cur ^ 1); // the current slot is full: the other one must be free to switch
         if (!ok) COUNTER_UPDATE(self->_no_buffer_counter, 1);
         return ok;
     }
     bool is_finished() const override { return _finished; }
     bool pending_finish() const override {
         auto* self = const_cast<GpuFragmentSinkOperator*>(this);
-        return _finished && (self->_batch[0].busy() || self->_batch[1].busy());
+        return _finished && (self->_busy(0) || self->_busy(1));
     }
     StatusOr<ChunkPtr> pull_chunk(RuntimeState*) override { return Status::InternalError("pull_chunk on a sink"); }
     Status push_chunk(RuntimeState* state, const ChunkPtr& chunk) override {
-        if (!_batch[0].initialised()) {
-            RETURN_IF_ERROR(_frag->prepare());
-            for (auto& b : _batch) RETURN_IF_ERROR(b.init(_frag->ctx(), *chunk, _batch_rows));
+        RETURN_IF_ERROR(_frag->prepare());
+        if (chunk->num_rows() == 0) return Status::OK();
+        if (ForwardedChunkList::forwardable(_frag->ctx(), *chunk)) {
+            if (_batch[_cur].rows() > 0 || _rows(_cur) >= _batch_rows) RETURN_IF_ERROR(_next_slot());
+            RETURN_IF_ERROR(_fwd[_cur].add(_frag->ctx(), chunk));
+            COUNTER_UPDATE(_forwarded_chunks_counter, 1);
+            COUNTER_UPDATE(_forwarded_rows_counter, (int64_t)chunk->num_rows());
+            return Status::OK();
         }
+        for (size_t i = 0; i < chunk->num_columns(); i++)
+            if (chunk->get_column_by_index(i)->is_nullable())
+                return Status::NotSupported("PinnedChunkBatch: nullable column (slot " + std::to_string(chunk->slot_of_index(i)) + ") outside a registered pool");
+        if (!_batch[0].initialised())
+            for (auto& b : _batch) RETURN_IF_ERROR(b.init(_frag->ctx(), *chunk, _batch_rows));
+        if (_fwd[_cur].rows() > 0) RETURN_IF_ERROR(_next_slot()); // a pending forward list goes first
         size_t from = 0;
         while (from < chunk->num_rows()) {
-            if (_batch[_cur].room() == 0) {
-                RETURN_IF_ERROR(_submit());
-                if (_batch[_cur].busy()) _batch[_cur].wait(); // cannot happen under the driver's need_input() protocol
-            }
+            if (_batch[_cur].room() == 0) RETURN_IF_ERROR(_next_slot());
             const size_t before = _batch[_cur].rows();
             {
                 SCOPED_TIMER(_append_timer);
@@ -1093,7 +1176,7 @@ public:
     Status set_finishing(RuntimeState* state) override {
         if (_finished) return Status::OK();
         RETURN_IF_ERROR(_frag->prepare());
-        if (_batch[_cur].initialised() && _batch[_cur].rows() > 0) RETURN_IF_ERROR(_submit());
+        if (_rows(_cur) > 0) RETURN_IF_ERROR(_submit());
         _finished = true;
         return _frag->sink_finished();
     }
@@ -1103,24 +1186,40 @@ public:
     }
 
 private:
-    Status _submit() { // hand the current batch over, continue with the other one
-        sr_chunk_view v = _batch[_cur].view();
+    size_t _rows(int k) const { return _batch[k].rows() + _fwd[k].rows(); }
+    bool _busy(int k) { return _batch[k].busy() | _fwd[k].busy(); }
+    Status _next_slot() { // hand the current slot over and make the other one current
+        RETURN_IF_ERROR(_submit());
+        if (_busy(_cur)) { // cannot happen under the driver's need_input() protocol
+            _batch[_cur].wait();
+            _fwd[_cur].wait();
+        }
+        return Status::OK();
+    }
+    Status _submit() { // hand the current slot over, continue with the other one
         {
             SCOPED_TIMER(_push_timer);
-            RETURN_IF_SR_ERROR(_frag->ctx(), sr_fragment_push(_frag->frag(), &v));
+            if (_fwd[_cur].rows() > 0) {
+                RETURN_IF_ERROR(_fwd[_cur].submit(_frag->frag()));
+            } else {
+                sr_chunk_view v = _batch[_cur].view();
+                RETURN_IF_SR_ERROR(_frag->ctx(), sr_fragment_push(_frag->frag(), &v));
+                COUNTER_UPDATE(_bytes_counter, (int64_t)_batch[_cur].bytes());
+                RETURN_IF_ERROR(_batch[_cur].mark_submitted());
+            }
         }
         COUNTER_UPDATE(_batches_counter, 1);
-        COUNTER_UPDATE(_bytes_counter, (int64_t)_batch[_cur].bytes());
-        RETURN_IF_ERROR(_batch[_cur].mark_submitted());
         _cur ^= 1;
         return Status::OK();
     }
     GpuFragmentPtr _frag;
     size_t _batch_rows;
     PinnedChunkBatch _batch[2];
+    ForwardedChunkList _fwd[2];
     int _cur = 0;
     bool _finished = false;
-    RuntimeProfile::Counter *_append_timer, *_push_timer, *_batches_counter, *_bytes_counter, *_no_buffer_counter;
+    RuntimeProfile::Counter *_append_timer, *_push_timer, *_batches_counter, *_bytes_counter, *_forwarded_chunks_counter, *_forwarded_rows_counter,
+            *_no_buffer_counter;
     GpuOpCounters _gpu;
 };
 
