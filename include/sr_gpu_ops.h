@@ -83,12 +83,14 @@ int32_t sr_type_width(int32_t type);
  *   cudaHostRegister, e.g. a registered ColumnAllocator pool).
  * One rule for all entry points:
  *  1. An unknown kind is refused with SR_ERR_INVALID_ARGUMENT before any copy, allocation or launch.
- *  2. Only sr_fragment_push (the fact columns), sr_fragment_push_chunks (the chunks' columns) and sr_pages_decode (the
- *     pages) read SR_MEM_HOST_PINNED buffers IN PLACE over PCIe: the fragment fetches a column only for the 32-byte
- *     sectors holding rows that survived the earlier joins, so far fewer bytes cross the bus than a full H2D copy;
- *     sr_fragment_push_chunks reads every column the fragment needs in full, once, with device loads.  Where a buffer is
- *     read in place, memory that is not page-locked and mapped is refused with SR_ERR_INVALID_ARGUMENT.  Every other
- *     entry point treats SR_MEM_HOST_PINNED exactly like SR_MEM_HOST, for inputs and for outputs.
+ *  2. Only sr_fragment_push (the fact columns), sr_fragment_push_chunks (the chunks' columns) and sr_pages_decode /
+ *     sr_null_maps_decode (the pages) read SR_MEM_HOST_PINNED buffers IN PLACE over PCIe: the fragment fetches a column
+ *     only for the 32-byte sectors holding rows that survived the earlier joins, so far fewer bytes cross the bus than a
+ *     full H2D copy; sr_fragment_push_chunks reads every column the fragment needs in full, once, with device loads.
+ *     These three resolve a buffer read in place through the library's registry of the ranges made by sr_host_alloc and
+ *     sr_host_register first (no driver call); a pointer outside it costs one driver lookup per allocation and call.
+ *     Memory that is not page-locked and mapped is refused with SR_ERR_INVALID_ARGUMENT.  Every other entry point treats
+ *     SR_MEM_HOST_PINNED exactly like SR_MEM_HOST, for inputs and for outputs.
  *  3. A call that writes its result into host memory (either host kind) synchronises before it returns; a result
  *     handed back in host memory (sr_chunk_out.mem) is reported as SR_MEM_HOST.
  *  4. Host inputs: a call waits for the copies of its host inputs before it returns, so that the caller may free or
@@ -113,7 +115,10 @@ typedef struct sr_col_view {
     int32_t slot_id; /* SlotId the column is registered under in the Chunk */
 } sr_col_view;
 
-/* mirrors column::Chunk (be/src/column/chunk.h:52-354). */
+/* mirrors column::Chunk (be/src/column/chunk.h:52-354).
+ * Every entry point that takes one refuses, with SR_ERR_INVALID_ARGUMENT before any allocation, copy or launch: an
+ * unknown mem kind, num_rows < 0, num_cols < 0, cols == NULL with num_cols > 0, and, in a column it reads, an unknown
+ * type, data == NULL with num_rows > 0 or a column read in place that is not naturally aligned (see sr_col_view). */
 typedef struct sr_chunk_view {
     const sr_col_view* cols;
     int32_t num_cols;
@@ -660,8 +665,6 @@ int32_t sr_fragment_push(sr_fragment* frag, const sr_chunk_view* fact);
  *    num_chunks > 0, an unknown mem kind, chunks of different schemas, negative rows, data == NULL with rows > 0, a device
  *    or pinned column that is not naturally aligned (see sr_col_view), pinned memory that is not page-locked and mapped.
  *    A total of 0xFFFFFFF0 rows or more: SR_ERR_NOT_SUPPORTED, before any column is looked at.
- *  - Pinned pointers are resolved through the library's registry of the ranges made by sr_host_alloc and
- *    sr_host_register (no driver call); a pointer outside it costs one driver lookup per allocation and call.
  *  - Zero chunks, or only empty ones, behave like a zero-row sr_fragment_push (the first push still plans).
  *  - sr_mem rules 2 and 4: the call only queues work; pinned and device chunk buffers must stay valid and unchanged until
  *    an event recorded after the call has completed, or until the next synchronising call. */

@@ -812,10 +812,7 @@ static int32_t frag_push_chunks(sr_fragment* f, const sr_chunk_view* chunks, int
     // headers first: the row total is refused before any column is looked at
     int64_t total = 0;
     for (int32_t c = 0; c < num_chunks; c++) {
-        SR_TRY(mem_check(ctx, chunks[c].mem, "chunk"));
-        if (chunks[c].num_rows < 0) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "chunk %d has %lld rows", c, (long long)chunks[c].num_rows);
-        if (chunks[c].num_cols < 0 || (chunks[c].num_cols > 0 && chunks[c].cols == nullptr))
-            return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "chunk %d: %d columns at %p", c, chunks[c].num_cols, (const void*)chunks[c].cols);
+        SR_TRY(chunk_check(ctx, &chunks[c], c));
         total += chunks[c].num_rows;
         if (total >= 0xFFFFFFF0ll) return sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "fragment batch of more than 2^32 rows; push smaller chunk lists");
     }
@@ -836,12 +833,8 @@ static int32_t frag_push_chunks(sr_fragment* f, const sr_chunk_view* chunks, int
             const sr_col_view& s = c0.cols[k];
             const sr_col_view* m = (ch.cols[k].slot_id == s.slot_id) ? &ch.cols[k] : find_col(&ch, s.slot_id);
             if (!m || m->type != s.type) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "chunk %d: slot %d missing or of another type than in chunk 0", c, s.slot_id);
-            const int w = srd::type_width(m->type);
-            if (w == 0) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "unknown column type %d (slot %d)", m->type, m->slot_id);
-            if (ch.num_rows > 0 && m->data == nullptr) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "chunk %d: null data pointer (slot %d)", c, m->slot_id);
-            const bool in_place = ch.mem == SR_MEM_DEVICE || (ch.mem == SR_MEM_HOST_PINNED && ch.num_rows > 0);
-            if (in_place && !col_aligned(m->data, w))
-                return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "chunk %d: slot %d column at %p is not %d-byte aligned", c, m->slot_id, m->data, std::min(w, 8));
+            int w;
+            SR_TRY(col_check(ctx, *m, ch.num_rows, ch.mem == SR_MEM_DEVICE || (ch.mem == SR_MEM_HOST_PINNED && ch.num_rows > 0), &w, c));
             col_of[(size_t)c * ncols + k] = m;
         }
     }

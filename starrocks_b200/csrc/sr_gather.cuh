@@ -1,13 +1,7 @@
 // sr_gather.cuh -- the chunk-list form of the fragment push (sr_fragment_push_chunks): k_chunk_gather copies the columns
 // of many small chunks (device memory, or page-locked host memory read over PCIe) into one contiguous device batch in
-// one launch, and the host registry of page-locked ranges (sr_host_alloc / sr_host_register) that resolves a pinned
-// pointer to its device alias without a driver call.
+// one launch; ChunkGather launches it and gather_pieces cuts a column into its descriptor entries.
 #pragma once
-
-#include <cuda.h>
-
-#include <map>
-#include <mutex>
 
 #include "sr_host.cuh"
 
@@ -95,98 +89,6 @@ __global__ void __launch_bounds__(CHUNK_GATHER_BLOCK) k_chunk_gather(const Gathe
 }
 
 } // namespace srd
-
-// ---------------------------------------------------------------------------------------
-// page-locked host ranges made by sr_host_alloc / sr_host_register (process-wide: both are portable allocations)
-// ---------------------------------------------------------------------------------------
-struct HostRange {
-    size_t bytes;
-    uintptr_t dev;   // device alias of the range's first byte
-    bool registered; // sr_host_register (else sr_host_alloc)
-};
-struct HostRegistry {
-    std::mutex mu;
-    std::map<uintptr_t, HostRange> ranges; // by first byte
-    // the range holding [p, p + bytes), or nullptr; caller holds mu
-    const std::pair<const uintptr_t, HostRange>* find(uintptr_t p, size_t bytes) {
-        auto it = ranges.upper_bound(p);
-        if (it == ranges.begin()) return nullptr;
-        --it;
-        if (p + bytes > it->first + it->second.bytes) return nullptr;
-        return &*it;
-    }
-    bool overlaps(uintptr_t p, size_t bytes) {
-        auto it = ranges.lower_bound(p);
-        if (it != ranges.end() && it->first < p + bytes) return true;
-        if (it == ranges.begin()) return false;
-        --it;
-        return it->first + it->second.bytes > p;
-    }
-};
-static HostRegistry& host_registry() {
-    static HostRegistry r;
-    return r;
-}
-
-// Device aliases of SR_MEM_HOST_PINNED buffers within one call: the registry first; any other pointer is resolved with
-// cudaPointerGetAttributes, and the allocation it lies in (its extent from the driver's range query, where the driver
-// gives one) is remembered for the rest of the call, so a list of chunks cut from one allocation costs one lookup.
-struct PinnedResolver {
-    struct Known {
-        uintptr_t base;
-        size_t bytes;
-        uintptr_t dev;
-    };
-    std::vector<Known> known;
-    int32_t resolve(sr_ctx* ctx, const void* host, size_t bytes, int32_t slot, const void** dev) {
-        const uintptr_t p = (uintptr_t)host;
-        {
-            HostRegistry& reg = host_registry();
-            std::lock_guard<std::mutex> lk(reg.mu);
-            if (const auto* r = reg.find(p, bytes)) {
-                *dev = (const void*)(r->second.dev + (p - r->first));
-                return SR_OK;
-            }
-        }
-        for (const Known& k : known)
-            if (p >= k.base && p + bytes <= k.base + k.bytes) {
-                *dev = (const void*)(k.dev + (p - k.base));
-                return SR_OK;
-            }
-        cudaPointerAttributes at;
-        memset(&at, 0, sizeof(at));
-        if (cudaPointerGetAttributes(&at, host) != cudaSuccess || at.type != cudaMemoryTypeHost || at.devicePointer == nullptr) {
-            cudaGetLastError();
-            return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "slot %d: SR_MEM_HOST_PINNED buffer is not page-locked mapped host memory", slot);
-        }
-        Known k{p, bytes, (uintptr_t)at.devicePointer};
-        CUdeviceptr start = 0;
-        size_t size = 0;
-        if (range_query(p, &start, &size) && start <= p && p + bytes <= start + size) {
-            k.base = (uintptr_t)start;
-            k.bytes = size;
-            k.dev = (uintptr_t)at.devicePointer - (p - (uintptr_t)start);
-        }
-        known.push_back(k);
-        *dev = at.devicePointer;
-        return SR_OK;
-    }
-    // cuPointerGetAttribute(RANGE_START_ADDR / RANGE_SIZE), fetched through the runtime (the library links no libcuda)
-    static bool range_query(uintptr_t p, CUdeviceptr* start, size_t* size) {
-        typedef CUresult (*get_attr_fn)(void*, CUpointer_attribute, CUdeviceptr);
-        static get_attr_fn fn = []() -> get_attr_fn {
-            void* f = nullptr;
-            cudaDriverEntryPointQueryResult q;
-            if (cudaGetDriverEntryPoint("cuPointerGetAttribute", &f, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess) {
-                cudaGetLastError();
-                return nullptr;
-            }
-            return (get_attr_fn)f;
-        }();
-        return fn && fn(start, CU_POINTER_ATTRIBUTE_RANGE_START_ADDR, (CUdeviceptr)p) == CUDA_SUCCESS &&
-               fn(size, CU_POINTER_ATTRIBUTE_RANGE_SIZE, (CUdeviceptr)p) == CUDA_SUCCESS && *size > 0;
-    }
-};
 
 // What one fragment keeps for sr_fragment_push_chunks: the gathered batch columns, the descriptor table on the device
 // and the page-locked copies of the table it is uploaded from.  An upload buffer is rewritten only once the copy out of

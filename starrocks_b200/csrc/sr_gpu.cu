@@ -724,7 +724,7 @@ int32_t sr_rf_evaluate(sr_rf* rf, const sr_chunk_view* in, int32_t slot_id, uint
     if (!rf || !in || (!selection && in->num_rows > 0)) return SR_ERR_INVALID_ARGUMENT;
     sr_ctx* ctx = rf->ctx;
     SR_BIND(ctx);
-    SR_TRY(mem_check(ctx, in->mem, "chunk"));
+    SR_TRY(chunk_check(ctx, in));
     SR_TRY(mem_check(ctx, sel_mem, "sel_mem"));
     const int64_t n = in->num_rows;
     if (n <= 0) return SR_OK;

@@ -1,13 +1,15 @@
-// sr_host.cuh -- host-side plumbing of libsr_gpu.so: context, device buffers, error handling,
-// compilation of sr_pred / sr_expr descriptors against a chunk's slots.
+// sr_host.cuh -- host-side plumbing of libsr_gpu.so: context, device buffers, error handling, memory kinds and the checks
+// of a caller's chunks, the page-locked host registry, compilation of sr_pred / sr_expr descriptors against a chunk's slots.
 #pragma once
 
+#include <cuda.h>
 #include <cuda_runtime.h>
 
 #include <algorithm>
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
+#include <map>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -248,8 +250,8 @@ static inline bool col_aligned(const void* p, int width) {
     return ((uintptr_t)p & (uintptr_t)(std::min(width, 8) - 1)) == 0;
 }
 
-// memory kinds: the sr_mem rule of include/sr_gpu_ops.h.  Outside the two in-place readers (Staged::stage for
-// sr_fragment_push, pages_decode), SR_MEM_HOST_PINNED is host memory like SR_MEM_HOST.
+// memory kinds: the sr_mem rule of include/sr_gpu_ops.h.  Outside the in-place readers, which resolve pinned buffers with
+// a PinnedResolver (Staged::stage for sr_fragment_push, frag_push_chunks, stage_pages), SR_MEM_HOST_PINNED is SR_MEM_HOST.
 static inline bool mem_is_host(int32_t mem) {
     return mem == SR_MEM_HOST || mem == SR_MEM_HOST_PINNED;
 }
@@ -284,72 +286,168 @@ static int32_t mem_sync(sr_ctx* ctx, int32_t mem) {
     return SR_OK;
 }
 
-// A chunk made resident on the device: host chunks are staged (H2D on the ctx stream) into
-// buffers owned by `Staged`; device chunks (and pinned ones read in place) are referenced in place and must be
-// naturally aligned.
-struct Staged {
-    ColBufs bufs;
-    std::vector<srd::DCol> cols;
-    std::vector<int32_t> slots;
-    int64_t num_rows = 0;
-    // device-visible alias of a page-locked, mapped host buffer (SR_MEM_HOST_PINNED); fails for pageable memory
-    static int32_t mapped_alias(sr_ctx* ctx, const void* host, int32_t slot, const void** dev) {
+// what a refusal calls a caller's chunk: "chunk", or "chunk <index>" for chunk `index` of a list (made only on refusal)
+struct ChunkName {
+    char s[24] = "chunk";
+    explicit ChunkName(int index) { if (index >= 0) snprintf(s, sizeof(s), "chunk %d", index); }
+};
+
+// The header of a caller's chunk, checked before any of its columns is read: a known kind, no negative row or column
+// count, and a column array when it has columns.  `index`: the chunk's place in a list, -1 for a single chunk.
+static int32_t chunk_check(sr_ctx* ctx, const sr_chunk_view* in, int index = -1) {
+    if (in->mem != SR_MEM_DEVICE && !mem_is_host(in->mem)) return mem_check(ctx, in->mem, ChunkName(index).s);
+    if (in->num_rows < 0 || in->num_cols < 0 || (in->num_cols > 0 && in->cols == nullptr))
+        return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "%s: %lld rows, %d columns at %p", ChunkName(index).s, (long long)in->num_rows, in->num_cols, (const void*)in->cols);
+    return SR_OK;
+}
+
+// One column of a caller's chunk of `rows` rows: a known type (*width receives its width), data when there are rows,
+// and, when the kernels read it in place, natural alignment.  `index` as for chunk_check.
+static int32_t col_check(sr_ctx* ctx, const sr_col_view& c, int64_t rows, bool in_place, int* width, int index = -1) {
+    const int w = srd::type_width(c.type);
+    if (w == 0) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "%s: unknown column type %d (slot %d)", ChunkName(index).s, c.type, c.slot_id);
+    if (rows > 0 && c.data == nullptr) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "%s: null data pointer (slot %d)", ChunkName(index).s, c.slot_id);
+    if (in_place && !col_aligned(c.data, w))
+        return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "%s: slot %d column at %p is not %d-byte aligned", ChunkName(index).s, c.slot_id, c.data, std::min(w, 8));
+    *width = w;
+    return SR_OK;
+}
+
+// ---------------------------------------------------------------------------------------
+// page-locked host ranges made by sr_host_alloc / sr_host_register (process-wide: both are portable allocations)
+// ---------------------------------------------------------------------------------------
+struct HostRange {
+    size_t bytes;
+    uintptr_t dev;   // device alias of the range's first byte
+    bool registered; // sr_host_register (else sr_host_alloc)
+};
+struct HostRegistry {
+    std::mutex mu;
+    std::map<uintptr_t, HostRange> ranges; // by first byte
+    // the range holding [p, p + bytes), or nullptr; caller holds mu
+    const std::pair<const uintptr_t, HostRange>* find(uintptr_t p, size_t bytes) {
+        auto it = ranges.upper_bound(p);
+        if (it == ranges.begin()) return nullptr;
+        --it;
+        if (p + bytes > it->first + it->second.bytes) return nullptr;
+        return &*it;
+    }
+    bool overlaps(uintptr_t p, size_t bytes) {
+        auto it = ranges.lower_bound(p);
+        if (it != ranges.end() && it->first < p + bytes) return true;
+        if (it == ranges.begin()) return false;
+        --it;
+        return it->first + it->second.bytes > p;
+    }
+};
+static HostRegistry& host_registry() {
+    static HostRegistry r;
+    return r;
+}
+
+// Device aliases of SR_MEM_HOST_PINNED buffers read in place, within one call: the registry first; any other pointer costs a
+// driver query, and the allocation it lies in (its extent from the driver's range query, where the driver gives one) is
+// remembered for the rest of the call, so buffers cut from one allocation cost one lookup.  Unmapped memory is refused.
+struct PinnedResolver {
+    struct Known {
+        uintptr_t base;
+        size_t bytes;
+        uintptr_t dev;
+    };
+    std::vector<Known> known;
+    int32_t resolve(sr_ctx* ctx, const void* host, size_t bytes, int32_t slot, const void** dev) {
+        const uintptr_t p = (uintptr_t)host;
+        {
+            HostRegistry& reg = host_registry();
+            std::lock_guard<std::mutex> lk(reg.mu);
+            if (const auto* r = reg.find(p, bytes)) {
+                *dev = (const void*)(r->second.dev + (p - r->first));
+                return SR_OK;
+            }
+        }
+        for (const Known& k : known)
+            if (p >= k.base && p + bytes <= k.base + k.bytes) {
+                *dev = (const void*)(k.dev + (p - k.base));
+                return SR_OK;
+            }
         cudaPointerAttributes at;
         memset(&at, 0, sizeof(at));
         if (cudaPointerGetAttributes(&at, host) != cudaSuccess || at.type != cudaMemoryTypeHost || at.devicePointer == nullptr) {
             cudaGetLastError();
             return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "slot %d: SR_MEM_HOST_PINNED buffer is not page-locked mapped host memory", slot);
         }
+        Known k{p, bytes, (uintptr_t)at.devicePointer};
+        CUdeviceptr start = 0;
+        size_t size = 0;
+        if (range_query(p, &start, &size) && start <= p && p + bytes <= start + size) {
+            k.base = (uintptr_t)start;
+            k.bytes = size;
+            k.dev = (uintptr_t)at.devicePointer - (p - (uintptr_t)start);
+        }
+        known.push_back(k);
         *dev = at.devicePointer;
         return SR_OK;
     }
+    // cuPointerGetAttribute(RANGE_START_ADDR / RANGE_SIZE), fetched through the runtime (the library links no libcuda)
+    static bool range_query(uintptr_t p, CUdeviceptr* start, size_t* size) {
+        typedef CUresult (*get_attr_fn)(void*, CUpointer_attribute, CUdeviceptr);
+        static get_attr_fn fn = []() -> get_attr_fn {
+            void* f = nullptr;
+            cudaDriverEntryPointQueryResult q;
+            if (cudaGetDriverEntryPoint("cuPointerGetAttribute", &f, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess) {
+                cudaGetLastError();
+                return nullptr;
+            }
+            return (get_attr_fn)f;
+        }();
+        return fn && fn(start, CU_POINTER_ATTRIBUTE_RANGE_START_ADDR, (CUdeviceptr)p) == CUDA_SUCCESS &&
+               fn(size, CU_POINTER_ATTRIBUTE_RANGE_SIZE, (CUdeviceptr)p) == CUDA_SUCCESS && *size > 0;
+    }
+};
+
+// A chunk made resident on the device: host chunks are staged (H2D on the ctx stream) into buffers owned by `Staged`;
+// device chunks, and pinned ones read in place (`in_place_pinned`), are referenced in place.  Every column is checked,
+// and a pinned one resolved, before anything is allocated or copied.
+struct Staged {
+    ColBufs bufs;
+    std::vector<srd::DCol> cols;
+    std::vector<int32_t> slots;
+    int64_t num_rows = 0;
     int32_t stage(sr_ctx* ctx, const sr_chunk_view* in, const std::vector<int32_t>* only_slots = nullptr, bool in_place_pinned = false) {
         cols.clear();
         slots.clear();
         num_rows = in->num_rows;
-        SR_TRY(mem_check(ctx, in->mem, "chunk"));
-        bufs.resize(in->num_cols);
+        SR_TRY(chunk_check(ctx, in));
+        const bool pinned = in->mem == SR_MEM_HOST_PINNED && in_place_pinned && in->num_rows > 0;
+        const bool in_place = in->mem == SR_MEM_DEVICE || pinned;
+        PinnedResolver resolver;
         for (int k = 0; k < in->num_cols; k++) {
             const sr_col_view& c = in->cols[k];
             if (only_slots && std::find(only_slots->begin(), only_slots->end(), c.slot_id) == only_slots->end()) continue;
-            const int w = srd::type_width(c.type);
-            if (w == 0) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "unknown column type %d (slot %d)", c.type, c.slot_id);
-            if (in->num_rows > 0 && c.data == nullptr)
-                return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "null data pointer (slot %d)", c.slot_id);
-            srd::DCol d;
-            d.type = c.type;
-            d.width = w;
-            if (in->mem == SR_MEM_DEVICE) {
-                if (!col_aligned(c.data, w))
-                    return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "slot %d: device column at %p is not %d-byte aligned", c.slot_id, c.data, std::min(w, 8));
-                d.data = c.data;
-                d.nulls = c.nulls;
-            } else if (in->mem == SR_MEM_HOST_PINNED && in_place_pinned && in->num_rows > 0) {
-                if (!col_aligned(c.data, w))
-                    return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "slot %d: pinned column at %p is not %d-byte aligned", c.slot_id, c.data, std::min(w, 8));
-                const void* p = nullptr;
-                SR_TRY(mapped_alias(ctx, c.data, c.slot_id, &p));
-                d.data = p;
-                d.nulls = nullptr;
-                if (c.nulls) {
-                    SR_TRY(mapped_alias(ctx, c.nulls, c.slot_id, &p));
-                    d.nulls = (const uint8_t*)p;
-                }
-            } else {
-                DevBuf& data = bufs.cols[k].data;
-                DevBuf& nulls = bufs.cols[k].nulls;
-                SR_TRY(data.reserve(ctx, (size_t)in->num_rows * w + 16));
-                SR_CUDA(ctx, cudaMemcpyAsync(data.p, c.data, (size_t)in->num_rows * w, cudaMemcpyHostToDevice, ctx->stream));
-                d.data = data.p;
-                d.nulls = nullptr;
-                if (c.nulls) {
-                    SR_TRY(nulls.reserve(ctx, (size_t)in->num_rows + 16));
-                    SR_CUDA(ctx, cudaMemcpyAsync(nulls.p, c.nulls, (size_t)in->num_rows, cudaMemcpyHostToDevice, ctx->stream));
-                    d.nulls = (const uint8_t*)nulls.p;
-                }
+            srd::DCol d{c.data, c.nulls, c.type, 0};
+            SR_TRY(col_check(ctx, c, num_rows, in_place, &d.width));
+            if (pinned) {
+                SR_TRY(resolver.resolve(ctx, c.data, (size_t)num_rows * d.width, c.slot_id, &d.data));
+                const void* nulls = nullptr;
+                if (c.nulls) SR_TRY(resolver.resolve(ctx, c.nulls, (size_t)num_rows, c.slot_id, &nulls));
+                d.nulls = (const uint8_t*)nulls;
             }
             cols.push_back(d);
             slots.push_back(c.slot_id);
+        }
+        if (in_place) return SR_OK;
+        bufs.resize((int)cols.size());
+        for (size_t k = 0; k < cols.size(); k++) {
+            srd::DCol& d = cols[k];
+            ColBufs::Col& b = bufs.cols[k];
+            SR_TRY(b.data.reserve(ctx, (size_t)num_rows * d.width + 16));
+            SR_CUDA(ctx, cudaMemcpyAsync(b.data.p, d.data, (size_t)num_rows * d.width, cudaMemcpyHostToDevice, ctx->stream));
+            d.data = b.data.p;
+            if (d.nulls) {
+                SR_TRY(b.nulls.reserve(ctx, (size_t)num_rows + 16));
+                SR_CUDA(ctx, cudaMemcpyAsync(b.nulls.p, d.nulls, (size_t)num_rows, cudaMemcpyHostToDevice, ctx->stream));
+                d.nulls = (const uint8_t*)b.nulls.p;
+            }
         }
         return SR_OK;
     }

@@ -707,17 +707,17 @@ static int32_t join_grow(sr_join* j, int64_t need_rows_incl_sentinel) {
 static int32_t join_append(sr_join* j, const sr_chunk_view* chunk) {
     sr_ctx* ctx = j->ctx;
     if (j->built) return sr_fail(ctx, SR_ERR_STATE, "append_build after build_finish");
-    SR_TRY(mem_check(ctx, chunk->mem, "chunk"));
+    SR_TRY(chunk_check(ctx, chunk));
+    int w;
+    for (int k = 0; k < chunk->num_cols; k++) SR_TRY(col_check(ctx, chunk->cols[k], chunk->num_rows, false, &w)); // copied: any alignment
     const cudaMemcpyKind kind = mem_is_host(chunk->mem) ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice;
     if (j->cols.empty()) {
         for (int k = 0; k < chunk->num_cols; k++) {
             const sr_col_view& c = chunk->cols[k];
-            const int w = srd::type_width(c.type);
-            if (w == 0) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "unknown build column type %d", c.type);
             auto* bc = new BuildCol();
             bc->slot = c.slot_id;
             bc->type = c.type;
-            bc->width = w;
+            bc->width = srd::type_width(c.type);
             j->cols.push_back(bc);
         }
         for (int k = 0; k < j->desc.num_keys; k++) {

@@ -766,9 +766,10 @@ static int32_t stage_pages(sr_ctx* ctx, PageScratch* sc, const View* pv, int32_t
             at += (r.bytes + 15) & ~(size_t)15;
         }
     } else {
+        PinnedResolver pinned;
         for (int p = 0; p < num_pages; p++) {
             const void* d = pv[p].data;
-            if (mem == SR_MEM_HOST_PINNED && pv[p].size > 0) SR_TRY(Staged::mapped_alias(ctx, pv[p].data, p, &d));
+            if (mem == SR_MEM_HOST_PINNED && pv[p].size > 0) SR_TRY(pinned.resolve(ctx, pv[p].data, (size_t)pv[p].size, p, &d));
             hp[p].data = (const uint8_t*)d;
             hp[p].size = pv[p].size;
         }

@@ -47,17 +47,17 @@ static int64_t serde_size(const sr_chunk_view* c, int64_t rows) {
 }
 
 static int32_t serde_serialize(sr_ctx* ctx, const sr_chunk_view* c, int64_t r0, int64_t r1, void* dst, int64_t cap, int32_t dst_mem, sr_chunk_pb_meta* meta) {
-    if (c->num_cols < 0 || c->num_cols > SR_MAX_OUT_COLS) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "%d columns", c->num_cols);
+    SR_TRY(chunk_check(ctx, c));
+    if (c->num_cols > SR_MAX_OUT_COLS) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "%d columns", c->num_cols);
     if (r0 < 0 || r1 < r0 || r1 > c->num_rows) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "rows [%lld, %lld) of %lld", (long long)r0, (long long)r1, (long long)c->num_rows);
     const int64_t rows = r1 - r0;
     for (int k = 0; k < c->num_cols; k++) {
-        const int w = srd::type_width(c->cols[k].type);
-        if (w == 0) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "unknown column type %d (slot %d)", c->cols[k].type, c->cols[k].slot_id);
+        int w;
+        SR_TRY(col_check(ctx, c->cols[k], c->num_rows, false, &w)); // copied: any alignment
         if (rows * w >= (1ll << 32)) return sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "a column of %lld bytes: the format stores sizes as uint32", (long long)(rows * w));
     }
     const int64_t total = serde_size(c, rows);
     if (total > cap) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "destination of %lld bytes, %lld needed", (long long)cap, (long long)total);
-    SR_TRY(mem_check(ctx, c->mem, "chunk"));
     SR_TRY(mem_check(ctx, dst_mem, "dst_mem"));
     const bool dst_dev = !mem_is_host(dst_mem), src_dev = !mem_is_host(c->mem);
     const cudaMemcpyKind kind = src_dev ? (dst_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost) : (dst_dev ? cudaMemcpyHostToDevice : cudaMemcpyHostToHost);
