@@ -589,7 +589,9 @@ int32_t sr_agg_convert_to_states(sr_agg* agg, const sr_chunk_view* chunk, sr_chu
  * aggregate_streaming_sink_operator.cpp:173-210: build_hash_map_with_selection, compute_batch_agg_states_with_selection,
  * output_chunk_by_streaming_with_selection): rows whose group is already in the table are aggregated into it; the others
  * create no group and come back in `out` as intermediate rows (the format of sr_agg_convert_to_states), in input order.
- * `out` is owned by the aggregate (valid until its next call). */
+ * `out` is owned by the aggregate (valid until its next call).  A hash-table aggregate refuses a batch of 0x7FFFFFF0 rows
+ * or more with SR_ERR_NOT_SUPPORTED once the chunk is staged, before the conversion to intermediate rows allocates or
+ * launches anything. */
 int32_t sr_agg_push_selective(sr_agg* agg, const sr_chunk_view* chunk, sr_chunk_out* out);
 
 /* Element-wise mergeable view of a DENSE aggregate table (group-by columns with declared ranges, or no

@@ -1048,7 +1048,9 @@ int64_t sr_agg_current_groups(sr_agg* a) {
 }
 
 // the body of sr_agg_convert_to_states; *vt_out receives the bound value table of the staged chunk
-static int32_t agg_convert_impl(sr_agg* a, const sr_chunk_view* chunk, sr_chunk_out* out, VTab* vt_out) {
+// selective: the rows are for sr_agg_push_selective, whose keyed (hash-table) form refuses batches of 0x7FFFFFF0 rows or
+// more; the refusal comes before the conversion allocates or launches anything
+static int32_t agg_convert_impl(sr_agg* a, const sr_chunk_view* chunk, sr_chunk_out* out, VTab* vt_out, bool selective = false) {
     sr_ctx* ctx = a->ctx;
     const sr_agg_desc& d = a->desc;
     if (desc_has_distinct(&d)) return sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "COUNT(DISTINCT) has no intermediate state column");
@@ -1063,6 +1065,9 @@ static int32_t agg_convert_impl(sr_agg* a, const sr_chunk_view* chunk, sr_chunk_
     if (vt_out) *vt_out = vt;
     const int64_t n = chunk->num_rows;
     const srd::AggDev& h = a->host;
+    // at 0x7FFFFFF0 rows the check used to follow the conversion: n * 9 bytes and more were allocated and written first
+    if (selective && !(h.dense || h.num_keys == 0) && n >= 0x7FFFFFF0ll)
+        return sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "selective push of more than 2^31 rows: push smaller batches");
     a->conv_cols.resize(d.num_fns);
     ColBufs::header(out, d.num_group_keys + d.num_fns, n);
     for (int k = 0; k < d.num_group_keys; k++) { // group-by columns travel as they are (device copies of the staged input)
@@ -1109,7 +1114,7 @@ int32_t sr_agg_push_selective(sr_agg* a, const sr_chunk_view* chunk, sr_chunk_ou
     SR_BIND(ctx);
     if (a->finished) return sr_fail(ctx, SR_ERR_STATE, "push after sink_finish");
     VTab vt;
-    SR_TRY(agg_convert_impl(a, chunk, out, &vt)); // every row's intermediate form; compacted to the streamed rows below
+    SR_TRY(agg_convert_impl(a, chunk, out, &vt, true)); // every row's intermediate form; compacted to the streamed rows below
     const int64_t n = chunk->num_rows;
     const srd::AggDev& h = a->host;
     if (h.dense || h.num_keys == 0) { // every group of a range-declared (or single-state) table exists: plain pre-aggregation
@@ -1118,7 +1123,6 @@ int32_t sr_agg_push_selective(sr_agg* a, const sr_chunk_view* chunk, sr_chunk_ou
         return SR_OK;
     }
     if (n == 0) return SR_OK;
-    if (n >= 0x7FFFFFF0ll) return sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "selective push of more than 2^31 rows: push smaller batches");
     SR_TRY(a->sel_flags.reserve(ctx, (size_t)n + 16));
     SR_TRY(a->sel_pos.reserve(ctx, sizeof(uint32_t) * ((size_t)n + 2)));
     SR_CUDA(ctx, cudaMemsetAsync((uint8_t*)a->sel_flags.p + n, 0, 1, ctx->stream)); // flag n = 0: its prefix sum is the total
