@@ -620,8 +620,15 @@ int32_t sr_agg_dense_state(sr_agg* agg, sr_agg_state_array* arrays, int32_t max_
  * pass over the fact columns (no intermediate Chunk materialisation).  This is what the GPU
  * ScanOperator runs when the downstream operators of its pipeline are GPU join probes and a
  * GPU aggregate sink (SURVEY.md section 7 "keep the API, change the cadence").
- * The joins must be built (sr_join_build_finish) INNER / LEFT_SEMI joins with unique build
- * keys; otherwise SR_ERR_NOT_SUPPORTED is returned and the caller runs the per-operator path.
+ * The joins must be built (sr_join_build_finish) INNER, LEFT_SEMI, LEFT_ANTI or LEFT_OUTER joins
+ * on one key column without an other-join conjunct; otherwise SR_ERR_NOT_SUPPORTED is returned
+ * and the caller runs the per-operator path.  Duplicate build keys are allowed (INNER and
+ * LEFT_OUTER joins emit one combination per matching build row).  Payloads are allowed on INNER
+ * and LEFT_OUTER joins only (SR_ERR_INVALID_ARGUMENT otherwise); a LEFT_OUTER payload is
+ * nullable for the aggregate: a probe row without a build row reads NULL.  A build side that
+ * never received a chunk takes a payload's type from sr_join_desc.build_out_types, as
+ * sr_join_probe does, and reads it as NULL (SR_ERR_STATE when the type is not declared).
+ * LEFT_ANTI is not null-aware: a row passes when its key is NULL or no build row has it.
  * ------------------------------------------------------------------------------------- */
 #define SR_MAX_FRAG_JOINS 6
 #define SR_MAX_FRAG_PAYLOAD 2

@@ -66,7 +66,7 @@ struct sr_fragment {
     int cascade_grid = 0;
     // selective mode (sr_frag_pass.cuh): streaming pass -> gather passes -> final pass, planned by frag_plan_passes
     bool selective = false;
-    bool expand = false; // some INNER join has duplicate build keys: selection-vector passes + k_frag_gather_agg<false, SINGLE, true>
+    bool expand = false; // some INNER / LEFT OUTER join has duplicate build keys: selection-vector passes + k_frag_gather_agg<false, SINGLE, true>
     srd::PassDev pass;
     std::vector<int> gather_joins; // probe positions that get a pass of their own
     DevBuf sel[2], pass_counters;
@@ -86,6 +86,10 @@ struct sr_fragment {
     cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
     bool timed_push = false;
     ChunkGather chunk_gather; // sr_fragment_push_chunks: the batch a list of chunks is gathered into
+    // payload columns of a join whose build side never received a chunk (a dimension scan that filtered everything out):
+    // the type sr_join_desc.build_out_types declares over a zeroed row 0, which every probe row reads as NULL
+    // (FragLoader::load) -- what sr_join_probe pads a LEFT OUTER join's rows with
+    BuildCol empty_payload[SR_MAX_FRAG_JOINS][SR_MAX_FRAG_PAYLOAD];
     ~sr_fragment() {
         for (int e = 0; e < 4; e++)
             if (ev[e]) cudaEventDestroy(ev[e]);
@@ -104,8 +108,18 @@ struct FragPayload {
 static FragPayload frag_find_payload(const sr_fragment* f, int32_t slot) {
     for (int j = 0; j < f->num_joins; j++)
         for (int p = 0; p < f->joins[j].num_payload; p++)
-            if (f->joins[j].payload_build_slots[p] == slot) return FragPayload{f->joins[j].join->find_col(slot), j};
+            if (f->joins[j].payload_build_slots[p] == slot) {
+                const BuildCol* bc = f->joins[j].join->find_col(slot);
+                return FragPayload{bc ? bc : &f->empty_payload[j][p], j}; // sr_fragment_create filled the latter
+            }
     return FragPayload{nullptr, -1};
+}
+
+// the type sr_join_desc.build_out_types declares for build slot `slot`, 0 when none is declared
+static int32_t join_declared_out_type(const sr_join* jn, int32_t slot) {
+    for (int k = 0; k < std::min<int32_t>(jn->desc.num_build_out, SR_MAX_JOIN_OUT); k++)
+        if (jn->desc.build_out_slots[k] == slot && srd::type_width(jn->desc.build_out_types[k]) > 0) return jn->desc.build_out_types[k];
+    return 0;
 }
 
 // slot type: fact chunk first, then payload columns of the joins
@@ -116,12 +130,20 @@ static int32_t frag_slot_type(void* user, int32_t slot) {
     const BuildCol* bc = frag_find_payload(f, slot).col;
     return bc ? bc->type : 0;
 }
+// a payload of a LEFT OUTER join is nullable whatever its build column is: a probe row without a build row reads NULL
 static bool frag_slot_nullable(void* user, int32_t slot) {
     sr_fragment* f = ((FragTypeCtx*)user)->f;
     const int k = f->staged.find(slot);
     if (k >= 0) return f->staged.cols[k].nulls != nullptr;
-    const BuildCol* bc = frag_find_payload(f, slot).col;
-    return bc && bc->nullable;
+    const FragPayload pl = frag_find_payload(f, slot);
+    if (pl.join >= 0 && f->joins[pl.join].join->desc.join_type == SR_JOIN_LEFT_OUTER) return true;
+    return pl.col && pl.col->nullable;
+}
+
+// what join j (hint order) does to a probe row (srd::FRAG_FILTER / FRAG_ANTI / FRAG_OUTER)
+static int32_t frag_join_kind(const sr_fragment* f, int j) {
+    const int32_t t = f->joins[j].join->desc.join_type;
+    return t == SR_JOIN_LEFT_ANTI ? srd::FRAG_ANTI : t == SR_JOIN_LEFT_OUTER ? srd::FRAG_OUTER : srd::FRAG_FILTER;
 }
 
 static int32_t frag_bind_vtab(sr_fragment* f, VTab* vt) {
@@ -188,11 +210,13 @@ static int32_t frag_compile(sr_fragment* f) {
         h.joins[j].smem_off = -1;
         h.joins[j].use_bitmap = jn->method != SR_JOIN_METHOD_LINEAR_CHAINED ? 1 : 0;
         h.joins[j].bitmap_words = (int32_t)((std::max<int64_t>(jn->bucket_size, 1) + 31) / 32);
-        // one-to-many INNER join: the final pass walks the build chain of every surviving row
-        h.joins[j].expand = (jn->has_dup && jn->desc.join_type == SR_JOIN_INNER) ? 1 : 0;
+        // one-to-many INNER / LEFT OUTER join: the final pass walks the build chain of every surviving row
+        h.joins[j].kind = frag_join_kind(f, j);
+        h.joins[j].expand = (jn->has_dup && (jn->desc.join_type == SR_JOIN_INNER || jn->desc.join_type == SR_JOIN_LEFT_OUTER)) ? 1 : 0;
         h.joins[j].need_head = h.joins[j].expand;
         h.joins[j].idx32 = (h.joins[j].use_bitmap && jn->min_value >= INT32_MIN && jn->max_value <= INT32_MAX && jn->max_value >= jn->min_value) ? 1 : 0;
         f->order[j] = j;
+        if (h.joins[j].kind != srd::FRAG_OUTER) h.num_filter_joins++;
     }
     // aggregate (its expressions may reference fact slots and payload slots)
     SR_TRY(agg_compile(f->agg, frag_slot_type, frag_slot_nullable, &tc));
@@ -232,11 +256,17 @@ static int32_t frag_compile(sr_fragment* f) {
     return SR_OK;
 }
 
+// whether the final pass of selective mode tests join q (probe order): the filtering and anti joins it was left
+static bool frag_final_tests(const sr_fragment* f, int q) {
+    return q >= f->pass.final_first_join && f->host.joins[q].kind != srd::FRAG_OUTER;
+}
+
 // Plan the batched final pass (k_frag_final_dense) of selective mode, once the join order is fixed.  It applies when
 //  * the aggregate is dense, accumulates in shared memory and has fewer slots than the reserved digit values;
 //  * every join the final pass looks up is range-mapped with unique keys and an int32 range, and its payload columns
-//    are only group keys: it gets a slot-digit directory, built here;
-//  * every join the final pass only tests is a bitmap test;
+//    are only group keys: it gets a slot-digit directory, built here (a LEFT OUTER join's directory holds the all-NULL
+//    digit, 0, for keys without a build row, and the pass reads that digit for keys outside the range too);
+//  * every join the final pass only tests is a bitmap test (inverted for an anti join);
 //  * every aggregate input is one fact column in an integer mode acc_apply_shared handles (COUNT(*), SUM, COUNT, MIN,
 //    MAX on int64 states).
 // Otherwise the generic final pass runs.  That the fact columns are plain int32 is checked per push.
@@ -306,25 +336,27 @@ static int32_t frag_plan_final_dense(sr_fragment* f) {
     int look_join[srd::FINAL_MAX_LOOK] = {};
     for (int q = 0; q < f->num_joins; q++) {
         const srd::FragJoinDev& fj = h.joins[q];
-        const bool test = q >= f->pass.final_first_join;
+        const bool test = frag_final_tests(f, q);
         if (!fj.need_head && !test) continue;
         const int kv = val_of(fj.key_value_id);
         if (!fj.use_bitmap || !fj.idx32 || fj.expand || kv < 0) return SR_OK;
         const uint32_t lo = (uint32_t)(int32_t)fj.j.min_value, span = (uint32_t)(fj.j.max_value - fj.j.min_value);
         if (!fj.need_head) {
             if (fp.num_test == srd::FINAL_MAX_TEST) return SR_OK;
-            fp.test[fp.num_test++] = srd::FinalDense::Test{fj.j.bitmap, lo, span, kv, 0};
+            fp.test[fp.num_test++] = srd::FinalDense::Test{fj.j.bitmap, lo, span, kv, fj.kind == srd::FRAG_ANTI ? 1u : 0u};
             continue;
         }
         if (!key_of_join[q] || fp.num_look == srd::FINAL_MAX_LOOK) return SR_OK;
         look_join[fp.num_look] = q;
-        fp.look[fp.num_look++] = srd::FinalDense::Look{nullptr, lo, span, kv, 0};
+        // every payload of an outer join is a nullable group key (frag_slot_nullable): NULL is index 0 of each, digit 0
+        fp.look[fp.num_look++] = srd::FinalDense::Look{nullptr, lo, span, kv, fj.kind == srd::FRAG_OUTER ? 0u : (uint32_t)SR_DIGIT_MISS};
     }
     // the directories
     for (int L = 0; L < fp.num_look; L++) {
         const int q = look_join[L];
         srd::DigitPlan dp;
         memset(&dp, 0, sizeof(dp));
+        dp.miss = fp.look[L].miss;
         for (int k = 0; k < ah.num_keys; k++) {
             const int id = ah.key_value_id[k];
             if (f->value_src[id] != q) continue;
@@ -357,14 +389,16 @@ static int32_t frag_plan_final_dense(sr_fragment* f) {
 // ---- selection-vector mode (sr_frag_pass.cuh) ----
 
 // which joins the streaming pass, the gather passes and the final pass test, and the streamed join that carries its key
+// (only filtering and anti joins: the outer joins behind them are looked up by the final pass and never tested)
 static void frag_plan_stream_joins(sr_fragment* f) {
     const srd::FragDev& h = f->host;
     const int* ord = f->order;
+    const int nf = h.num_filter_joins;
     // joins whose key column is streamed: the first one, and the second when >= 8 % of the rows reach it
-    int ns = f->num_joins > 0 ? 1 : 0;
-    if (f->num_joins > 1 && f->pred_rate * f->pass_rate[ord[0]] >= 0.08) ns = 2;
+    int ns = nf > 0 ? 1 : 0;
+    if (nf > 1 && f->pred_rate * f->pass_rate[ord[0]] >= 0.08) ns = 2;
     // trailing joins that filter (almost) nothing are tested inline by the final pass
-    int ff = f->num_joins;
+    int ff = nf;
     while (ff > ns && f->pass_rate[ord[ff - 1]] >= 0.9) ff--;
     f->pass.num_stream_joins = ns;
     f->pass.final_first_join = ff;
@@ -451,8 +485,11 @@ static void frag_plan_stream_tests(sr_fragment* f, double reach_pred0) {
         t.span = st.span;
         t.smem_off = -1;
         t.bm = nullptr;
+        t.inv = 0;
+        t.pad = 0;
         if (st.kind == 1) {
             const srd::FragJoinDev& fj = h.joins[st.join];
+            t.inv = fj.kind == srd::FRAG_ANTI ? ~0u : 0u;
             if (fj.use_bitmap && fj.idx32) {
                 t.lo = (uint32_t)(int32_t)fj.j.min_value;
                 t.span = (uint32_t)(fj.j.max_value - fj.j.min_value);
@@ -476,7 +513,7 @@ static void frag_plan_final_vals(sr_fragment* f) {
         if (id >= 0 && id < (int)f->value_src.size() && f->value_src[id] < 0 && std::find(need.begin(), need.end(), id) == need.end()) need.push_back(id);
     };
     for (int q = 0; q < f->num_joins; q++)
-        if (h.joins[q].need_head || q >= f->pass.final_first_join) want(h.joins[q].key_value_id);
+        if (h.joins[q].need_head || frag_final_tests(f, q)) want(h.joins[q].key_value_id);
     const srd::AggDev& ah = f->agg->host;
     for (int k = 0; k < ah.num_keys; k++) want(ah.key_value_id[k]);
     for (int q = 0; q < ah.num_fns; q++)
@@ -553,7 +590,7 @@ static int32_t frag_plan_cascade(sr_fragment* f) {
     for (int q = 0; q < f->num_joins; q++) {
         srd::FragJoinDev& fj = h.joins[q];
         fj.smem_off = -1;
-        if (fj.use_bitmap && words + (size_t)fj.bitmap_words + queue_words <= budget_words) {
+        if (q < h.num_filter_joins && fj.use_bitmap && words + (size_t)fj.bitmap_words + queue_words <= budget_words) {
             fj.smem_off = (int32_t)words;
             words += (size_t)fj.bitmap_words;
             words = (words + 3) & ~(size_t)3;
@@ -604,6 +641,8 @@ static int32_t frag_plan(sr_fragment* f, const VTab& vt, int64_t n) {
         if (std::abs(pa - pb) > 0.15 * std::max(pa, pb)) return pa < pb;
         return h.joins[a].bitmap_words < h.joins[b].bitmap_words;
     });
+    // outer joins filter nothing: they go behind every filtering join
+    std::stable_partition(ord.begin(), ord.end(), [&](int j) { return h.joins[j].kind != srd::FRAG_OUTER; });
     srd::FragJoinDev reordered[SR_MAX_FRAG_JOINS];
     std::vector<int> inv(f->num_joins);
     for (int q = 0; q < f->num_joins; q++) {
@@ -616,7 +655,7 @@ static int32_t frag_plan(sr_fragment* f, const VTab& vt, int64_t n) {
         if (f->value_src[k] >= 0) f->value_src[k] = inv[f->value_src[k]];
     // stream the second join's key together with the first when most of its 64-byte DRAM bursts would
     // be touched anyway: 1 - (1 - p)^16 >= 0.74 for p >= 0.08
-    h.eager1 = (f->num_joins >= 2 && f->pass_rate[ord[0]] >= 0.08) ? 1 : 0;
+    h.eager1 = (h.num_filter_joins >= 2 && f->pass_rate[ord[0]] >= 0.08) ? 1 : 0;
     // ---- mode: when few rows reach the aggregate, run selection-vector passes instead of the cascade ----
     double total_rate = f->pred_rate;
     for (int q = 0; q < f->num_joins; q++) total_rate *= f->pass_rate[ord[q]];

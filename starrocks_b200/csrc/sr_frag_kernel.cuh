@@ -13,15 +13,30 @@ struct FragJoinDev {
     int32_t use_bitmap; // range-mapped table: test the bitmap; otherwise probe the hash table
     int32_t need_head;  // a payload column of this join is read downstream
     int32_t idx32;      // bitmap join whose [min, max] fits int32: 32-bit index arithmetic is exact
-    int32_t expand;     // INNER join whose build side has duplicate keys: a probe row is emitted once per chain entry
-    int32_t pad;
+    int32_t expand;     // INNER / LEFT OUTER join whose build side has duplicate keys: a probe row is emitted once per chain entry
+    int32_t kind;       // FRAG_FILTER, FRAG_ANTI or FRAG_OUTER
 };
+
+// What a fragment join does to a probe row.  FILTER (INNER, LEFT SEMI): the row passes when a build row has its key (a
+// NULL key never matches).  ANTI (LEFT ANTI): the inverted test -- the row passes when its key is NULL or no build row
+// has it.  OUTER (LEFT OUTER): never drops a row; a row without a build row reads NULL payloads (build row 0, the
+// sentinel).  Outer joins are placed after every filtering join and are only ever looked up, in a final pass.
+constexpr int32_t FRAG_FILTER = 0;
+constexpr int32_t FRAG_ANTI = 1;
+constexpr int32_t FRAG_OUTER = 2;
+
+// whether a tested row passes a filtering or anti join: `nul` its key is NULL, `hit` a build row has the key
+__device__ __forceinline__ bool frag_join_pass(int32_t kind, bool nul, bool hit) {
+    return kind == FRAG_ANTI ? (nul || !hit) : (!nul && hit);
+}
 
 struct FragDev {
     int32_t num_preds, num_exprs, num_joins;
     // the second join's key column is streamed together with the first one (its sectors would
     // nearly all be fetched anyway) and travels through queue 0 with the row id
     int32_t eager1;
+    int32_t num_filter_joins; // joins [0, num_filter_joins) filter (FILTER / ANTI), the outer joins follow them
+    int32_t pad;
     CPred preds[8];
     CExpr exprs[4];
     FragJoinDev joins[SR_MAX_FRAG_JOINS];
@@ -88,8 +103,9 @@ struct FragLoader {
             bits = is_float_class(d.type) ? __double_as_longlong(load_double(d.data, d.type, row)) : load_int(d.data, d.type, row);
             return nul;
         }
+        // build row 0 is the sentinel: a LEFT OUTER join without a matching build row reads NULL payloads
         const int64_t r = bidx[d.src];
-        const bool nul = d.nulls != nullptr && d.nulls[r] != 0;
+        const bool nul = r == 0 || (d.nulls != nullptr && d.nulls[r] != 0);
         if (is_float_class(d.type))
             bits = __double_as_longlong(d.type == SR_TYPE_FLOAT ? (double)__ldg((const float*)d.data + r) : __ldg((const double*)d.data + r));
         else
@@ -149,33 +165,32 @@ __device__ __forceinline__ bool join_hit_global(const FragJoinDev& fj, int64_t k
     return join_lookup(fj.j, key) != 0;
 }
 
-// The joins of one row that reached a final pass, in probe order: joins [first_test, S) are tested (a NULL key, a key
-// without a build row or a clear bitmap bit fails the row), and every join whose payload is read downstream (need_head)
-// is looked up.  Fills ld.bidx with the build rows found and, when `head` is given, head[j] with the same chain heads (0
-// for a join not looked up).  Returns whether the row passed.  `joins` and `S` are read through references: the cascade
-// keeps them in its per-warp state in local memory, and re-reading them there per join keeps copies out of k_fragment's
-// registers (capped at 64, already spilling) across the walk.
+// The joins of one row that reached a final pass, in probe order: the filtering and anti joins of [first_test, S) are
+// tested (frag_join_pass), and every join whose payload is read downstream or whose chain expands (need_head) is looked
+// up -- an outer join only that way: it never fails the row, and a NULL key or a key without a build row leaves build
+// row 0, whose payloads read NULL.  Fills ld.bidx with the build rows found and, when `head` is given, head[j] with the
+// same chain heads (0 for a join not looked up).  Returns whether the row passed.  `joins` and `S` are read through
+// references: the cascade keeps them in its per-warp state in local memory, and re-reading them there per join keeps
+// copies out of k_fragment's registers (capped at 64, already spilling) across the walk.
 __device__ __forceinline__ bool frag_final_joins(const FragJoinDev* const& joins, const int& S, int first_test, FragLoader& ld, uint32_t* head) {
     bool ok = true;
 #pragma unroll 1
     for (int j = 0; j < S && ok; j++) {
         if (head) head[j] = 0;
-        const bool test = j >= first_test;
+        const bool test = j >= first_test && joins[j].kind != FRAG_OUTER;
         if (!test && !joins[j].need_head) continue;
         int64_t key;
         const bool nul = ld.load(joins[j].key_value_id, key);
-        if (test && nul) {
-            ok = false;
-            break;
-        }
+        bool hit = false;
         if (joins[j].need_head || !joins[j].use_bitmap) {
-            const uint32_t h = join_lookup(joins[j].j, key);
+            const uint32_t h = nul ? 0u : join_lookup(joins[j].j, key);
             ld.bidx[j] = h;
             if (head) head[j] = h;
-            if (test && h == 0) ok = false;
-        } else if (test) {
-            if (!join_hit_global(joins[j], key)) ok = false;
+            hit = h != 0;
+        } else if (test && !nul) {
+            hit = join_hit_global(joins[j], key);
         }
+        if (test && !frag_join_pass(joins[j].kind, nul, hit)) ok = false;
     }
     return ok;
 }
@@ -244,18 +259,18 @@ struct Cascade {
     // queue k < NQ-1: probe join k+1 for up to 32 queued rows, survivors go to queue k+1
     __device__ __forceinline__ void consume_join(int k, uint32_t row32, int32_t carried_key, bool valid) {
         const FragJoinDev& fj = joins[k + 1];
-        bool hit = false;
+        bool pass = false;
         if (valid) {
-            if (k == 0 && eager1) {
-                hit = frag_join_hit(fj, smem, (int64_t)carried_key);
+            if (k == 0 && eager1) { // the eagerly streamed key column is never nullable
+                pass = frag_join_pass(fj.kind, false, frag_join_hit(fj, smem, (int64_t)carried_key));
             } else {
                 const VDesc& d = vt.v[fj.key_value_id];
                 const int64_t key = load_int(d.data, d.type, (int64_t)row32);
                 const bool nul = d.nulls != nullptr && d.nulls[row32] != 0;
-                hit = !nul && frag_join_hit(fj, smem, key);
+                pass = frag_join_pass(fj.kind, nul, !nul && frag_join_hit(fj, smem, key));
             }
         }
-        append(k + 1, row32, hit);
+        append(k + 1, row32, pass);
     }
     // take the last `take` rows of queue k and run its consumer
     __device__ __noinline__ void drain(int k, uint32_t take) {
@@ -298,6 +313,8 @@ __global__ void __launch_bounds__(FRAG_BLOCK, 2) k_fragment(const FragDev* __res
     const FragDev& fd = *fdp;
     const AggDev& ad = *adp;
     const int S = fd.num_joins;
+    // the filtering joins are the queue stages; the outer joins behind them are looked up by consume_final only
+    const int SF = fd.num_filter_joins;
     // descriptors + bitmaps of the leading joins into shared memory
     smem_copy(s_joins, fd.joins, S);
     smem_copy(s_preds, fd.preds, fd.num_preds);
@@ -319,19 +336,19 @@ __global__ void __launch_bounds__(FRAG_BLOCK, 2) k_fragment(const FragDev* __res
     bool fast0 = false, fast1 = false;
     const int32_t* key0 = nullptr;
     const int32_t* key1 = nullptr;
-    if (S > 0 && fd.num_preds == 0 && fd.num_exprs == 0) {
+    if (SF > 0 && fd.num_preds == 0 && fd.num_exprs == 0) {
         const VDesc& d0 = vt.v[s_joins[0].key_value_id];
         fast0 = type_width(d0.type) == 4 && !is_float_class(d0.type) && d0.nulls == nullptr && (((uintptr_t)d0.data) & 15) == 0;
         key0 = (const int32_t*)d0.data;
-        if (fast0 && fd.eager1 && S > 1) {
+        if (fast0 && fd.eager1 && SF > 1) {
             const VDesc& d1 = vt.v[s_joins[1].key_value_id];
             fast1 = type_width(d1.type) == 4 && !is_float_class(d1.type) && d1.nulls == nullptr && (((uintptr_t)d1.data) & 15) == 0;
             key1 = (const int32_t*)d1.data;
         }
     }
 
-    // queue k feeds join k+1 (k+1 < S) or the aggregate (the last queue)
-    Cascade cs{vt, ad, acc, s_joins, smem, wq, wq + (SR_MAX_FRAG_JOINS + 1) * FRAG_QCAP, S, S > 1 ? S : 1, fast1 ? 1 : 0, SMEM_AGG ? 1 : 0, lane_id(), 0ull, fail_rows, fail_count};
+    // queue k feeds join k+1 (k+1 < SF) or the aggregate (the last queue)
+    Cascade cs{vt, ad, acc, s_joins, smem, wq, wq + (SR_MAX_FRAG_JOINS + 1) * FRAG_QCAP, S, SF > 1 ? SF : 1, fast1 ? 1 : 0, SMEM_AGG ? 1 : 0, lane_id(), 0ull, fail_rows, fail_count};
 
     const int64_t num_tiles = (n + FRAG_TILE - 1) / FRAG_TILE;
     const int64_t full_tiles = n / FRAG_TILE; // tiles [0, full_tiles) have every row in range
@@ -376,7 +393,7 @@ __global__ void __launch_bounds__(FRAG_BLOCK, 2) k_fragment(const FragDev* __res
                 k1v[g][3] = pk1[g].w;
 #pragma unroll
                 for (int r = 0; r < FRAG_ROWS; r++)
-                    if (!frag_join_hit(fj, smem, (int64_t)kv[r])) alive[g] &= ~(1u << r);
+                    if (!frag_join_pass(fj.kind, false, frag_join_hit(fj, smem, (int64_t)kv[r]))) alive[g] &= ~(1u << r);
             }
             prefetch(tile + gridDim.x);
         } else {
@@ -410,17 +427,19 @@ __global__ void __launch_bounds__(FRAG_BLOCK, 2) k_fragment(const FragDev* __res
                     }
             }
             // ---- first join on its key column ----
-            if (S > 0) {
+            if (SF > 0) {
                 const FragJoinDev& fj = s_joins[0];
                 const VDesc& d = vt.v[fj.key_value_id];
 #pragma unroll
                 for (int g = 0; g < FRAG_GROUPS; g++) load_rows4(d, row0[g], alive[g], vals[g], nullmask[g]);
 #pragma unroll
                 for (int g = 0; g < FRAG_GROUPS; g++) {
-                    alive[g] &= ~nullmask[g]; // NULL keys never match (join_hash_table.cpp:166-170)
+                    // NULL keys never match (join_hash_table.cpp:166-170): they fail a filtering join and pass an anti join
+                    const uint32_t tested = alive[g] & ~nullmask[g];
+                    if (fj.kind != FRAG_ANTI) alive[g] = tested;
 #pragma unroll
                     for (int r = 0; r < FRAG_ROWS; r++)
-                        if ((alive[g] & (1u << r)) && !frag_join_hit(fj, smem, vals[g][r])) alive[g] &= ~(1u << r);
+                        if ((tested & (1u << r)) && !frag_join_pass(fj.kind, false, frag_join_hit(fj, smem, vals[g][r]))) alive[g] &= ~(1u << r);
                 }
                 if (fast1) { // tail tile of a streamed run: the consumer of queue 0 expects the key to ride along
 #pragma unroll
@@ -490,13 +509,15 @@ __global__ void __launch_bounds__(256) k_frag_sample(const FragDev* __restrict__
             const uint32_t m = __ballot_sync(__activemask(), pass);
             if (pass && (m & lanemask_lt()) == 0) atomicAdd(&counts[SAMPLE_ALL_PREDS], (unsigned long long)__popc(m));
         }
+        // rows each join lets through: an outer join all of them
         for (int j = 0; j < fd.num_joins; j++) {
             const FragJoinDev& fj = fd.joins[j];
             int64_t key;
             const bool nul = ld.load(fj.key_value_id, key);
             const bool hit = !nul && join_lookup(fj.j, key) != 0;
-            const uint32_t m = __ballot_sync(__activemask(), hit);
-            if (hit && (m & lanemask_lt()) == 0) atomicAdd(&counts[j], (unsigned long long)__popc(m));
+            const bool pass = fj.kind == FRAG_OUTER || frag_join_pass(fj.kind, nul, hit);
+            const uint32_t m = __ballot_sync(__activemask(), pass);
+            if (pass && (m & lanemask_lt()) == 0) atomicAdd(&counts[j], (unsigned long long)__popc(m));
         }
     }
 }

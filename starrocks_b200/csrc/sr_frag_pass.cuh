@@ -35,12 +35,16 @@ struct StreamTest {
 // shared memory per tile.  kind: 0 = range conjunct, 1 = bitmap in shared memory at word smem_off (int32 index arithmetic,
 // zero GUARD bit at index span + 1: an out-of-range key is clamped onto it, so the test needs neither a predicate nor a
 // select), 2 = bitmap in global memory at bm (predicated word fetches, issued back to back), 3 = anything else (falls back
-// to stream_test).  lo / span: the range, or the join table's [min, min + span].
+// to stream_test).  lo / span: the range, or the join table's [min, min + span].  inv (kinds 1 and 2): all ones for an anti
+// join, whose test is the inverted bitmap test -- one 3-input logic op, (hits ^ inv) & alive; an out-of-range key reads a
+// clear bit and so passes it.
 struct VecTest {
     uint32_t kind;
     uint32_t lo, span;
     int32_t smem_off;
     const uint32_t* bm;
+    uint32_t inv;
+    uint32_t pad;
 };
 
 struct PassDev {
@@ -309,10 +313,13 @@ __global__ void __launch_bounds__(STREAM_BLOCK, 2) k_frag_stream(const FragDev* 
                 for (int g = 0; g < STREAM_GROUPS; g++) load_rows4(d, row0[g], alive[g], vals[g], nullmask[g]);
 #pragma unroll
                 for (int g = 0; g < STREAM_GROUPS; g++) {
-                    alive[g] &= ~nullmask[g]; // NULL keys never match (join_hash_table.cpp:166-170)
+                    // NULL keys never match (join_hash_table.cpp:166-170): they fail a filtering join and pass an anti join
+                    const uint32_t tested = alive[g] & ~nullmask[g];
+                    if (s_joins[j].kind != FRAG_ANTI) alive[g] = tested;
 #pragma unroll
                     for (int r = 0; r < STREAM_ROWS; r++)
-                        if ((alive[g] & (1u << r)) && !frag_join_hit(s_joins[j], smem, vals[g][r])) alive[g] &= ~(1u << r);
+                        if ((tested & (1u << r)) && !frag_join_pass(s_joins[j].kind, false, frag_join_hit(s_joins[j], smem, vals[g][r])))
+                            alive[g] &= ~(1u << r);
                 }
                 if (CARRY && j == pd.carry_join) {
 #pragma unroll
@@ -349,7 +356,9 @@ __device__ __forceinline__ uint32_t stream_test(const StreamTest& st, const Frag
         for (int i = 0; i < N; i++) out |= ((uint32_t)k[i] - st.lo <= st.span ? 1u : 0u) << i;
         return out & alive;
     }
-    return join_test_batch<N>(s_joins[st.join], smem, k, alive);
+    const FragJoinDev& fj = s_joins[st.join];
+    const uint32_t inv = fj.kind == FRAG_ANTI ? ~0u : 0u; // the hits are a subset of `alive`
+    return (join_test_batch<N>(fj, smem, k, alive) ^ inv) & alive;
 }
 
 // one of the two vector-column tests of k_frag_stream_tests in the form the host planned (VecTest); sbm = smem +
@@ -366,7 +375,7 @@ __device__ __forceinline__ uint32_t stream_test_reg(const VecTest& t, const uint
             const uint32_t word = sbm[idx >> 5];
             out |= __funnelshift_r(word, word, idx - (uint32_t)i) & (1u << i);
         }
-        return out & alive;
+        return (out ^ t.inv) & alive;
     }
     if (t.kind == 2) {
         uint32_t words[N];
@@ -380,7 +389,7 @@ __device__ __forceinline__ uint32_t stream_test_reg(const VecTest& t, const uint
             const uint32_t idx = (uint32_t)k[i] - t.lo;
             out |= __funnelshift_r(words[i], words[i], idx - (uint32_t)i) & (1u << i);
         }
-        return out;
+        return (out ^ t.inv) & alive;
     }
     if (t.kind == 0) {
 #pragma unroll
@@ -528,7 +537,7 @@ __global__ void __launch_bounds__(GATHER_BLOCK) k_frag_gather_join(const FragDev
             // directories resident changed neither pass on H100: 0.569 / 0.752 ms against 0.569 / 0.748 ms)
             const int64_t key = load_int(d.data, d.type, (int64_t)row);
             const bool nul = d.nulls != nullptr && d.nulls[row] != 0;
-            hit = !nul && join_hit_global(fj, key); // global bitmap copy: L1/L2 resident
+            hit = frag_join_pass(fj.kind, nul, !nul && join_hit_global(fj, key)); // global bitmap copy: L1/L2 resident
         }
         const uint32_t m = __ballot_sync(SR_FULL_MASK, hit);
         if (m) {
@@ -666,9 +675,9 @@ __global__ void __launch_bounds__(GATHER_BLOCK, GATHER_AGG_MIN_BLOCKS) k_frag_ga
 // A SLOT-DIGIT DIRECTORY replaces the two dependent lookups first[key - min] -> payload[b] of a join whose payload
 // columns are only dense group keys: digit[key - min] is that join's share of the group slot, sum of idx_k * stride_k
 // over the group keys that are its payloads (idx_k as agg_find_slot computes it).  Two values are reserved: MISS (no
-// build row: the row fails the join) and BAD (a payload outside the declared range, or NULL where the key is not
-// nullable: the row passes, flags[1] is set, nothing is aggregated -- what agg_find_slot does).  2 bytes per key of
-// the range, half of first[].
+// build row: the row fails the join; a LEFT OUTER join's directory holds its all-NULL digit there instead) and BAD (a
+// payload outside the declared range, or NULL where the key is not nullable: the row passes, flags[1] is set, nothing
+// is aggregated -- what agg_find_slot does).  2 bytes per key of the range, half of first[].
 #define SR_DIGIT_MISS 0xFFFFu
 #define SR_DIGIT_BAD 0xFFFEu
 
@@ -682,7 +691,7 @@ struct DigitKey {
 };
 struct DigitPlan {
     int32_t num_keys;
-    int32_t pad;
+    uint32_t miss; // the digit of a key without a build row: SR_DIGIT_MISS, or a LEFT OUTER join's all-NULL digit
     DigitKey k[SR_MAX_GROUP_KEYS];
 };
 
@@ -691,7 +700,7 @@ __global__ void __launch_bounds__(256) k_frag_build_digits(const uint32_t* __res
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
         const uint32_t b = first[i];
         if (b == 0) {
-            digit[i] = (uint16_t)SR_DIGIT_MISS;
+            digit[i] = (uint16_t)dp.miss;
             continue;
         }
         long long slot = 0;
@@ -735,12 +744,14 @@ struct FinalDense {
     struct Look {
         const uint16_t* digit;
         uint32_t lo, span; // directory index = key - lo, valid when <= span
-        int32_t val, pad;
+        int32_t val;
+        uint32_t miss; // the digit of a key outside the directory: SR_DIGIT_MISS, or a LEFT OUTER join's all-NULL digit
     } look[FINAL_MAX_LOOK];
     struct Test {
         const uint32_t* bitmap;
         uint32_t lo, span;
-        int32_t val, pad;
+        int32_t val;
+        uint32_t inv; // 1 for an anti join: the row passes on a clear bit
     } test[FINAL_MAX_TEST];
     struct FKey {
         long long lo;     // dense_min
@@ -837,7 +848,7 @@ __global__ void __launch_bounds__(GATHER_BLOCK, FINAL_MIN_BLOCKS) k_frag_final_d
                 dg[r][L] = 0;
                 if (L < fp.num_look) {
                     const uint32_t idx = (uint32_t)final_pick(v[r], fp.look[L].val) - fp.look[L].lo;
-                    dg[r][L] = ldg_u16_pred(fp.look[L].digit + idx, ((live >> r) & 1u) && idx <= fp.look[L].span, SR_DIGIT_MISS);
+                    dg[r][L] = ldg_u16_pred(fp.look[L].digit + idx, ((live >> r) & 1u) && idx <= fp.look[L].span, fp.look[L].miss);
                 }
             }
         }
@@ -849,7 +860,7 @@ __global__ void __launch_bounds__(GATHER_BLOCK, FINAL_MIN_BLOCKS) k_frag_final_d
                 if (t < fp.num_test) {
                     const uint32_t idx = (uint32_t)final_pick(v[r], fp.test[t].val) - fp.test[t].lo;
                     tw[r][t] = ldg_u32_pred(fp.test[t].bitmap + (idx >> 5), ((live >> r) & 1u) && idx <= fp.test[t].span);
-                    tw[r][t] = (tw[r][t] >> (idx & 31)) & 1u;
+                    tw[r][t] = ((tw[r][t] >> (idx & 31)) & 1u) ^ fp.test[t].inv;
                 }
             }
         }

@@ -1188,8 +1188,9 @@ sr_fragment* sr_fragment_create(sr_ctx* ctx, const sr_fragment_desc* desc) {
             sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "fragment join %d belongs to another context", j);
             return nullptr;
         }
-        if (fj.join->desc.join_type != SR_JOIN_INNER && fj.join->desc.join_type != SR_JOIN_LEFT_SEMI) {
-            sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "fused fragment supports INNER / LEFT SEMI joins (join %d is type %d)", j, fj.join->desc.join_type);
+        const int32_t jt = fj.join->desc.join_type;
+        if (jt != SR_JOIN_INNER && jt != SR_JOIN_LEFT_SEMI && jt != SR_JOIN_LEFT_ANTI && jt != SR_JOIN_LEFT_OUTER) {
+            sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "fused fragment supports INNER / LEFT SEMI / LEFT ANTI / LEFT OUTER joins (join %d is type %d)", j, jt);
             return nullptr;
         }
         if (fj.join->desc.other_conjunct.num_nodes > 0) {
@@ -1200,15 +1201,24 @@ sr_fragment* sr_fragment_create(sr_ctx* ctx, const sr_fragment_desc* desc) {
             sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "fused fragment supports single-column join keys (join %d)", j);
             return nullptr;
         }
-        if (fj.num_payload < 0 || fj.num_payload > SR_MAX_FRAG_PAYLOAD || (fj.num_payload > 0 && fj.join->desc.join_type != SR_JOIN_INNER)) {
+        if (fj.num_payload < 0 || fj.num_payload > SR_MAX_FRAG_PAYLOAD || (fj.num_payload > 0 && jt != SR_JOIN_INNER && jt != SR_JOIN_LEFT_OUTER)) {
             sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "fragment join %d payload", j);
             return nullptr;
         }
-        for (int p = 0; p < fj.num_payload; p++)
-            if (!fj.join->find_col(fj.payload_build_slots[p])) {
-                sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "fragment join %d: payload slot %d not in the build chunk", j, fj.payload_build_slots[p]);
+        for (int p = 0; p < fj.num_payload; p++) {
+            const int32_t slot = fj.payload_build_slots[p];
+            if (fj.join->find_col(slot)) continue;
+            if (!fj.join->cols.empty()) {
+                sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "fragment join %d: payload slot %d not in the build chunk", j, slot);
                 return nullptr;
             }
+            // no build chunk ever arrived: the payload's type must be declared, as sr_join_probe needs it
+            if (join_declared_out_type(fj.join, slot) == 0) {
+                sr_fail(ctx, SR_ERR_STATE, "fragment join %d: build side is empty and the type of payload slot %d is unknown: declare it in sr_join_desc.build_out_types",
+                        j, slot);
+                return nullptr;
+            }
+        }
     }
     if (agg_validate_desc(ctx, &desc->agg) != SR_OK) return nullptr;
     if (desc_has_distinct(&desc->agg)) {
@@ -1223,8 +1233,29 @@ sr_fragment* sr_fragment_create(sr_ctx* ctx, const sr_fragment_desc* desc) {
     f->force_mode = (desc->mode_hint == 1 || desc->mode_hint == 2) ? desc->mode_hint : 0;
     for (int j = 0; j < desc->num_joins; j++) {
         f->joins[j] = desc->joins[j];
-        // one-to-many INNER join (duplicate build keys): always the selection-vector passes, whose final pass expands
-        if (desc->joins[j].join->has_dup && desc->joins[j].join->desc.join_type == SR_JOIN_INNER) f->expand = true;
+        for (int p = 0; p < desc->joins[j].num_payload; p++) {
+            const sr_join* jn = desc->joins[j].join;
+            const int32_t slot = desc->joins[j].payload_build_slots[p];
+            if (jn->find_col(slot)) continue;
+            BuildCol& bc = f->empty_payload[j][p];
+            bc.slot = slot;
+            bc.type = join_declared_out_type(jn, slot);
+            bc.width = srd::type_width(bc.type);
+            bc.nullable = false;
+            const auto zero_row = [&]() -> int32_t {
+                SR_TRY(bc.data.reserve(ctx, 16));
+                SR_CUDA(ctx, cudaMemsetAsync(bc.data.p, 0, 16, ctx->stream));
+                return SR_OK;
+            };
+            if (zero_row() != SR_OK) {
+                delete f;
+                return nullptr;
+            }
+        }
+        // one-to-many INNER / LEFT OUTER join (duplicate build keys): always the selection-vector passes, whose final pass
+        // expands
+        const int32_t jt = desc->joins[j].join->desc.join_type;
+        if (desc->joins[j].join->has_dup && (jt == SR_JOIN_INNER || jt == SR_JOIN_LEFT_OUTER)) f->expand = true;
     }
     f->agg = new sr_agg();
     f->agg->ctx = ctx;
