@@ -424,7 +424,7 @@ static void frag_plan_stream_joins(sr_fragment* f) {
 static void frag_plan_stream_smem(sr_fragment* f) {
     srd::FragDev& h = f->host;
     size_t sw = 0;
-    const size_t sbudget = (100 * 1024 - (f->pass.carry_join >= 0 ? sizeof(int4) * srd::STREAM_GROUPS * srd::STREAM_BLOCK : 0)) / 4;
+    const size_t sbudget = (100 * 1024 - (f->pass.carry_join >= 0 ? sizeof(int4) * srd::FRAG_GROUPS * srd::FRAG_BLOCK : 0)) / 4;
     for (int q = 0; q < f->num_joins; q++) {
         srd::FragJoinDev& fj = h.joins[q];
         fj.smem_off = -1;
@@ -546,7 +546,7 @@ static int32_t frag_plan_pass_grids(sr_fragment* f) {
     SR_CUDA(ctx, cudaFuncSetAttribute(srd::k_frag_stream_tests<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, stream_smem_limit));
     SR_CUDA(ctx, cudaFuncSetAttribute(srd::k_frag_stream_tests<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, stream_smem_limit));
     int per_sm = 0;
-    SR_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, srd::k_frag_stream<false>, srd::STREAM_BLOCK, f->stream_smem));
+    SR_CUDA(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, srd::k_frag_stream<false>, srd::FRAG_BLOCK, f->stream_smem));
     if (per_sm < 1) return sr_fail(ctx, SR_ERR_CUDA, "streaming pass does not fit on an SM (smem %zu)", f->stream_smem);
     f->stream_grid = per_sm * ctx->num_sms;
     // gather passes: exactly one wave of resident CTAs (grid-stride loops; a partial second wave only adds a tail)
@@ -742,7 +742,7 @@ static int32_t frag_push(sr_fragment* f, const sr_chunk_view* fact) {
     if (f->selective) {
         const srd::FragDev* fdev = (const srd::FragDev*)f->dev.p;
         // worst case every row survives, plus one partly used chunk per warp of the writing pass
-        const size_t slack = (size_t)srd::SEL_CHUNK * ((size_t)f->stream_grid * (srd::STREAM_BLOCK / 32) + (size_t)f->gather_grid * (srd::GATHER_BLOCK / 32));
+        const size_t slack = (size_t)srd::SEL_CHUNK * ((size_t)f->stream_grid * (srd::FRAG_BLOCK / 32) + (size_t)f->gather_grid * (srd::GATHER_BLOCK / 32));
         SR_TRY(f->sel[0].reserve(ctx, sizeof(srd::SelEntry) * ((size_t)n + slack)));
         if (!f->gather_joins.empty()) SR_TRY(f->sel[1].reserve(ctx, sizeof(srd::SelEntry) * ((size_t)n + slack)));
         const srd::PassDev& pass = f->pass;
@@ -750,7 +750,7 @@ static int32_t frag_push(sr_fragment* f, const sr_chunk_view* fact) {
         unsigned long long* cnt = f->pass_counters.as<unsigned long long>();
         SR_CUDA(ctx, cudaMemsetAsync(cnt, 0, PASS_CNT_WORDS * sizeof(uint64_t), ctx->stream));
         unsigned long long* sel_count = cnt + PASS_CNT_SEL; // [k]: entries of the selection vector after k gather passes
-        const int sgrid = (int)std::min<int64_t>(f->stream_grid, (n + srd::STREAM_TILE - 1) / srd::STREAM_TILE);
+        const int sgrid = (int)std::min<int64_t>(f->stream_grid, (n + srd::FRAG_TILE - 1) / srd::FRAG_TILE);
         // pass boundaries are bracketed with CUDA events (bench.py reads them back as per-kernel durations)
         if (!f->ev[0])
             for (int e = 0; e < 4; e++) SR_CUDA(ctx, cudaEventCreate(&f->ev[e]));
@@ -764,13 +764,13 @@ static int32_t frag_push(sr_fragment* f, const sr_chunk_view* fact) {
         }
         if (tests) {
             if (carry)
-                srd::k_frag_stream_tests<true><<<sgrid, srd::STREAM_BLOCK, f->stream_smem, ctx->stream>>>(fdev, pass, vt, n, f->sel[0].as<srd::SelEntry>(), sel_count);
+                srd::k_frag_stream_tests<true><<<sgrid, srd::FRAG_BLOCK, f->stream_smem, ctx->stream>>>(fdev, pass, vt, n, f->sel[0].as<srd::SelEntry>(), sel_count);
             else
-                srd::k_frag_stream_tests<false><<<sgrid, srd::STREAM_BLOCK, f->stream_smem, ctx->stream>>>(fdev, pass, vt, n, f->sel[0].as<srd::SelEntry>(), sel_count);
+                srd::k_frag_stream_tests<false><<<sgrid, srd::FRAG_BLOCK, f->stream_smem, ctx->stream>>>(fdev, pass, vt, n, f->sel[0].as<srd::SelEntry>(), sel_count);
         } else if (carry) {
-            srd::k_frag_stream<true><<<sgrid, srd::STREAM_BLOCK, f->stream_smem, ctx->stream>>>(fdev, pass, vt, n, f->sel[0].as<srd::SelEntry>(), sel_count);
+            srd::k_frag_stream<true><<<sgrid, srd::FRAG_BLOCK, f->stream_smem, ctx->stream>>>(fdev, pass, vt, n, f->sel[0].as<srd::SelEntry>(), sel_count);
         } else {
-            srd::k_frag_stream<false><<<sgrid, srd::STREAM_BLOCK, f->stream_smem, ctx->stream>>>(fdev, pass, vt, n, f->sel[0].as<srd::SelEntry>(), sel_count);
+            srd::k_frag_stream<false><<<sgrid, srd::FRAG_BLOCK, f->stream_smem, ctx->stream>>>(fdev, pass, vt, n, f->sel[0].as<srd::SelEntry>(), sel_count);
         }
         SR_LAUNCH_CHECK(ctx);
         SR_CUDA(ctx, cudaEventRecord(f->ev[1], ctx->stream));

@@ -70,11 +70,25 @@ __device__ __forceinline__ void smem_stage_bitmaps(uint32_t* smem, const FragJoi
     }
 }
 
+// the tile shape of the cascade (k_fragment) and of the streaming passes (k_frag_stream, k_frag_stream_tests)
 constexpr int FRAG_BLOCK = 512;
 constexpr int FRAG_WARPS = FRAG_BLOCK / 32;
 constexpr int FRAG_ROWS = 4;   // consecutive rows per thread and group (one 128-bit load of an int32 column)
 constexpr int FRAG_GROUPS = 2; // independent groups per thread and tile (memory-level parallelism)
 constexpr int FRAG_TILE = FRAG_BLOCK * FRAG_ROWS * FRAG_GROUPS;
+
+// the first row of each of the calling thread's groups in `tile`, and which of their rows lie below n
+__device__ __forceinline__ void frag_tile_rows(int64_t tile, int64_t n, int64_t (&row0)[FRAG_GROUPS], uint32_t (&alive)[FRAG_GROUPS]) {
+#pragma unroll
+    for (int g = 0; g < FRAG_GROUPS; g++) {
+        row0[g] = tile * FRAG_TILE + (int64_t)g * (FRAG_BLOCK * FRAG_ROWS) + (int64_t)threadIdx.x * FRAG_ROWS;
+        alive[g] = 0;
+#pragma unroll
+        for (int r = 0; r < FRAG_ROWS; r++)
+            if (row0[g] + r < n) alive[g] |= 1u << r;
+    }
+}
+
 constexpr int FRAG_QCAP = 64; // queue capacity per warp and stage: < 32 pending + <= 32 appended
 // dynamic shared memory per warp for the cascade: SR_MAX_FRAG_JOINS row queues, the key lane of
 // queue 0, and the fill counts
@@ -145,24 +159,68 @@ __device__ __forceinline__ void load_rows4(const VDesc& d, int64_t row0, uint32_
     }
 }
 
+// whether a build row has the (non-NULL) key: the range-mapped bitmap, or the hash table's first[].  STAGED: the kernel
+// copied the bitmaps with smem_off >= 0 to `smem` (smem_stage_bitmaps); otherwise every bitmap is read from global memory
+template <bool STAGED>
 __device__ __forceinline__ bool frag_join_hit(const FragJoinDev& fj, const uint32_t* smem, int64_t key) {
     if (fj.use_bitmap) {
         if (key < fj.j.min_value || key > fj.j.max_value) return false;
         const uint64_t idx = (uint64_t)(key - fj.j.min_value);
-        const uint32_t word = fj.smem_off >= 0 ? smem[fj.smem_off + (idx >> 5)] : __ldg(fj.j.bitmap + (idx >> 5));
+        const uint32_t word = STAGED && fj.smem_off >= 0 ? smem[fj.smem_off + (idx >> 5)] : __ldg(fj.j.bitmap + (idx >> 5));
         return (word >> (idx & 31)) & 1u;
     }
     return join_lookup(fj.j, key) != 0;
 }
 
-// bitmap / hash test against the global copies only (gather passes do not stage bitmaps)
-__device__ __forceinline__ bool join_hit_global(const FragJoinDev& fj, int64_t key) {
-    if (fj.use_bitmap) {
-        if (key < fj.j.min_value || key > fj.j.max_value) return false;
-        const uint64_t idx = (uint64_t)(key - fj.j.min_value);
-        return (__ldg(fj.j.bitmap + (idx >> 5)) >> (idx & 31)) & 1u;
+// whether a row passes filtering or anti join fj: `nul` its key is NULL
+template <bool STAGED>
+__device__ __forceinline__ bool frag_join_row(const FragJoinDev& fj, const uint32_t* smem, int64_t key, bool nul) {
+    return frag_join_pass(fj.kind, nul, !nul && frag_join_hit<STAGED>(fj, smem, key));
+}
+
+// the rows of a 4-row group (`alive` bits, keys `vals`, NULL keys `nullmask`) that pass filtering or anti join fj,
+// tested row by row against the staged bitmaps
+template <typename K>
+__device__ __forceinline__ uint32_t frag_join_group(const FragJoinDev& fj, const uint32_t* smem, const K (&vals)[FRAG_ROWS], uint32_t nullmask, uint32_t alive) {
+    // NULL keys never match (join_hash_table.cpp:166-170): they fail a filtering join and pass an anti join
+    const uint32_t tested = alive & ~nullmask;
+    if (fj.kind != FRAG_ANTI) alive = tested;
+#pragma unroll
+    for (int r = 0; r < FRAG_ROWS; r++)
+        if ((tested & (1u << r)) && !frag_join_pass(fj.kind, false, frag_join_hit<true>(fj, smem, (int64_t)vals[r]))) alive &= ~(1u << r);
+    return alive;
+}
+
+// a tile's filter: the scan conjuncts (ColumnPredicate form, `preds` the shared copies; warp-uniform loop, the loads of
+// both groups first), then the generic boolean conjuncts row by row.  Clears the alive bits of the rows that fail.  vals /
+// nullmask: the caller's load registers, which its join test reuses (separate arrays cost the streaming pass spills)
+__device__ __forceinline__ void frag_tile_filter(const FragDev& fd, const CPred* preds, const VTab& vt, const int64_t (&row0)[FRAG_GROUPS], uint32_t (&alive)[FRAG_GROUPS],
+                                                 int64_t (&vals)[FRAG_GROUPS][FRAG_ROWS], uint32_t (&nullmask)[FRAG_GROUPS]) {
+#pragma unroll 1
+    for (int p = 0; p < fd.num_preds; p++) {
+        const VDesc& d = vt.v[preds[p].value_id];
+#pragma unroll
+        for (int g = 0; g < FRAG_GROUPS; g++) load_rows4(d, row0[g], alive[g], vals[g], nullmask[g]);
+#pragma unroll
+        for (int g = 0; g < FRAG_GROUPS; g++)
+#pragma unroll
+            for (int r = 0; r < FRAG_ROWS; r++)
+                if ((alive[g] & (1u << r)) && !eval_pred(preds[p], vals[g][r], (nullmask[g] >> r) & 1u)) alive[g] &= ~(1u << r);
     }
-    return join_lookup(fj.j, key) != 0;
+#pragma unroll 1
+    for (int e = 0; e < fd.num_exprs; e++) {
+#pragma unroll 1
+        for (int g = 0; g < FRAG_GROUPS; g++)
+#pragma unroll 1
+            for (int r = 0; r < FRAG_ROWS; r++) {
+                if (alive[g] & (1u << r)) {
+                    ChunkLoader ld{vt, row0[g] + r};
+                    int64_t bits;
+                    const bool nul = eval_expr(fd.exprs[e], ld, bits);
+                    if (nul || bits == 0) alive[g] &= ~(1u << r);
+                }
+            }
+    }
 }
 
 // The joins of one row that reached a final pass, in probe order: the filtering and anti joins of [first_test, S) are
@@ -181,16 +239,14 @@ __device__ __forceinline__ bool frag_final_joins(const FragJoinDev* const& joins
         if (!test && !joins[j].need_head) continue;
         int64_t key;
         const bool nul = ld.load(joins[j].key_value_id, key);
-        bool hit = false;
         if (joins[j].need_head || !joins[j].use_bitmap) {
             const uint32_t h = nul ? 0u : join_lookup(joins[j].j, key);
             ld.bidx[j] = h;
             if (head) head[j] = h;
-            hit = h != 0;
-        } else if (test && !nul) {
-            hit = join_hit_global(joins[j], key);
+            if (test && !frag_join_pass(joins[j].kind, nul, h != 0)) ok = false;
+        } else if (!frag_join_row<false>(joins[j], nullptr, key, nul)) {
+            ok = false;
         }
-        if (test && !frag_join_pass(joins[j].kind, nul, hit)) ok = false;
     }
     return ok;
 }
@@ -262,12 +318,12 @@ struct Cascade {
         bool pass = false;
         if (valid) {
             if (k == 0 && eager1) { // the eagerly streamed key column is never nullable
-                pass = frag_join_pass(fj.kind, false, frag_join_hit(fj, smem, (int64_t)carried_key));
+                pass = frag_join_row<true>(fj, smem, (int64_t)carried_key, false);
             } else {
                 const VDesc& d = vt.v[fj.key_value_id];
                 const int64_t key = load_int(d.data, d.type, (int64_t)row32);
                 const bool nul = d.nulls != nullptr && d.nulls[row32] != 0;
-                pass = frag_join_pass(fj.kind, nul, !nul && frag_join_hit(fj, smem, key));
+                pass = frag_join_row<true>(fj, smem, key, nul);
             }
         }
         append(k + 1, row32, pass);
@@ -371,19 +427,11 @@ __global__ void __launch_bounds__(FRAG_BLOCK, 2) k_fragment(const FragDev* __res
         int64_t row0[FRAG_GROUPS];
         uint32_t alive[FRAG_GROUPS];
         int32_t k1v[FRAG_GROUPS][FRAG_ROWS]; // eager second key
-#pragma unroll
-        for (int g = 0; g < FRAG_GROUPS; g++) {
-            row0[g] = tile * FRAG_TILE + (int64_t)g * (FRAG_BLOCK * FRAG_ROWS) + (int64_t)threadIdx.x * FRAG_ROWS;
-            alive[g] = 0;
-#pragma unroll
-            for (int r = 0; r < FRAG_ROWS; r++)
-                if (row0[g] + r < n) alive[g] |= 1u << r;
-        }
+        frag_tile_rows(tile, n, row0, alive);
         const bool streamed = fast0 && tile < full_tiles;
         if (streamed) {
             // keys of this tile were requested one iteration ago: test them, then request the next tile's
             // (the requests stay in flight while this tile's survivors run through the cascade)
-            const FragJoinDev& fj = s_joins[0];
 #pragma unroll
             for (int g = 0; g < FRAG_GROUPS; g++) {
                 const int32_t kv[FRAG_ROWS] = {pk0[g].x, pk0[g].y, pk0[g].z, pk0[g].w};
@@ -391,56 +439,20 @@ __global__ void __launch_bounds__(FRAG_BLOCK, 2) k_fragment(const FragDev* __res
                 k1v[g][1] = pk1[g].y;
                 k1v[g][2] = pk1[g].z;
                 k1v[g][3] = pk1[g].w;
-#pragma unroll
-                for (int r = 0; r < FRAG_ROWS; r++)
-                    if (!frag_join_pass(fj.kind, false, frag_join_hit(fj, smem, (int64_t)kv[r]))) alive[g] &= ~(1u << r);
+                alive[g] = frag_join_group(s_joins[0], smem, kv, 0u, alive[g]);
             }
             prefetch(tile + gridDim.x);
         } else {
             int64_t vals[FRAG_GROUPS][FRAG_ROWS];
             uint32_t nullmask[FRAG_GROUPS];
-            // ---- scan conjuncts (ColumnPredicate form): warp-uniform loop, loads of both groups first ----
-#pragma unroll 1
-            for (int p = 0; p < fd.num_preds; p++) {
-                const VDesc& d = vt.v[s_preds[p].value_id];
-#pragma unroll
-                for (int g = 0; g < FRAG_GROUPS; g++) load_rows4(d, row0[g], alive[g], vals[g], nullmask[g]);
-#pragma unroll
-                for (int g = 0; g < FRAG_GROUPS; g++)
-#pragma unroll
-                    for (int r = 0; r < FRAG_ROWS; r++)
-                        if ((alive[g] & (1u << r)) && !eval_pred(s_preds[p], vals[g][r], (nullmask[g] >> r) & 1u)) alive[g] &= ~(1u << r);
-            }
-            // ---- generic boolean conjuncts ----
-#pragma unroll 1
-            for (int e = 0; e < fd.num_exprs; e++) {
-#pragma unroll 1
-                for (int g = 0; g < FRAG_GROUPS; g++)
-#pragma unroll 1
-                    for (int r = 0; r < FRAG_ROWS; r++) {
-                        if (alive[g] & (1u << r)) {
-                            ChunkLoader ld{vt, row0[g] + r};
-                            int64_t bits;
-                            const bool nul = eval_expr(fd.exprs[e], ld, bits);
-                            if (nul || bits == 0) alive[g] &= ~(1u << r);
-                        }
-                    }
-            }
+            frag_tile_filter(fd, s_preds, vt, row0, alive, vals, nullmask);
             // ---- first join on its key column ----
             if (SF > 0) {
-                const FragJoinDev& fj = s_joins[0];
-                const VDesc& d = vt.v[fj.key_value_id];
+                const VDesc& d = vt.v[s_joins[0].key_value_id];
 #pragma unroll
                 for (int g = 0; g < FRAG_GROUPS; g++) load_rows4(d, row0[g], alive[g], vals[g], nullmask[g]);
 #pragma unroll
-                for (int g = 0; g < FRAG_GROUPS; g++) {
-                    // NULL keys never match (join_hash_table.cpp:166-170): they fail a filtering join and pass an anti join
-                    const uint32_t tested = alive[g] & ~nullmask[g];
-                    if (fj.kind != FRAG_ANTI) alive[g] = tested;
-#pragma unroll
-                    for (int r = 0; r < FRAG_ROWS; r++)
-                        if ((tested & (1u << r)) && !frag_join_pass(fj.kind, false, frag_join_hit(fj, smem, vals[g][r]))) alive[g] &= ~(1u << r);
-                }
+                for (int g = 0; g < FRAG_GROUPS; g++) alive[g] = frag_join_group(s_joins[0], smem, vals[g], nullmask[g], alive[g]);
                 if (fast1) { // tail tile of a streamed run: the consumer of queue 0 expects the key to ride along
 #pragma unroll
                     for (int g = 0; g < FRAG_GROUPS; g++)
@@ -514,8 +526,7 @@ __global__ void __launch_bounds__(256) k_frag_sample(const FragDev* __restrict__
             const FragJoinDev& fj = fd.joins[j];
             int64_t key;
             const bool nul = ld.load(fj.key_value_id, key);
-            const bool hit = !nul && join_lookup(fj.j, key) != 0;
-            const bool pass = fj.kind == FRAG_OUTER || frag_join_pass(fj.kind, nul, hit);
+            const bool pass = fj.kind == FRAG_OUTER || frag_join_row<false>(fj, nullptr, key, nul);
             const uint32_t m = __ballot_sync(__activemask(), pass);
             if (pass && (m & lanemask_lt()) == 0) atomicAdd(&counts[j], (unsigned long long)__popc(m));
         }

@@ -165,10 +165,6 @@ __device__ __forceinline__ uint32_t join_test_batch(const FragJoinDev& fj, const
     return out;
 }
 
-constexpr int STREAM_BLOCK = 512;
-constexpr int STREAM_ROWS = 4;
-constexpr int STREAM_GROUPS = 2;
-constexpr int STREAM_TILE = STREAM_BLOCK * STREAM_ROWS * STREAM_GROUPS;
 constexpr int STREAM_MAX_JOINS = 2;
 
 // Selection vectors are written through a per-warp chunk allocator: a warp takes SEL_CHUNK entries at a
@@ -216,12 +212,12 @@ __device__ __forceinline__ void warp_append_rows(uint32_t alive_all, int64_t row
     if (total == 0) return;
     SelEntry* __restrict__ sel_out = w.out + (w.reserve(total) + incl - cnt);
     // few rows survive (a lane holds 0..2 of its 8): walk the set bits instead of testing all eight
-    const uint32_t r0 = (uint32_t)row0_g0, r1 = (uint32_t)row0_g1 - STREAM_ROWS;
+    const uint32_t r0 = (uint32_t)row0_g0, r1 = (uint32_t)row0_g1 - FRAG_ROWS;
     uint32_t m = alive_all, pos = 0;
     while (m) {
         const uint32_t i = (uint32_t)__ffs((int)m) - 1u;
         m &= m - 1u;
-        const uint32_t row = (i < STREAM_ROWS ? r0 : r1) + i;
+        const uint32_t row = (i < FRAG_ROWS ? r0 : r1) + i;
         sel_out[pos++] = CARRY ? sel_make(row, key_at(i)) : (SelEntry)row;
     }
 }
@@ -231,8 +227,8 @@ __device__ __forceinline__ void warp_append_rows(uint32_t alive_all, int64_t row
 // sector from pinned host memory).  (Re-reading the key for the survivors in this pass instead puts an L2 round trip
 // on every tile's critical path.)
 template <bool CARRY>
-__global__ void __launch_bounds__(STREAM_BLOCK, 2) k_frag_stream(const FragDev* __restrict__ fdp, PassDev pd, const __grid_constant__ VTab vt, int64_t n,
-                                                                 SelEntry* __restrict__ sel_out, unsigned long long* __restrict__ counter) {
+__global__ void __launch_bounds__(FRAG_BLOCK, 2) k_frag_stream(const FragDev* __restrict__ fdp, PassDev pd, const __grid_constant__ VTab vt, int64_t n,
+                                                               SelEntry* __restrict__ sel_out, unsigned long long* __restrict__ counter) {
     extern __shared__ __align__(16) uint32_t smem[];
     __shared__ FragJoinDev s_joins[STREAM_MAX_JOINS];
     __shared__ CPred s_preds[8];
@@ -245,8 +241,8 @@ __global__ void __launch_bounds__(STREAM_BLOCK, 2) k_frag_stream(const FragDev* 
 
     // (the common shapes -- range conjuncts and joins on plain int32 columns -- run in k_frag_stream_tests below;
     // this kernel is the general form: any predicate, generic filter expressions, nullable / wide key columns)
-    const int64_t num_tiles = (n + STREAM_TILE - 1) / STREAM_TILE;
-    const int64_t full_tiles = n / STREAM_TILE;
+    const int64_t num_tiles = (n + FRAG_TILE - 1) / FRAG_TILE;
+    const int64_t full_tiles = n / FRAG_TILE;
     // Each CTA streams a CONTIGUOUS run of tiles (not a grid-stride walk): the rows a warp appends to one
     // selection-vector chunk then come from a narrow band of the table (~25 tiles) instead of being spread over
     // the whole batch, so the later gather passes touch neighbouring sectors / pages back to back.
@@ -257,86 +253,44 @@ __global__ void __launch_bounds__(STREAM_BLOCK, 2) k_frag_stream(const FragDev* 
     writer.init(sel_out, counter);
 
     for (int64_t tile = tile_begin; tile < tile_end; tile++) {
-        int64_t row0[STREAM_GROUPS];
-        uint32_t alive[STREAM_GROUPS];
+        int64_t row0[FRAG_GROUPS];
+        uint32_t alive[FRAG_GROUPS];
 #pragma unroll
-        for (int g = 0; g < STREAM_GROUPS; g++) {
-            row0[g] = tile * STREAM_TILE + (int64_t)g * (STREAM_BLOCK * STREAM_ROWS) + (int64_t)threadIdx.x * STREAM_ROWS;
+        for (int g = 0; g < FRAG_GROUPS; g++) {
+            row0[g] = tile * FRAG_TILE + (int64_t)g * (FRAG_BLOCK * FRAG_ROWS) + (int64_t)threadIdx.x * FRAG_ROWS;
             alive[g] = 0xFu;
         }
-        if (tile >= full_tiles) { // only the last tile can be ragged
-#pragma unroll
-            for (int g = 0; g < STREAM_GROUPS; g++) {
-                alive[g] = 0;
-#pragma unroll
-                for (int r = 0; r < STREAM_ROWS; r++)
-                    if (row0[g] + r < n) alive[g] |= 1u << r;
-            }
-        }
-        int32_t carry[STREAM_GROUPS * STREAM_ROWS];
+        if (tile >= full_tiles) frag_tile_rows(tile, n, row0, alive); // only the last tile can be ragged
+        int32_t carry[FRAG_GROUPS * FRAG_ROWS];
         if (CARRY) {
 #pragma unroll
-            for (int i = 0; i < STREAM_GROUPS * STREAM_ROWS; i++) carry[i] = 0;
+            for (int i = 0; i < FRAG_GROUPS * FRAG_ROWS; i++) carry[i] = 0;
         }
-        {
-            int64_t vals[STREAM_GROUPS][STREAM_ROWS];
-            uint32_t nullmask[STREAM_GROUPS];
+        int64_t vals[FRAG_GROUPS][FRAG_ROWS];
+        uint32_t nullmask[FRAG_GROUPS];
+        frag_tile_filter(fd, s_preds, vt, row0, alive, vals, nullmask);
 #pragma unroll 1
-            for (int p = 0; p < fd.num_preds; p++) {
-                const VDesc& d = vt.v[s_preds[p].value_id];
+        for (int j = 0; j < SJ; j++) {
+            const VDesc& d = vt.v[s_joins[j].key_value_id];
 #pragma unroll
-                for (int g = 0; g < STREAM_GROUPS; g++) load_rows4(d, row0[g], alive[g], vals[g], nullmask[g]);
+            for (int g = 0; g < FRAG_GROUPS; g++) load_rows4(d, row0[g], alive[g], vals[g], nullmask[g]);
 #pragma unroll
-                for (int g = 0; g < STREAM_GROUPS; g++)
+            for (int g = 0; g < FRAG_GROUPS; g++) alive[g] = frag_join_group(s_joins[j], smem, vals[g], nullmask[g], alive[g]);
+            if (CARRY && j == pd.carry_join) {
 #pragma unroll
-                    for (int r = 0; r < STREAM_ROWS; r++)
-                        if ((alive[g] & (1u << r)) && !eval_pred(s_preds[p], vals[g][r], (nullmask[g] >> r) & 1u)) alive[g] &= ~(1u << r);
-            }
-#pragma unroll 1
-            for (int e = 0; e < fd.num_exprs; e++) {
-#pragma unroll 1
-                for (int g = 0; g < STREAM_GROUPS; g++)
-#pragma unroll 1
-                    for (int r = 0; r < STREAM_ROWS; r++) {
-                        if (alive[g] & (1u << r)) {
-                            ChunkLoader ld{vt, row0[g] + r};
-                            int64_t bits;
-                            const bool nul = eval_expr(fd.exprs[e], ld, bits);
-                            if (nul || bits == 0) alive[g] &= ~(1u << r);
-                        }
-                    }
-            }
-#pragma unroll 1
-            for (int j = 0; j < SJ; j++) {
-                const VDesc& d = vt.v[s_joins[j].key_value_id];
+                for (int g = 0; g < FRAG_GROUPS; g++)
 #pragma unroll
-                for (int g = 0; g < STREAM_GROUPS; g++) load_rows4(d, row0[g], alive[g], vals[g], nullmask[g]);
-#pragma unroll
-                for (int g = 0; g < STREAM_GROUPS; g++) {
-                    // NULL keys never match (join_hash_table.cpp:166-170): they fail a filtering join and pass an anti join
-                    const uint32_t tested = alive[g] & ~nullmask[g];
-                    if (s_joins[j].kind != FRAG_ANTI) alive[g] = tested;
-#pragma unroll
-                    for (int r = 0; r < STREAM_ROWS; r++)
-                        if ((tested & (1u << r)) && !frag_join_pass(s_joins[j].kind, false, frag_join_hit(s_joins[j], smem, vals[g][r])))
-                            alive[g] &= ~(1u << r);
-                }
-                if (CARRY && j == pd.carry_join) {
-#pragma unroll
-                    for (int g = 0; g < STREAM_GROUPS; g++)
-#pragma unroll
-                        for (int r = 0; r < STREAM_ROWS; r++) carry[g * STREAM_ROWS + r] = (int32_t)vals[g][r];
-                }
+                    for (int r = 0; r < FRAG_ROWS; r++) carry[g * FRAG_ROWS + r] = (int32_t)vals[g][r];
             }
         }
-        static_assert(STREAM_GROUPS == 2, "two groups of alive bits are packed into one word");
+        static_assert(FRAG_GROUPS == 2, "two groups of alive bits are packed into one word");
         auto key_at = [&](uint32_t i) { // a select chain: indexing the register array with i would put it in local memory
             int32_t v = carry[0];
 #pragma unroll
-            for (int k = 1; k < STREAM_GROUPS * STREAM_ROWS; k++) v = i == (uint32_t)k ? carry[k] : v;
+            for (int k = 1; k < FRAG_GROUPS * FRAG_ROWS; k++) v = i == (uint32_t)k ? carry[k] : v;
             return v;
         };
-        warp_append_rows<CARRY>(alive[0] | (alive[1] << STREAM_ROWS), row0[0], row0[1], key_at, writer);
+        warp_append_rows<CARRY>(alive[0] | (alive[1] << FRAG_ROWS), row0[0], row0[1], key_at, writer);
     }
     writer.finish();
 }
@@ -404,12 +358,12 @@ __device__ __forceinline__ uint32_t stream_test_reg(const VecTest& t, const uint
 // spilled: the spill stores of the prefetched vectors then waited on their loads on every tile.  Two 128-bit shared stores
 // per tile instead, and a shared load per surviving row.
 template <bool CARRY>
-__global__ void __launch_bounds__(STREAM_BLOCK, 2) k_frag_stream_tests(const FragDev* __restrict__ fdp, const __grid_constant__ PassDev pd, const __grid_constant__ VTab vt, int64_t n,
-                                                                       SelEntry* __restrict__ sel_out, unsigned long long* __restrict__ counter) {
+__global__ void __launch_bounds__(FRAG_BLOCK, 2) k_frag_stream_tests(const FragDev* __restrict__ fdp, const __grid_constant__ PassDev pd, const __grid_constant__ VTab vt, int64_t n,
+                                                                     SelEntry* __restrict__ sel_out, unsigned long long* __restrict__ counter) {
     extern __shared__ __align__(16) uint32_t smem[];
     __shared__ FragJoinDev s_joins[STREAM_MAX_JOINS];
     __shared__ StreamTest s_tests[SR_MAX_STREAM_TESTS];
-    __shared__ int4 s_carry[CARRY ? STREAM_GROUPS * STREAM_BLOCK : 1]; // [group][thread]: the keys of the thread's 4 rows
+    __shared__ int4 s_carry[CARRY ? FRAG_GROUPS * FRAG_BLOCK : 1]; // [group][thread]: the keys of the thread's 4 rows
     const FragDev& fd = *fdp;
     const int SJ = pd.num_stream_joins;
     const int NT = pd.num_tests;
@@ -426,22 +380,22 @@ __global__ void __launch_bounds__(STREAM_BLOCK, 2) k_frag_stream_tests(const Fra
     const bool carry1 = CARRY && NV > 1 && s_tests[1].kind == 1 && s_tests[1].join == pd.carry_join;
     const int32_t* col0 = (const int32_t*)vt.v[pd.tests[0].value_id].data;
     const int32_t* col1 = NV > 1 ? (const int32_t*)vt.v[pd.tests[1].value_id].data : nullptr;
-    const int64_t num_tiles = (n + STREAM_TILE - 1) / STREAM_TILE;
-    const int64_t full_tiles = n / STREAM_TILE;
+    const int64_t num_tiles = (n + FRAG_TILE - 1) / FRAG_TILE;
+    const int64_t full_tiles = n / FRAG_TILE;
     const int64_t tiles_per_cta = (num_tiles + gridDim.x - 1) / gridDim.x;
     const int64_t tile_begin = (int64_t)blockIdx.x * tiles_per_cta;
     const int64_t tile_end = tile_begin + tiles_per_cta < num_tiles ? tile_begin + tiles_per_cta : num_tiles;
     const int64_t prefetch_end = tile_end < full_tiles ? tile_end : full_tiles;
-    int4 pk[2][STREAM_GROUPS];
+    int4 pk[2][FRAG_GROUPS];
 #pragma unroll
     for (int j = 0; j < 2; j++)
 #pragma unroll
-        for (int g = 0; g < STREAM_GROUPS; g++) pk[j][g] = make_int4(0, 0, 0, 0);
+        for (int g = 0; g < FRAG_GROUPS; g++) pk[j][g] = make_int4(0, 0, 0, 0);
     auto prefetch = [&](int64_t tile) {
         if (tile < prefetch_end) {
 #pragma unroll
-            for (int g = 0; g < STREAM_GROUPS; g++) {
-                const int64_t r0 = tile * STREAM_TILE + (int64_t)g * (STREAM_BLOCK * STREAM_ROWS) + (int64_t)threadIdx.x * STREAM_ROWS;
+            for (int g = 0; g < FRAG_GROUPS; g++) {
+                const int64_t r0 = tile * FRAG_TILE + (int64_t)g * (FRAG_BLOCK * FRAG_ROWS) + (int64_t)threadIdx.x * FRAG_ROWS;
                 pk[0][g] = ldg_stream_v4(col0 + r0);
                 if (col1) pk[1][g] = ldg_stream_v4(col1 + r0);
             }
@@ -450,19 +404,19 @@ __global__ void __launch_bounds__(STREAM_BLOCK, 2) k_frag_stream_tests(const Fra
     prefetch(tile_begin);
     WarpSelWriter writer;
     writer.init(sel_out, counter);
-    static_assert(STREAM_GROUPS == 2 && STREAM_ROWS == 4, "8 rows per thread and tile");
+    static_assert(FRAG_GROUPS == 2 && FRAG_ROWS == 4, "8 rows per thread and tile");
     for (int64_t tile = tile_begin; tile < tile_end; tile++) {
-        int64_t row0[STREAM_GROUPS];
+        int64_t row0[FRAG_GROUPS];
 #pragma unroll
-        for (int g = 0; g < STREAM_GROUPS; g++)
-            row0[g] = tile * STREAM_TILE + (int64_t)g * (STREAM_BLOCK * STREAM_ROWS) + (int64_t)threadIdx.x * STREAM_ROWS;
+        for (int g = 0; g < FRAG_GROUPS; g++)
+            row0[g] = tile * FRAG_TILE + (int64_t)g * (FRAG_BLOCK * FRAG_ROWS) + (int64_t)threadIdx.x * FRAG_ROWS;
         uint32_t a8 = 0xFFu;
         int first_pred = 0; // tests [first_pred, NT) load their column for the live rows only
         if (tile < full_tiles) {
 #pragma unroll
-            for (int g = 0; g < STREAM_GROUPS; g++) {
-                if (carry0) s_carry[g * STREAM_BLOCK + threadIdx.x] = pk[0][g];
-                if (carry1) s_carry[g * STREAM_BLOCK + threadIdx.x] = pk[1][g];
+            for (int g = 0; g < FRAG_GROUPS; g++) {
+                if (carry0) s_carry[g * FRAG_BLOCK + threadIdx.x] = pk[0][g];
+                if (carry1) s_carry[g * FRAG_BLOCK + threadIdx.x] = pk[1][g];
             }
             const int32_t k0[8] = {pk[0][0].x, pk[0][0].y, pk[0][0].z, pk[0][0].w, pk[0][1].x, pk[0][1].y, pk[0][1].z, pk[0][1].w};
             const int32_t k1[8] = {pk[1][0].x, pk[1][0].y, pk[1][0].z, pk[1][0].w, pk[1][1].x, pk[1][1].y, pk[1][1].z, pk[1][1].w};
@@ -486,11 +440,11 @@ __global__ void __launch_bounds__(STREAM_BLOCK, 2) k_frag_stream_tests(const Fra
             a8 = stream_test<8>(st, s_joins, smem, kk, a8);
             if (CARRY && st.kind == 1 && st.join == pd.carry_join) {
 #pragma unroll
-                for (int g = 0; g < STREAM_GROUPS; g++) s_carry[g * STREAM_BLOCK + threadIdx.x] = make_int4(kk[4 * g], kk[4 * g + 1], kk[4 * g + 2], kk[4 * g + 3]);
+                for (int g = 0; g < FRAG_GROUPS; g++) s_carry[g * FRAG_BLOCK + threadIdx.x] = make_int4(kk[4 * g], kk[4 * g + 1], kk[4 * g + 2], kk[4 * g + 3]);
             }
         }
-        const int32_t* stash = (const int32_t*)s_carry + STREAM_ROWS * threadIdx.x;
-        warp_append_rows<CARRY>(a8, row0[0], row0[1], [&](uint32_t i) { return stash[(i >> 2) * (STREAM_ROWS * STREAM_BLOCK) + (i & 3)]; }, writer);
+        const int32_t* stash = (const int32_t*)s_carry + FRAG_ROWS * threadIdx.x;
+        warp_append_rows<CARRY>(a8, row0[0], row0[1], [&](uint32_t i) { return stash[(i >> 2) * (FRAG_ROWS * FRAG_BLOCK) + (i & 3)]; }, writer);
     }
     writer.finish();
 }
@@ -537,7 +491,7 @@ __global__ void __launch_bounds__(GATHER_BLOCK) k_frag_gather_join(const FragDev
             // directories resident changed neither pass on H100: 0.569 / 0.752 ms against 0.569 / 0.748 ms)
             const int64_t key = load_int(d.data, d.type, (int64_t)row);
             const bool nul = d.nulls != nullptr && d.nulls[row] != 0;
-            hit = frag_join_pass(fj.kind, nul, !nul && join_hit_global(fj, key)); // global bitmap copy: L1/L2 resident
+            hit = frag_join_row<false>(fj, nullptr, key, nul); // global bitmap copy: L1/L2 resident
         }
         const uint32_t m = __ballot_sync(SR_FULL_MASK, hit);
         if (m) {

@@ -1309,7 +1309,7 @@ int32_t sr_fragment_get_plan(sr_fragment* frag, sr_fragment_plan* plan) {
     if (frag->selective) {
         plan->smem_bytes = (int32_t)frag->stream_smem;
         plan->grid = frag->stream_grid;
-        plan->block = srd::STREAM_BLOCK;
+        plan->block = srd::FRAG_BLOCK;
     } else {
         plan->smem_bytes = (int32_t)frag->cascade_smem;
         plan->grid = frag->cascade_grid;
