@@ -66,7 +66,8 @@ struct sr_fragment {
     int cascade_grid = 0;
     // selective mode (sr_frag_pass.cuh): streaming pass -> gather passes -> final pass, planned by frag_plan_passes
     bool selective = false;
-    bool expand = false; // some INNER / LEFT OUTER join has duplicate build keys: selection-vector passes + k_frag_gather_agg<false, SINGLE, true>
+    bool expand = false; // some INNER / LEFT OUTER join has duplicate build keys: selection-vector passes + k_frag_gather_agg<false, SINGLE, true, CONJ>
+    bool conj = false;   // some INNER / LEFT SEMI join has an other-join conjunct: selection-vector passes + k_frag_gather_agg<..., true>
     srd::PassDev pass;
     std::vector<int> gather_joins; // probe positions that get a pass of their own
     DevBuf sel[2], pass_counters;
@@ -90,6 +91,8 @@ struct sr_fragment {
     // the type sr_join_desc.build_out_types declares over a zeroed row 0, which every probe row reads as NULL
     // (FragLoader::load) -- what sr_join_probe pads a LEFT OUTER join's rows with
     BuildCol empty_payload[SR_MAX_FRAG_JOINS][SR_MAX_FRAG_PAYLOAD];
+    // the same for the build columns an other-join conjunct reads (never evaluated: such an INNER / SEMI join passes nothing)
+    std::vector<std::unique_ptr<BuildCol>> empty_conj[SR_MAX_FRAG_JOINS];
     ~sr_fragment() {
         for (int e = 0; e < 4; e++)
             if (ev[e]) cudaEventDestroy(ev[e]);
@@ -100,18 +103,45 @@ struct FragTypeCtx {
     sr_fragment* f;
 };
 
-// the first join (hint order) that carries `slot` as a payload, and its build column; join = -1 when none does
+// the slots expression `e` reads, appended to `slots`
+static void expr_slots(const sr_expr& e, std::vector<int32_t>* slots) {
+    for (int k = 0; k < std::min<int32_t>(e.num_nodes, SR_MAX_EXPR_NODES); k++)
+        if (e.nodes[k].op == SR_EX_COL) slots->push_back(e.nodes[k].slot_id);
+}
+static bool expr_reads(const sr_expr& e, int32_t slot) {
+    std::vector<int32_t> s;
+    expr_slots(e, &s);
+    return std::find(s.begin(), s.end(), slot) != s.end();
+}
+// the slots an aggregate reads: group keys and function inputs
+static void frag_agg_slots(const sr_agg_desc& d, std::vector<int32_t>* slots) {
+    slots->clear();
+    for (int k = 0; k < std::min<int32_t>(d.num_group_keys, SR_MAX_GROUP_KEYS); k++) slots->push_back(d.group_slots[k]);
+    for (int q = 0; q < std::min<int32_t>(d.num_fns, SR_MAX_AGG_FNS); q++) {
+        if (d.fns[q].kind != SR_AGG_COUNT_STAR) expr_slots(d.fns[q].input, slots);
+        if (d.fns[q].kind == SR_AGG_AVG_MERGE) slots->push_back(d.fns[q].reserved);
+    }
+}
+
+// the first join (hint order) that carries `slot` as a payload, else the first whose other-join conjunct reads `slot` as
+// one of its build columns (unless payload_only), and that build column; join = -1 when none does
 struct FragPayload {
     const BuildCol* col;
     int join;
 };
-static FragPayload frag_find_payload(const sr_fragment* f, int32_t slot) {
+static FragPayload frag_find_payload(const sr_fragment* f, int32_t slot, bool payload_only = false) {
     for (int j = 0; j < f->num_joins; j++)
         for (int p = 0; p < f->joins[j].num_payload; p++)
             if (f->joins[j].payload_build_slots[p] == slot) {
                 const BuildCol* bc = f->joins[j].join->find_col(slot);
                 return FragPayload{bc ? bc : &f->empty_payload[j][p], j}; // sr_fragment_create filled the latter
             }
+    for (int j = 0; j < f->num_joins && !payload_only; j++) {
+        if (!expr_reads(f->joins[j].join->desc.other_conjunct, slot)) continue;
+        if (const BuildCol* bc = f->joins[j].join->find_col(slot)) return FragPayload{bc, j};
+        for (const auto& bc : f->empty_conj[j])
+            if (bc->slot == slot) return FragPayload{bc.get(), j};
+    }
     return FragPayload{nullptr, -1};
 }
 
@@ -218,7 +248,44 @@ static int32_t frag_compile(sr_fragment* f) {
         f->order[j] = j;
         if (h.joins[j].kind != srd::FRAG_OUTER) h.num_filter_joins++;
     }
-    // aggregate (its expressions may reference fact slots and payload slots)
+    // other-join conjuncts (INNER / LEFT SEMI, sr_fragment_create): each reads fact columns and its own join's build
+    // columns, the fact chunk first as sr_join_probe resolves them.  The final pass evaluates them at the join's build rows
+    for (int j = 0; j < f->num_joins; j++) {
+        const sr_expr& e = f->joins[j].join->desc.other_conjunct;
+        if (e.num_nodes <= 0) continue;
+        for (int k = 0; k < std::min<int32_t>(e.num_nodes, SR_MAX_EXPR_NODES); k++) {
+            const int32_t slot = e.nodes[k].slot_id;
+            if (e.nodes[k].op != SR_EX_COL || f->staged.find(slot) >= 0) continue;
+            // one slot id names one value of the fragment: a slot another join carries (a payload, a column its conjunct
+            // reads, or any column of its build chunks) is that join's, even when this join's build side has one too
+            const FragPayload pl = frag_find_payload(f, slot);
+            int other = pl.join;
+            for (int q = 0; q < f->num_joins && other < 0; q++)
+                if (q != j && f->joins[q].join->find_col(slot)) other = q;
+            if (other >= 0 && other != j)
+                return sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "other-join conjunct of join %d reads slot %d, a column of join %d: a conjunct reads fact columns and its own join's build columns",
+                               j, slot, other);
+            if (pl.join < 0) {
+                if (f->joins[j].join->cols.empty())
+                    return sr_fail(ctx, SR_ERR_STATE, "fragment join %d: build side is empty and the type of conjunct slot %d is unknown: declare it in sr_join_desc.build_out_types",
+                                   j, slot);
+                return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "other-join conjunct of join %d: slot %d is in neither the fact chunk nor the build chunk", j, slot);
+            }
+        }
+        SR_TRY(compile_expr(ctx, &e, &f->reg, frag_slot_type, &tc, &h.conj[j]));
+        if (h.conj[j].result_is_double) return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "other-join conjunct of join %d is not boolean", j);
+        h.conj_mask |= 1 << j;
+        h.joins[j].need_head = 1;
+    }
+    // aggregate (its expressions may reference fact slots and payload slots: a build column only a conjunct reads is not
+    // part of the join's output)
+    {
+        std::vector<int32_t> read;
+        frag_agg_slots(f->agg->desc, &read);
+        for (const int32_t slot : read)
+            if (f->staged.find(slot) < 0 && frag_find_payload(f, slot).join >= 0 && frag_find_payload(f, slot, true).join < 0)
+                return sr_fail(ctx, SR_ERR_INVALID_ARGUMENT, "slot %d is neither a fact column nor a join payload", slot);
+    }
     SR_TRY(agg_compile(f->agg, frag_slot_type, frag_slot_nullable, &tc));
     // the fragment and its aggregate share one value table: rebuild the aggregate's value ids on top
     // of the fragment registry
@@ -277,7 +344,7 @@ static int32_t frag_plan_final_dense(sr_fragment* f) {
     srd::FinalDense& fp = f->final_dense;
     memset(&fp, 0, sizeof(fp));
     f->final_dense_ok = false;
-    if (f->expand || !f->smem_agg || !ah.dense || ah.num_keys == 0 || ah.cap >= SR_DIGIT_BAD) return SR_OK;
+    if (f->expand || f->conj || !f->smem_agg || !ah.dense || ah.num_keys == 0 || ah.cap >= SR_DIGIT_BAD) return SR_OK;
     const int nv = f->pass.num_final_vals;
     if (nv > srd::FINAL_MAX_VALS) return SR_OK;
     auto val_of = [&](int id) {
@@ -505,20 +572,25 @@ static void frag_plan_stream_tests(sr_fragment* f, double reach_pred0) {
     }
 }
 
-// fact values the final pass reads: keys of the joins it looks up or tests, group keys, aggregate inputs
+// fact values the final pass reads: keys of the joins it looks up or tests, other-join conjunct inputs, group keys,
+// aggregate inputs
 static void frag_plan_final_vals(sr_fragment* f) {
     const srd::FragDev& h = f->host;
     std::vector<int> need;
     auto want = [&](int id) {
         if (id >= 0 && id < (int)f->value_src.size() && f->value_src[id] < 0 && std::find(need.begin(), need.end(), id) == need.end()) need.push_back(id);
     };
-    for (int q = 0; q < f->num_joins; q++)
+    auto want_expr = [&](const srd::CExpr& e) {
+        for (int k = 0; k < e.num_nodes; k++)
+            if (e.nodes[k].op == srd::C_LOAD_I || e.nodes[k].op == srd::C_LOAD_D) want(e.nodes[k].arg);
+    };
+    for (int q = 0; q < f->num_joins; q++) {
         if (h.joins[q].need_head || frag_final_tests(f, q)) want(h.joins[q].key_value_id);
+        if ((h.conj_mask >> q) & 1) want_expr(h.conj[q]);
+    }
     const srd::AggDev& ah = f->agg->host;
     for (int k = 0; k < ah.num_keys; k++) want(ah.key_value_id[k]);
-    for (int q = 0; q < ah.num_fns; q++)
-        for (int k = 0; k < ah.fns[q].input.num_nodes; k++)
-            if (ah.fns[q].input.nodes[k].op == srd::C_LOAD_I || ah.fns[q].input.nodes[k].op == srd::C_LOAD_D) want(ah.fns[q].input.nodes[k].arg);
+    for (int q = 0; q < ah.num_fns; q++) want_expr(ah.fns[q].input);
     for (int k = 0; k < SR_FINAL_PREFETCH; k++) f->pass.final_vals[k] = k < (int)need.size() ? (int8_t)need[k] : (int8_t)-1;
     f->pass.num_final_vals = (int8_t)std::min<size_t>(need.size(), 127);
 }
@@ -529,12 +601,16 @@ struct FinalKernel {
                unsigned long long*);
     size_t smem;
 };
-static FinalKernel frag_final_kernel(const sr_fragment* f) {
+template <bool CONJ>
+static FinalKernel frag_final_kernel_of(const sr_fragment* f) {
     const bool single = f->agg->host.num_keys == 0;
-    if (f->expand) return {single ? srd::k_frag_gather_agg<false, true, true> : srd::k_frag_gather_agg<false, false, true>, 0};
-    if (single) return {srd::k_frag_gather_agg<false, true, false>, 0};
-    if (f->smem_agg) return {srd::k_frag_gather_agg<true, false, false>, f->agg->smem_bytes};
-    return {srd::k_frag_gather_agg<false, false, false>, 0};
+    if (f->expand) return {single ? srd::k_frag_gather_agg<false, true, true, CONJ> : srd::k_frag_gather_agg<false, false, true, CONJ>, 0};
+    if (single) return {srd::k_frag_gather_agg<false, true, false, CONJ>, 0};
+    if (f->smem_agg) return {srd::k_frag_gather_agg<true, false, false, CONJ>, f->agg->smem_bytes};
+    return {srd::k_frag_gather_agg<false, false, false, CONJ>, 0};
+}
+static FinalKernel frag_final_kernel(const sr_fragment* f) {
+    return f->conj ? frag_final_kernel_of<true>(f) : frag_final_kernel_of<false>(f);
 }
 
 // launch grids of the passes (and the dynamic shared-memory limit of the streaming kernels)
@@ -644,13 +720,21 @@ static int32_t frag_plan(sr_fragment* f, const VTab& vt, int64_t n) {
     // outer joins filter nothing: they go behind every filtering join
     std::stable_partition(ord.begin(), ord.end(), [&](int j) { return h.joins[j].kind != srd::FRAG_OUTER; });
     srd::FragJoinDev reordered[SR_MAX_FRAG_JOINS];
+    srd::CExpr reordered_conj[SR_MAX_FRAG_JOINS];
+    int32_t conj_mask = 0;
     std::vector<int> inv(f->num_joins);
     for (int q = 0; q < f->num_joins; q++) {
         reordered[q] = h.joins[ord[q]];
+        reordered_conj[q] = h.conj[ord[q]];
+        conj_mask |= ((h.conj_mask >> ord[q]) & 1) << q;
         inv[ord[q]] = q;
         f->order[q] = ord[q];
     }
-    for (int q = 0; q < f->num_joins; q++) h.joins[q] = reordered[q];
+    for (int q = 0; q < f->num_joins; q++) {
+        h.joins[q] = reordered[q];
+        h.conj[q] = reordered_conj[q];
+    }
+    h.conj_mask = conj_mask;
     for (size_t k = 0; k < f->value_src.size(); k++)
         if (f->value_src[k] >= 0) f->value_src[k] = inv[f->value_src[k]];
     // stream the second join's key together with the first when most of its 64-byte DRAM bursts would
@@ -660,7 +744,8 @@ static int32_t frag_plan(sr_fragment* f, const VTab& vt, int64_t n) {
     double total_rate = f->pred_rate;
     for (int q = 0; q < f->num_joins; q++) total_rate *= f->pass_rate[ord[q]];
     f->est_rate = total_rate;
-    f->selective = f->expand || f->force_mode == 2 || (f->force_mode == 0 && total_rate < 0.25 && n >= (1 << 16));
+    // (the cascade neither expands a row nor evaluates an other-join conjunct)
+    f->selective = f->expand || f->conj || f->force_mode == 2 || (f->force_mode == 0 && total_rate < 0.25 && n >= (1 << 16));
     f->smem_agg = f->agg->smem_bytes > 0;
     if (f->selective)
         SR_TRY(frag_plan_passes(f, (double)counts[srd::SAMPLE_PREDS_UPTO] / (double)std::max<int64_t>(sample, 1)));
@@ -675,7 +760,7 @@ static int32_t frag_plan(sr_fragment* f, const VTab& vt, int64_t n) {
 
 // The final pass of selective mode over the selection vector `in` (its entry count at `in_count`): k_frag_final_dense
 // when the push allows it, else the instantiation of k_frag_gather_agg that frag_final_kernel picks.  A hash aggregate is
-// neither dense nor kept in shared memory and has group keys, so it always runs k_frag_gather_agg<false, false, EXPAND>,
+// neither dense nor kept in shared memory and has group keys, so it always runs k_frag_gather_agg<false, false, EXPAND, CONJ>,
 // which appends the rows its table refuses to `fail_list` (counted at `fail_count`).
 static int32_t frag_launch_final(sr_fragment* f, const VTab& vt, const srd::SelEntry* in, const unsigned long long* in_count, srd::SelEntry* fail_list,
                                  unsigned long long* fail_count) {
@@ -823,23 +908,19 @@ static int32_t frag_push(sr_fragment* f, const sr_chunk_view* fact) {
     return agg_push_rows(a, vt, n, launch);
 }
 
-// the fact slots the fragment reads: scan conjuncts, probe keys, group keys and aggregate inputs (a slot of the list the
-// fact chunk does not carry is a join payload)
+// the fact slots the fragment reads: scan conjuncts, probe keys, other-join conjuncts, group keys and aggregate inputs (a
+// slot of the list the fact chunk does not carry is a build column)
 static void frag_read_slots(const sr_fragment* f, std::vector<int32_t>* slots) {
     slots->clear();
-    const auto expr_slots = [&](const sr_expr& e) {
-        for (int k = 0; k < std::min<int32_t>(e.num_nodes, SR_MAX_EXPR_NODES); k++)
-            if (e.nodes[k].op == SR_EX_COL) slots->push_back(e.nodes[k].slot_id);
-    };
     for (const sr_pred& p : f->preds) slots->push_back(p.slot_id);
-    for (const sr_expr& e : f->exprs) expr_slots(e);
-    for (int j = 0; j < f->num_joins; j++) slots->push_back(f->joins[j].probe_key_slot);
-    const sr_agg_desc& d = f->agg->desc;
-    for (int k = 0; k < std::min<int32_t>(d.num_group_keys, SR_MAX_GROUP_KEYS); k++) slots->push_back(d.group_slots[k]);
-    for (int q = 0; q < std::min<int32_t>(d.num_fns, SR_MAX_AGG_FNS); q++) {
-        if (d.fns[q].kind != SR_AGG_COUNT_STAR) expr_slots(d.fns[q].input);
-        if (d.fns[q].kind == SR_AGG_AVG_MERGE) slots->push_back(d.fns[q].reserved);
+    for (const sr_expr& e : f->exprs) expr_slots(e, slots);
+    for (int j = 0; j < f->num_joins; j++) {
+        slots->push_back(f->joins[j].probe_key_slot);
+        expr_slots(f->joins[j].join->desc.other_conjunct, slots);
     }
+    std::vector<int32_t> agg;
+    frag_agg_slots(f->agg->desc, &agg);
+    slots->insert(slots->end(), agg.begin(), agg.end());
 }
 
 // sr_fragment_push_chunks: validate the whole list, gather the columns the fragment reads into one device batch (one

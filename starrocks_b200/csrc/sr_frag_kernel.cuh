@@ -41,6 +41,11 @@ struct FragDev {
     CExpr exprs[4];
     FragJoinDev joins[SR_MAX_FRAG_JOINS];
     unsigned long long* rows_passed;
+    // other-join conjuncts of INNER / LEFT SEMI joins, by probe position: bit j of conj_mask says conj[j] is join j's.  Only
+    // the final pass reads them (k_frag_gather_agg<..., CONJ = true>)
+    int32_t conj_mask;
+    int32_t pad2;
+    CExpr conj[SR_MAX_FRAG_JOINS];
 };
 
 // k_frag_sample's counters: [j] rows passing join j, [SAMPLE_ALL_PREDS] rows passing every scan conjunct,
@@ -494,7 +499,9 @@ __global__ void __launch_bounds__(FRAG_BLOCK, 2) k_fragment(const FragDev* __res
     if (lane_id() == 0 && passed) atomicAdd(fd.rows_passed, passed);
 }
 
-// adaptive join ordering: independent pass counts of each join on a sample of rows
+// adaptive join ordering: independent pass counts of each join on a sample of rows.  A join's other-join conjunct is not
+// evaluated here, so its sampled pass rate is that of the key test alone: an overestimate, which orders the join later than
+// it might go and sizes a hash aggregate's table for more survivors than arrive (the safe side)
 __global__ void __launch_bounds__(256) k_frag_sample(const FragDev* __restrict__ fdp, const __grid_constant__ VTab vt, int64_t n,
                                                       unsigned long long* __restrict__ counts) {
     const FragDev& fd = *fdp;

@@ -505,15 +505,51 @@ __global__ void __launch_bounds__(GATHER_BLOCK) k_frag_gather_join(const FragDev
 // the final pass is a chain of dependent gathers per row: latency bound, so resident warps matter more than spills.
 // Five CTAs per SM (48 registers) balance resident warps against spills.
 constexpr int GATHER_AGG_MIN_BLOCKS = 5;
+// (The CONJ instantiations spill 72-504 B under this cap.  Three CTAs per SM remove every spill but made the Q95 ws_wh
+// leg slower on H100, 1229 against 1023 ms: tools/frag_conjuncts.py, DESIGN.md section 6.)
+
+// the first entry of join j's build chain, from ld.bidx[j] on, that makes the join's other-join conjunct TRUE (NULL counts
+// as false).  Leaves ld.bidx[j] on it and returns whether there is one.
+__device__ __forceinline__ bool frag_conj_seek(const FragDev& fd, const FragJoinDev& fj, int j, FragLoader& ld) {
+#pragma unroll 1
+    for (uint32_t b = ld.bidx[j]; b != 0; b = fj.j.has_dup ? __ldg(fj.j.next + b) : 0u) {
+        ld.bidx[j] = b;
+        int64_t bits;
+        if (!eval_expr(fd.conj[j], ld, bits) && bits != 0) return true;
+    }
+    return false;
+}
+
+// The other-join conjuncts of a row that passed frag_final_joins.  A LEFT SEMI join passes the row when some entry of its
+// chain makes its conjunct TRUE; an INNER join with unique keys when its one build row does; an expanding INNER join when
+// some entry does, and that first entry becomes the head its odometer starts from and returns to (frag_next_combination
+// then skips the entries that fail).  Each conjunct reads only fact values and its own join's build row, so the passing
+// combinations are exactly the product of each join's passing entries.
+template <bool EXPAND>
+__device__ __forceinline__ bool frag_final_conjuncts(const FragDev& fd, const FragJoinDev* joins, int S, FragLoader& ld, uint32_t* head) {
+    const int32_t mask = fd.conj_mask;
+#pragma unroll 1
+    for (int j = 0; j < S; j++) {
+        if (!((mask >> j) & 1)) continue;
+        if (!frag_conj_seek(fd, joins[j], j, ld)) return false;
+        if (EXPAND) head[j] = ld.bidx[j];
+    }
+    return true;
+}
 
 // the next combination of chain entries of a row's expanding joins, like an odometer: advance the last expanding join,
-// carry into the one before it when its chain ends.  False when every chain is back at its head.
-__device__ __forceinline__ bool frag_next_combination(const FragJoinDev* joins, int S, FragLoader& ld, const uint32_t* head) {
+// carry into the one before it when its chain ends.  False when every chain is back at its head.  CONJ: a join with an
+// other-join conjunct advances to its next entry that makes the conjunct TRUE.
+template <bool CONJ>
+__device__ __forceinline__ bool frag_next_combination(const FragDev& fd, const FragJoinDev* joins, int S, FragLoader& ld, const uint32_t* head) {
 #pragma unroll 1
     for (int j = S - 1; j >= 0; j--) {
         if (!joins[j].expand) continue;
         const uint32_t nx = __ldg(joins[j].j.next + ld.bidx[j]);
-        if (nx) {
+        if (CONJ && ((fd.conj_mask >> j) & 1)) {
+            ld.bidx[j] = nx;
+            if (frag_conj_seek(fd, joins[j], j, ld)) return true;
+        } else if (nx) {
             ld.bidx[j] = nx;
             return true;
         }
@@ -529,7 +565,9 @@ __device__ __forceinline__ bool frag_next_combination(const FragJoinDev* joins, 
 // key).  The probe output is never materialised: the thread that owns a surviving fact row walks the chains of its
 // expanding joins like an odometer (last join fastest) and applies the aggregate once per combination, reading the
 // payload columns at the current chain entries, into global accumulators.
-template <bool SMEM_AGG, bool SINGLE, bool EXPAND>
+// CONJ: some join has an other-join conjunct (frag_final_conjuncts); only the combinations that pass them are applied and
+// counted, by both walks of the hash-table path.
+template <bool SMEM_AGG, bool SINGLE, bool EXPAND, bool CONJ>
 __global__ void __launch_bounds__(GATHER_BLOCK, GATHER_AGG_MIN_BLOCKS) k_frag_gather_agg(const FragDev* __restrict__ fdp, const AggDev* __restrict__ adp, const __grid_constant__ PassDev pd,
                                                                    const __grid_constant__ VTab vt, const SelEntry* __restrict__ sel_in,
                                                                    const unsigned long long* __restrict__ n_in_ptr, SelEntry* __restrict__ fail_list,
@@ -575,6 +613,7 @@ __global__ void __launch_bounds__(GATHER_BLOCK, GATHER_AGG_MIN_BLOCKS) k_frag_ga
         FragLoader ld{vt, (int64_t)row, {0, 0, 0, 0, 0, 0}, pd.carry_join >= 0 ? (int32_t)pd.carry_value_id : -1, sel_carry(entry)};
         uint32_t head[EXPAND ? SR_MAX_FRAG_JOINS : 1];
         if (!frag_final_joins(s_joins, S, pd.final_first_join, ld, EXPAND ? head : nullptr)) continue;
+        if (CONJ && !frag_final_conjuncts<EXPAND>(fd, s_joins, S, ld, head)) continue;
         auto hash_slot = [&]() {
             HKey key;
             agg_pack_key(ad, ld, key);
@@ -589,7 +628,7 @@ __global__ void __launch_bounds__(GATHER_BLOCK, GATHER_AGG_MIN_BLOCKS) k_frag_ga
             bool refused = false;
             do {
                 refused = hash_slot() < 0;
-            } while (!refused && frag_next_combination(s_joins, S, ld, head));
+            } while (!refused && frag_next_combination<CONJ>(fd, s_joins, S, ld, head));
             if (refused) {
                 if (fail_list) fail_list[atomicAdd(fail_count, 1ull)] = entry;
                 continue;
@@ -612,7 +651,7 @@ __global__ void __launch_bounds__(GATHER_BLOCK, GATHER_AGG_MIN_BLOCKS) k_frag_ga
                 if (slot >= 0) agg_apply_row<SMEM_AGG>(ad, acc, slot, ld);
             }
             passed++;
-            if (!EXPAND || !frag_next_combination(s_joins, S, ld, head)) break;
+            if (!EXPAND || !frag_next_combination<CONJ>(fd, s_joins, S, ld, head)) break;
         }
     }
     __syncwarp();

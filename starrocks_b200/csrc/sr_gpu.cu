@@ -1193,7 +1193,7 @@ sr_fragment* sr_fragment_create(sr_ctx* ctx, const sr_fragment_desc* desc) {
             sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "fused fragment supports INNER / LEFT SEMI / LEFT ANTI / LEFT OUTER joins (join %d is type %d)", j, jt);
             return nullptr;
         }
-        if (fj.join->desc.other_conjunct.num_nodes > 0) {
+        if (fj.join->desc.other_conjunct.num_nodes > 0 && jt != SR_JOIN_INNER && jt != SR_JOIN_LEFT_SEMI) {
             sr_fail(ctx, SR_ERR_NOT_SUPPORTED, "fused fragment: join %d has an other-join conjunct; use the per-operator path", j);
             return nullptr;
         }
@@ -1256,6 +1256,29 @@ sr_fragment* sr_fragment_create(sr_ctx* ctx, const sr_fragment_desc* desc) {
         // expands
         const int32_t jt = desc->joins[j].join->desc.join_type;
         if (desc->joins[j].join->has_dup && (jt == SR_JOIN_INNER || jt == SR_JOIN_LEFT_OUTER)) f->expand = true;
+        // an other-join conjunct: always the selection-vector passes, whose final pass evaluates it.  Over a build side that
+        // never received a chunk, each slot the conjunct reads that sr_join_desc.build_out_types declares gets a zeroed row
+        // of that type (the others must be fact columns, which frag_compile checks on the first push)
+        const sr_expr& conj = desc->joins[j].join->desc.other_conjunct;
+        if (conj.num_nodes > 0) f->conj = true;
+        if (conj.num_nodes > 0 && desc->joins[j].join->cols.empty()) {
+            for (int k = 0; k < std::min<int32_t>(conj.num_nodes, SR_MAX_EXPR_NODES); k++) {
+                const int32_t slot = conj.nodes[k].slot_id, type = join_declared_out_type(desc->joins[j].join, slot);
+                bool payload = false; // its own payload has a zeroed column already
+                for (int p = 0; p < desc->joins[j].num_payload; p++) payload |= desc->joins[j].payload_build_slots[p] == slot;
+                if (conj.nodes[k].op != SR_EX_COL || type == 0 || payload) continue;
+                f->empty_conj[j].push_back(std::make_unique<BuildCol>());
+                BuildCol& bc = *f->empty_conj[j].back();
+                bc.slot = slot;
+                bc.type = type;
+                bc.width = srd::type_width(type);
+                if (bc.data.reserve(ctx, 16) != SR_OK || cudaMemsetAsync(bc.data.p, 0, 16, ctx->stream) != cudaSuccess) {
+                    sr_fail(ctx, SR_ERR_CUDA, "fragment join %d: zeroed conjunct column", j);
+                    delete f;
+                    return nullptr;
+                }
+            }
+        }
     }
     f->agg = new sr_agg();
     f->agg->ctx = ctx;

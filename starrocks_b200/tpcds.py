@@ -163,6 +163,49 @@ def q95_descs():
     return d
 
 
+WR_ORDER = 40                        # web_returns' order number as a build key
+
+
+def fused_conj_descs():
+    """The self join with wh1 <> wh2 as its other-join conjunct, in the two shapes the fused fragment runs:
+      ws_wh  web_sales ws1 JOIN web_sales ws2 ON order AND wh1 <> wh2, GROUP BY ws1.ws_order_number (Q95's CTE);
+      q94    the Q94 body: ship date BETWEEN, LEFT SEMI date / address / site, EXISTS (ws2: same order, other warehouse)
+             as a LEFT SEMI self join with the conjunct, NOT EXISTS web_returns as a LEFT ANTI join, then COUNT(*),
+             SUM(ws_ext_ship_cost), SUM(ws_net_profit).
+    -> {name: join descriptor or (scan, agg) descriptors}; the self joins' build side is web_sales as (WS2_ORDER, WS2_WH)"""
+    wh_differs = [("col", WS_WH), ("col", WS2_WH), "!="]
+    d = {}
+    d["ws_wh_join"] = abi.make_join_desc(abi.JOIN_INNER, [WS2_ORDER], [WS_ORDER], [abi.TYPE_BIGINT], probe_out=[WS_ORDER], other_conjunct=wh_differs)
+    d["ws_wh_agg"] = lambda expected: abi.make_agg_desc([WS_ORDER], [abi.TYPE_BIGINT], expected_groups=expected)
+    body = [WS_ORDER, WS_WH, WS_COST, WS_PROFIT]
+    d["q94_scan"] = abi.ScanDesc(preds=[abi.make_pred(WS_SHIP_DATE, abi.PRED_BETWEEN, DATE_LO, DATE_LO + 60)], out_slots=[WS_SHIP_DATE, WS_ADDR, WS_SITE] + body)
+    d["q94_semi_date"] = abi.make_join_desc(abi.JOIN_LEFT_SEMI, [D_DATE_SK], [WS_SHIP_DATE], [abi.TYPE_INT], probe_out=[WS_ADDR, WS_SITE] + body)
+    d["q94_semi_addr"] = abi.make_join_desc(abi.JOIN_LEFT_SEMI, [CA_ADDRESS_SK], [WS_ADDR], [abi.TYPE_INT], probe_out=[WS_SITE] + body)
+    d["q94_semi_site"] = abi.make_join_desc(abi.JOIN_LEFT_SEMI, [WEB_SITE_SK], [WS_SITE], [abi.TYPE_INT], probe_out=body)
+    d["q94_exists"] = abi.make_join_desc(abi.JOIN_LEFT_SEMI, [WS2_ORDER], [WS_ORDER], [abi.TYPE_BIGINT], probe_out=body, other_conjunct=wh_differs)
+    d["q94_not_returned"] = abi.make_join_desc(abi.JOIN_LEFT_ANTI, [WR_ORDER], [WS_ORDER], [abi.TYPE_BIGINT], probe_out=[WS_COST, WS_PROFIT])
+    d["q94_agg"] = abi.make_agg_desc(fns=[(abi.AGG_COUNT_STAR, 0, OUT_DISTINCT, None), (abi.AGG_SUM, abi.TYPE_BIGINT, OUT_COST, [("col", WS_COST)]),
+                                          (abi.AGG_SUM, abi.TYPE_BIGINT, OUT_PROFIT, [("col", WS_PROFIT)])])
+    return d
+
+
+def q94_expected(gen, lo, hi):
+    """the q94 body of fused_conj_descs over the generator functions, join-free, for the orders [lo, hi) -> (count, cost,
+    profit); numpy generator only"""
+    ws = gen.web_sales_of_orders(lo, hi)
+    o = gen._arange(lo, hi)
+    rep, _ = gen._expand(gen.lines_per_order(o))
+    wh = ws["ws_warehouse_sk"]
+    mn = np.full(hi - lo, 1 << 30, dtype=np.int64)
+    mx = np.zeros(hi - lo, dtype=np.int64)
+    np.minimum.at(mn, rep, wh)
+    np.maximum.at(mx, rep, wh)
+    order_ok = (mn != mx) & (gen.returns_per_order(o) == 0)
+    d = ws["ws_ship_date_sk"]
+    ok = order_ok[rep] & (d >= DATE_LO) & (d <= DATE_LO + 60) & gen.address_ok(ws["ws_ship_addr_sk"].astype(np.int64)) & gen.site_ok(ws["ws_web_site_sk"])
+    return int(ok.sum()), int(ws["ws_ext_ship_cost"][ok].sum()), int(ws["ws_net_profit"][ok].sum())
+
+
 # ---------------------------------------------------------------------------------------------------------------------
 # engines: the same four verbs over the CUDA operators and over the oracle
 # ---------------------------------------------------------------------------------------------------------------------
